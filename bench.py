@@ -1,9 +1,16 @@
 #!/usr/bin/env python
 """
-bench.py -- map_cells_to_space iterations/sec on B200 (BASELINE.json metric).
+bench.py -- map_cells_to_space iterations/sec on an H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c3|c2|c4|c5] [--precision bf16|fp32]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c3|c2|c4|c5] [--precision bf16|fp32] [--dump-outputs DIR]
     python bench.py --impl reference ...      # the reference's own CPU path (unmodified Mapper from oracle/_ref), full size
+
+--dump-outputs DIR writes what the timed steps computed, after the last one: DIR/loss_history.npy (every history row of
+the run, the columns of the loss terms the workload enables, float32) and DIR/mapping_rows.npy (softmax(M) on a fixed,
+seeded sample of cells, float32, at most 48 MB).
+The inputs are seeded, so two builds run with the same arguments can be compared output for output.  The comparison
+legs against the unmodified reference (reference_gpu, parity.vs_reference_gpu, cpu_baseline) need the copy
+oracle/build_ref.py makes; without it, or without room on the device, they are reported as {"skipped": <reason>}.
 
 A "step" is one optimizer iteration (loss, backward, Adam) of the hot path on synthetic
 expression-like inputs (SURVEY.md 8(d)).  N>1: launched by torchrun, one rank per GPU, the
@@ -26,8 +33,9 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {
     # name: (cells, voxels, genes, types, clusters-mode, description)
-    "c1": (26_431, 9_852, 249, 0, False,
-           "reference fixtures data/test_ad_sc.h5ad x data/test_ad_sp.h5ad (tests/golden/c1_reference.npz), mode=cells"),
+    "c1": (5_000, 9_852, 249, 0, False,
+           "a seeded 5000-cell sample of the reference fixtures data/test_ad_sc.h5ad (26431 cells) x data/test_ad_sp.h5ad "
+           "(tests/golden/c1_reference.npz), mode=cells"),
     "c2": (10_000, 1_000, 1_000, 0, False, "synthetic 10k cells x 1k voxels x 1k genes, mode=cells"),
     "c3": (100_000, 10_000, 2_000, 0, False, "synthetic 100k cells x 10k voxels x 2k genes, mode=cells"),
     "c4": (256, 50_000, 5_000, 0, True, "synthetic 256 clusters x 50k voxels x 5k genes, mode=clusters"),
@@ -35,9 +43,10 @@ WORKLOADS = {
            "synthetic 50k cells x 5k voxels x 2k genes, neighbourhood + ct-islands + Getis-Ord on"),
     "tiny": (300, 80, 50, 0, False, "synthetic 300 cells x 80 voxels x 50 genes (smoke test of the bench arms themselves)"),
 }
+FP32_TFLOPS = 67.0      # H100 SXM data sheet, FP32 (non-tensor)
 C5_LAMBDAS = dict(lambda_neighborhood_g1=0.96, lambda_ct_islands=0.17, lambda_getis_ord=0.71,
                   lambda_r=2.95e-9, lambda_l2=1e-18)
-L2_BYTES = 126e6
+L2_BYTES = 50e6          # H100 L2
 
 
 def shard_rows_for(n_cells, rank, world):
@@ -51,7 +60,7 @@ def peaks():
         j = json.load(open(p))
         return dict(hbm=j["hbm_gbs"], tf_burst=j["bf16_tflops"], tf_sust=j.get("bf16_tflops_sustained", j["bf16_tflops"]),
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet (dense BF16, 700 W), not measured")
 
 
 def gen_inputs(name, r0, r1, seed=0):
@@ -90,7 +99,7 @@ def gen_inputs(name, r0, r1, seed=0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -209,29 +218,39 @@ def reference_cpu_sample(name, target_seconds=15.0):
     t0 = time.perf_counter()
     mp.train(num_epochs=n, learning_rate=0.1, print_each=None)
     dt = (time.perf_counter() - t0) / n
-    return dict(value=1.0 / (dt * N / n_s), unit="iterations/s", cores=threads, kind="reference",
+    return dict(value=1.0 / (dt * N / n_s), unit="iterations/s", cores=threads, kind="reference", source=build_ref.source(),
                 sample=f"{n} epochs of the unmodified reference Mapper (oracle/_ref, device='cpu', {threads} threads) on "
                        f"cells[0:{n_s}] x {V} voxels x {K} genes: {dt * 1e3:.1f} ms/epoch on the sample; value = that rate "
                        f"scaled by {n_s}/{N} (work is linear in cells).  The full-size measurement is `bench.py --impl reference`.")
 
 
-def load_traffic():
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the kernels, from the committed
-    `ncu --set full` capture of this round: profiles/traffic.json is written by tools/ncu_traffic.py from the raw csv."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return json.load(open(p))
-    except (OSError, ValueError):
-        return {}
-
-
 def expected_losses(key):
-    """Loss trajectory of the default run recorded by an earlier single-GPU run (tests/golden/bench_expected.json);
+    """Loss trajectory of the default run recorded by an earlier single-GPU run on an H100 (tests/golden/bench_expected.json);
     the seeded inputs and the sharding-independent device RNG make it the same computation at every N."""
     try:
         return json.load(open(os.path.join(ROOT, "tests", "golden", "bench_expected.json"))).get(key)
     except (OSError, ValueError):
         return None
+
+
+def dump_outputs(out_dir, eng, n_rows, V, cap_bytes=48e6):
+    """What a caller of the timed path receives after its last step: the loss history (tgb200_get_history) and softmax(M)
+    (tgb200_get_mapping), the latter on a fixed, seeded sample of rows so that the files stay small.  The history keeps the
+    columns of the terms this configuration computes: a disabled term's column is NaN by contract (k_loss_scalars)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    c = eng.cfg
+    terms = [True, True, c.lambda_g2 != 0, c.density_mode != 0 and c.lambda_d != 0, c.lambda_r != 0, c.lambda_l1 != 0,
+             c.lambda_l2 != 0, c.lambda_neighborhood_g1 > 0, c.lambda_ct_islands > 0, c.lambda_getis_ord > 0]
+    np.save(os.path.join(out_dir, "loss_history.npy"), eng.history()[:, np.flatnonzero(terms)].astype(np.float32))
+    k = int(min(n_rows, max(1, cap_bytes // (4 * V))))
+    rows = np.sort(np.random.default_rng(0).choice(n_rows, k, replace=False))
+    full = torch.empty((n_rows, V), dtype=torch.float32, device="cuda")
+    eng.get_mapping(full)
+    sample = full[torch.from_numpy(rows).cuda()].cpu().numpy()
+    del full
+    torch.cuda.empty_cache()
+    np.save(os.path.join(out_dir, "mapping_rows.npy"), sample)
 
 
 def timed_steps(one_step, barrier, steps, flush_buf):
@@ -270,7 +289,7 @@ def rel_fro_gpu(a, b, rows=8192):
 
 
 def reference_gpu_legs(a, inp, local, engine_factory, n_total):
-    """The PyTorch-GPU comparator (SURVEY 8(d)(ii)): the UNMODIFIED reference Mapper with device='cuda' on this B200, and
+    """The PyTorch-GPU comparator (SURVEY 8(d)(ii)): the UNMODIFIED reference Mapper with device='cuda' on this GPU, and
     -- from the very same initial mapping (the reference's own seed-42 draw, taken from its device tensor) -- our bf16 and
     bf16x3 paths for the same number of epochs: loss-trajectory and final-mapping parity at the benchmark size."""
     import torch
@@ -324,6 +343,7 @@ def reference_gpu_legs(a, inp, local, engine_factory, n_total):
                         "mapping_rel_fro": rel_fro_gpu(o["out"], ref_out)}
     parity["reference_loss_first"], parity["reference_loss_last"] = float(ref_loss[0]), float(ref_loss[-1])
     refgpu = {"value": a.steps / dt, "unit": "iterations/s", "ms_per_step": dt / a.steps * 1e3, "steps": a.steps,
+              "source": build_ref.source(),
               "warmup": n_total, "init_s": init_s, "first_call_s": first_s,
               "what": "unmodified reference Mapper (oracle/_ref/mapping_optimizer.py) with device='cuda': fp32 cuBLAS SGEMM "
                       "(TF32 off), autograd, torch.optim.Adam, per-epoch .tolist() syncs; init_s includes its host-side "
@@ -347,6 +367,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-refgpu", action="store_true", help="skip the PyTorch-GPU comparator and the parity legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
 
@@ -373,7 +394,8 @@ def main():
                   f"init {r['init_s']:.1f} s; --steps {a.steps} --warmup {a.warmup} were requested and bounded to keep the run within minutes")
         if r["note"]:
             sample += "; " + r["note"]
-        cb = dict(value=value, unit="iterations/s", cores=r["threads"], kind="reference", sample=sample)
+        from oracle import build_ref
+        cb = dict(value=value, unit="iterations/s", cores=r["threads"], kind="reference", sample=sample, source=build_ref.source())
         line = {"impl": "reference", "metric": metric, "value": value, "unit": "iterations/s", "n_gpus": a.gpus,
                 "steps": r["steps"], "warmup": r["warmup"], "steps_requested": a.steps, "warmup_requested": a.warmup,
                 "ms_per_step": r["seconds"] / r["steps"] * 1e3, "higher_is_better": True,
@@ -383,7 +405,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ our arm (B200)
+    # ------------------------------------------------------------------ our arm (GPU)
     import torch
     import torch.distributed as dist
     from tangram_b200 import _lib
@@ -453,6 +475,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     elapsed = float(t.item())
     value = a.steps / elapsed
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, eng, r1 - r0, V)
 
     # ---------------- parity of this very run: the loss before the first and the last update against the recorded trajectory
     n_total = a.warmup + a.steps
@@ -466,6 +490,8 @@ def main():
     if exp and len(exp["total_loss"]) >= n_total:
         parity["expected_first"], parity["expected_last"] = exp["total_loss"][0], exp["total_loss"][n_total - 1]
         parity["max_abs_diff_vs_expected"] = float(np.max(np.abs(hist[:, 0].astype(np.float64) - np.array(exp["total_loss"][:n_total]))))
+    else:
+        parity["expected"] = f"no recorded trajectory of {n_total} epochs under {key}"
     if os.environ.get("TGB200_RECORD_EXPECTED") and rank == 0 and world == 1:
         parity["recorded_trajectory"] = [float(x) for x in hist[:, 0]]
 
@@ -504,12 +530,11 @@ def main():
         if known:
             top = max(known, key=known.get)
         key_k = next((k for k in work if k in top), None)
-        traffic = load_traffic().get(f"{a.workload}/{a.precision}", {})
         if key_k:
             fl, by = work[key_k]
             t_s = avg[top] / 1e3
-            # bf16x3 issues 6 bf16 MMAs per useful product; fp32 FFMA peak: 148 SM x 128 lanes x 2 x 1.965 GHz
-            tf_peak = pk["tf_sust"] if a.precision == "bf16" else (pk["tf_sust"] / 6.0 if a.precision == "bf16x3" else 74.0)
+            # bf16x3 issues 6 bf16 MMAs per useful product; fp32 FFMA peak (H100 SXM data sheet)
+            tf_peak = pk["tf_sust"] if a.precision == "bf16" else (pk["tf_sust"] / 6.0 if a.precision == "bf16x3" else FP32_TFLOPS)
             t_fl = fl / (tf_peak * 1e12) if fl else 0.0
             t_by = by / (pk["hbm"] * 1e9)
             if t_fl >= t_by:
@@ -519,7 +544,6 @@ def main():
                 roof = {"bound": "hbm", "achieved": by / t_s / 1e9, "peak": pk["hbm"], "unit": "GB/s"}
             roof["frac"] = roof["achieved"] / roof["peak"]
             roof.update({"kernel": top, "kernel_ms": avg[top], "share_of_step": avg[top] / step_ms,
-                         "traffic": traffic.get(key_k), "traffic_source": "profiles/traffic.json" if traffic.get(key_k) else None,
                          "peak_source": pk["src"], "per_kernel_ms": avg})
             # the contraction kernels against the tensor roofline (explains the step)
             others = {}
@@ -531,7 +555,7 @@ def main():
                                      "hbm_GBs": work[kk][1] / (ms / 1e3) / 1e9}
             roof["contractions"] = others
         hb, fl_it = eng.algorithmic_cost()
-        roof_step = max(hb / (pk["hbm"] * 1e9), fl_it / ({"bf16": pk["tf_sust"], "bf16x3": pk["tf_sust"] / 6.0}.get(a.precision, 74.0) * 1e12))
+        roof_step = max(hb / (pk["hbm"] * 1e9), fl_it / ({"bf16": pk["tf_sust"], "bf16x3": pk["tf_sust"] / 6.0}.get(a.precision, FP32_TFLOPS) * 1e12))
         if roof is not None:
             roof["step_roofline_frac"] = roof_step / (elapsed / a.steps)
             roof["sum_kernel_ms"] = step_ms
@@ -585,14 +609,27 @@ def main():
         del M0, Sp
 
     # ---------------- reference legs (rank 0, single GPU): PyTorch-GPU comparator + parity at the benchmark size, CPU sample
+    # Every reference leg is either run or reported as skipped with the reason (single GPU, rank 0 only).
+    from oracle import build_ref
+    no_ref = None if build_ref.source() else ("no copy of the reference (oracle/build_ref.py found no Tangram checkout "
+                                              "next to this repository or in TANGRAM_REFERENCE)")
     refgpu = x3 = None
-    if rank == 0 and world == 1 and not a.no_refgpu:
-        torch.cuda.empty_cache()
-        refgpu, par_ref, x3 = reference_gpu_legs(a, inp, local, make_engine, n_total)
-        parity["vs_reference_gpu"] = par_ref
     cpu = None
-    if rank == 0 and world == 1 and not a.no_cpu:
-        cpu = reference_cpu_sample(a.workload)
+    if rank == 0 and world == 1:
+        torch.cuda.empty_cache()
+        # device peak of the legs, estimated: the reference's autograd (~13 N x V fp32 buffers) while our engines run one after
+        # the other beside its resident M; at C3 (52 GB) the legs run on an 80 GB H100
+        need, free = 13.0 * 4 * N * V, torch.cuda.mem_get_info(local)[0]
+        skip = ("--no-refgpu" if a.no_refgpu else no_ref) or (
+            None if need < free else f"needs ~{need / 1e9:.0f} GB of device memory, {free / 1e9:.0f} GB free")
+        if skip:
+            refgpu = x3 = {"skipped": skip}
+            parity["vs_reference_gpu"] = {"skipped": skip}
+        else:
+            refgpu, par_ref, x3 = reference_gpu_legs(a, inp, local, make_engine, n_total)
+            parity["vs_reference_gpu"] = par_ref
+        skip = "--no-cpu" if a.no_cpu else no_ref
+        cpu = {"skipped": skip} if skip else reference_cpu_sample(a.workload)
 
     if rank == 0:
         line = {"metric": metric, "value": value, "unit": "iterations/s", "n_gpus": world, "steps": a.steps,
@@ -608,7 +645,7 @@ def main():
                                              "lives in ncclMemAlloc memory registered with the communicator (NVLS in-switch reduction on user buffers)"}
                                if world > 1 else None),
                 "parity": parity, "reference_gpu": refgpu,
-                "vs_reference_gpu": (value / refgpu["value"]) if refgpu else None, "bf16x3": x3}
+                "vs_reference_gpu": (value / refgpu["value"]) if refgpu and "value" in refgpu else None, "bf16x3": x3}
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * tangram_b200 -- C-ABI of the B200-native `map_cells_to_space` hot path.
+ * tangram_b200 -- C-ABI of the H100-native (sm_90a) `map_cells_to_space` hot path.
  *
  * This is the drop-in boundary for ONE path of broadinstitute/Tangram: the optimizer in
  * tangram/mapping_optimizer.py (class Mapper).  Each entry point cites the reference
@@ -38,13 +38,13 @@ typedef enum tgb200_status {
   TGB200_ERR_CUDA = -2,      /* CUDA runtime / driver error (message has the detail)   */
   TGB200_ERR_STATE = -3,     /* call order violated (e.g. run before set_expression)   */
   TGB200_ERR_UNSUPPORTED = -4, /* term outside the hot-path scope (Moran / Geary)      */
-  TGB200_ERR_NO_DEVICE = -5  /* no sm_100 device: there is NO CPU fallback             */
+  TGB200_ERR_NO_DEVICE = -5  /* no sm_90 device: there is NO CPU fallback              */
 } tgb200_status;
 
 /* Arithmetic of the two contractions (softmax(M)^T S and S dY^T). */
 typedef enum tgb200_precision {
   TGB200_PREC_FP32 = 0,  /* fp32 FFMA contraction: parity mode (reference is fp32, TF32 off) */
-  TGB200_PREC_BF16 = 1,  /* bf16 operands on tcgen05 tensor cores, fp32 accumulate in TMEM   */
+  TGB200_PREC_BF16 = 1,  /* bf16 operands on wgmma tensor cores, fp32 accumulate in registers */
   TGB200_PREC_BF16X3 = 2 /* parity mode on tensor cores: each fp32 operand = 3 bf16 planes, 6 partial products */
 } tgb200_precision;
 

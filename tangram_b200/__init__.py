@@ -1,4 +1,4 @@
-"""tangram_b200: B200-native drop-in for Tangram's map_cells_to_space hot path.
+"""tangram_b200: H100-native drop-in for Tangram's map_cells_to_space hot path.
 
     import tangram_b200 as tg
     tg.pp_adatas(ad_sc, ad_sp); ad_map = tg.map_cells_to_space(ad_sc, ad_sp, device="cuda:0")

@@ -1,7 +1,6 @@
-"""Builds the sm_100a C-ABI library in-tree (tangram_b200/libtangram_b200.so) with nvcc.
+"""Builds the sm_90a (H100) C-ABI library in-tree (tangram_b200/libtangram_b200.so) with nvcc.
 
-nvcc cross-compiles without a GPU; the built .so travels to the GPU box with the repo
-snapshot (it is git-ignored, not gpurun-ignored)."""
+nvcc cross-compiles without a GPU; the built library is git-ignored."""
 import hashlib
 import os
 import shutil
@@ -13,7 +12,7 @@ LIB = os.path.join(PKG, "libtangram_b200.so")
 STAMP = LIB + ".stamp"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared",
 ]
 

@@ -1,5 +1,5 @@
 """ctypes binding of include/tangram_b200.h.  There is NO CPU fallback: if the library is
-missing or no sm_100 GPU is visible the calls raise."""
+missing or no sm_90 GPU is visible the calls raise."""
 import ctypes
 import os
 

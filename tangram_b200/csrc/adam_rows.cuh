@@ -6,8 +6,8 @@
 //   Pt_ij  = exp(Mnew_ij - lse_i)  (bf16) and zt_i = sum_j Pt_ij      (the next forward's operand, see k_row_norm)
 //
 // Pure HBM streaming: 12 B/element in (M 4, m 2, v 4, dq 2), 12 B/element out (M 4, m 2, v 4, Pt 2).  One warp owns a row, so the row sums
-// need no partial arrays and are deterministic; every lane moves full 32-byte sectors (LDG.256 / STG.256), 8 columns per
-// lane and iteration, two iterations in flight.
+// need no partial arrays and are deterministic; every lane moves full 32-byte sectors (two 16-byte accesses), 8 columns
+// per lane and iteration, two iterations in flight.
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.cuh"
@@ -25,12 +25,15 @@ struct AdamRowsArgs {
   AdamScalars a;
 };
 
+// 8 floats = one 32-byte sector as two 16-byte streaming (evict-first) accesses
 __device__ __forceinline__ void ldg256f(const float* src, float (&x)[8]) {
-  asm volatile("ld.global.L1::no_allocate.L2::evict_first.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.cs.v4.f32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.cs.v4.f32 {%4,%5,%6,%7}, [%8+16];"
                : "=f"(x[0]), "=f"(x[1]), "=f"(x[2]), "=f"(x[3]), "=f"(x[4]), "=f"(x[5]), "=f"(x[6]), "=f"(x[7]) : "l"(src));
 }
 __device__ __forceinline__ void stg256f(float* dst, const float (&x)[8]) {
-  asm volatile("st.global.L1::no_allocate.L2::evict_first.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
+  asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};\n\t"
+               "st.global.cs.v4.f32 [%0+16], {%5,%6,%7,%8};"
                ::"l"(dst), "f"(x[0]), "f"(x[1]), "f"(x[2]), "f"(x[3]), "f"(x[4]), "f"(x[5]), "f"(x[6]), "f"(x[7]) : "memory");
 }
 __device__ __forceinline__ uint4 ldg128_stream(const void* src) {
@@ -59,9 +62,9 @@ __device__ __forceinline__ uint4 pack_bf8(const float (&f)[8]) {
   return o;
 }
 
-// PLAIN: default loss (no entropy / L1 / L2) -> packed f32x2 arithmetic, 4 MUFU per element.
+// PLAIN: default loss (no entropy / L1 / L2) -> no per-element branches, 4 MUFU per element.
 #ifndef TGB_ADAM_MAXNREG
-#define TGB_ADAM_MAXNREG 96     // 2 CTAs of this kernel + one contraction CTA (192 threads) per SM: 2 x 24.5K + 13.8K registers
+#define TGB_ADAM_MAXNREG 96     // two 8-column groups of M, m, v, dq in flight per lane without spills; 2 CTAs of 256 threads per SM
 #endif
 template <bool PLAIN>
 __global__ void __maxnreg__(TGB_ADAM_MAXNREG)
@@ -76,11 +79,7 @@ k_adam_rows(const AdamRowsArgs p) {
   const __nv_bfloat16* dr = p.dq + base;
   __nv_bfloat16* pr = p.Pt + base;
 
-  // packed constants of the default-loss path (TcEpiAdam::pair has the derivation)
-  const f32x2 k_l2e = pk2(1.4426950408889634f, 1.4426950408889634f), k_nlse = pk2(-lse_l2e, -lse_l2e), k_nr = pk2(-rc.r, -rc.r);
-  const f32x2 k_omb1 = pk2(p.a.one_minus_beta1, p.a.one_minus_beta1), k_omb2 = pk2(p.a.one_minus_beta2, p.a.one_minus_beta2);
-  const f32x2 k_b2 = pk2(p.a.beta2, p.a.beta2), k_ibc = pk2(p.a.inv_bc2_sqrt, p.a.inv_bc2_sqrt), k_eps = pk2(p.a.eps, p.a.eps);
-  const f32x2 k_nstep = pk2(-p.a.step_size, -p.a.step_size);
+  const float k_nstep = -p.a.step_size;
 
   float zs = 0.f, pxs = 0.f, l1s = 0.f, l2s = 0.f;
 
@@ -112,25 +111,18 @@ k_adam_rows(const AdamRowsArgs p) {
     if (c + 8 <= p.V) {
       if (PLAIN) {
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const __nv_bfloat162 d2 = *reinterpret_cast<const __nv_bfloat162*>(&dw[e]);
-          f32x2 x = pk2(L.x[2 * e], L.x[2 * e + 1]), m = pk2(L.m[2 * e], L.m[2 * e + 1]), v = pk2(L.v[2 * e], L.v[2 * e + 1]);
-          f32x2 t = fma2(x, k_l2e, k_nlse);
-          float e0, e1;
-          upk2(t, e0, e1);
-          const f32x2 g = mul2(add2(pk2(__low2float(d2), __high2float(d2)), k_nr), pk2(fast_ex2(e0), fast_ex2(e1)));
-          m = fma2(add2(g, m ^ 0x8000000080000000ull), k_omb1, m);          // m + (g - m)(1-b1)
-          v = fma2(mul2(k_omb2, g), g, mul2(v, k_b2));
-          float s0, s1;
-          upk2(v, s0, s1);
-          const f32x2 den = fma2(pk2(fast_sqrt(s0), fast_sqrt(s1)), k_ibc, k_eps);
-          float d0, d1;
-          upk2(den, d0, d1);
-          x = fma2(mul2(k_nstep, m), pk2(fast_rcp(d0), fast_rcp(d1)), x);
-          t = fma2(x, k_l2e, k_nlse);
-          upk2(t, e0, e1);
-          pt[2 * e] = fast_ex2(e0); pt[2 * e + 1] = fast_ex2(e1);
-          upk2(x, L.x[2 * e], L.x[2 * e + 1]); upk2(m, L.m[2 * e], L.m[2 * e + 1]); upk2(v, L.v[2 * e], L.v[2 * e + 1]);
+        for (int e = 0; e < 8; ++e) {
+          const __nv_bfloat162 d2 = *reinterpret_cast<const __nv_bfloat162*>(&dw[e >> 1]);
+          const float dq = (e & 1) ? __high2float(d2) : __low2float(d2);
+          float& x = L.x[e];
+          float& m = L.m[e];
+          float& v = L.v[e];
+          const float g = (dq + -rc.r) * fast_ex2(fmaf(x, 1.4426950408889634f, -lse_l2e));
+          m = fmaf(g + -m, p.a.one_minus_beta1, m);                          // m + (g - m)(1-b1)
+          v = fmaf(p.a.one_minus_beta2 * g, g, v * p.a.beta2);
+          const float den = fmaf(fast_sqrt(v), p.a.inv_bc2_sqrt, p.a.eps);
+          x = fmaf(k_nstep * m, fast_rcp(den), x);
+          pt[e] = fast_ex2(fmaf(x, 1.4426950408889634f, -lse_l2e));
         }
         zs += ((pt[0] + pt[1]) + (pt[2] + pt[3])) + ((pt[4] + pt[5]) + (pt[6] + pt[7]));
       } else {

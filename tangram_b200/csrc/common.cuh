@@ -1,4 +1,4 @@
-// Shared device helpers for the tangram_b200 kernels (sm_100a only).
+// Shared device helpers for the tangram_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

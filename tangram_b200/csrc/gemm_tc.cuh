@@ -1,17 +1,16 @@
-// tcgen05 / TMA tensor-core contraction path (sm_100a): bf16 operands staged in shared memory by
-// TMA (128B swizzle), tcgen05.mma issued by one elected thread, fp32 accumulators in TMEM,
-// tcgen05.ld back to registers for the fused epilogues.
+// wgmma / TMA tensor-core contraction path (sm_90a): bf16 operands staged in shared memory by
+// TMA (128B swizzle), wgmma.mma_async issued by two consumer warpgroups, fp32 accumulators in
+// registers, fused epilogues straight from the accumulator fragments.
 //
 //   forward   Y_ext[z] = P[z]^T S_ext[z]        A = P  (MN-major), B = S_ext (MN-major), split over cells / cell chunks
-//   backward  dP = S_ext dY_ext^T  -> stored (bf16 centred / fp32) + row-dot partials in the epilogue (A, B K-major);
-//             from 2048 cells up on CTA pairs (k_gemm_tc_pair: tcgen05 cta_group::2, 256-row tiles, half of B per CTA).
+//   backward  dP = S_ext dY_ext^T  -> stored (bf16 centred / fp32) + row-dot partials in the epilogue (A, B K-major).
 //             The update itself is a streaming kernel (adam_rows.cuh).
 //
-// Persistent, warp-specialised kernel: one CTA per SM loops over output tiles.
-//   warp 0      TMA producer: keeps the operand ring full across tile boundaries
-//   warp 1      TMEM allocator + MMA issuer: two accumulator buffers in TMEM, so the MMAs of tile i+1
-//               run while the epilogue warps drain tile i
-//   warps 2..   epilogue (TMEM lane quarter = warp_id % 4)
+// Persistent, warp-specialised kernel: one CTA per SM loops over 128 x 256 output tiles.
+//   warpgroup 0     TMA producer (one thread): keeps the operand ring full across tile boundaries, so the loads of
+//                   tile i+1 run while the consumers drain tile i
+//   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the tile, m64n256k16 wgmma into 128 fp32 registers per
+//                   thread, then the epilogue on those registers
 #pragma once
 #include <cuda.h>
 #include <cstdio>
@@ -20,11 +19,12 @@
 
 namespace tgb {
 
-constexpr int TC_BM = 128;        // UMMA M (TMEM lanes)
+constexpr int TC_BM = 128;        // output rows per tile (two 64-row wgmma warpgroups)
 constexpr int TC_BK = 64;         // one 128-byte swizzle row of bf16 per k-block
-constexpr int TC_UMMA_K = 16;
-constexpr int TC_THREADS = 192;
-constexpr int TC_RDOT_BN = 256;
+constexpr int TC_MMA_K = 16;
+constexpr int TC_BN = 256;        // output columns per tile (wgmma N)
+constexpr int TC_THREADS = 384;   // producer warpgroup + two consumer warpgroups
+constexpr int TC_ACC = TC_BN / 2; // fp32 accumulator registers per consumer thread
 
 // ---- PTX wrappers ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -49,25 +49,11 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // L2 policy: operand tiles are re-read by many CTAs -> evict_last (CUTLASS TMA::CacheHintSm90::EVICT_LAST)
 constexpr uint64_t kPolicyEvictNormal = 0x1000000000000000ull;
 constexpr uint64_t kPolicyEvictLast = 0x14F0000000000000ull;
 constexpr uint64_t kPolicyEvictFirst = 0x12F0000000000000ull;
-// one full 32-byte sector per instruction (sm_100+: STG.256) -- 16-byte stores from a row-per-thread layout are partial-sector
-// writes, which cost L2 fill reads from DRAM
-__device__ __forceinline__ void stg256(void* dst, const uint32_t* w) {
-  asm volatile("st.global.cs.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-}
-// one full 32-byte sector per thread, read-only path (sm_100+: LDG.256)
-__device__ __forceinline__ void ldg256(const void* src, uint32_t (&w)[8]) {
-  asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(src));
-}
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, uint64_t policy) {
   asm volatile(
@@ -78,61 +64,71 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> f32
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread t = lane base + t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// register budget of the two roles (warpgroup-wide): 128 x 40 + 256 x 232 <= 64K registers
+__device__ __forceinline__ void setmaxnreg_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void setmaxnreg_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float (&d)[TC_ACC]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < TC_ACC; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// D (64 x 256, fp32, registers) (+)= A[smem] * B[smem], bf16 x bf16; TA / TB: operand stored MN-major (transposed)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+      "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+      "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+      "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+      "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+      "}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
+}
 // ---- descriptors ----------------------------------------------------------------------------
-// Shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): start>>4 [0,14),
-// LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64).
+// Shared-memory matrix descriptor (cute/arch/mma_sm90_desc.hpp GmmaDescriptor): start>>4 [0,14),
+// LBO>>4 [16,30), SBO>>4 [32,46), layout SWIZZLE_128B=1 [62,64).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor (InstrDescriptor): c=F32 [4,6)=1, a=BF16 [7,10)=1, b=BF16 [10,13)=1,
-// a_major [15], b_major [16] (1 = MN-major), N>>3 [17,23), M>>4 [24,29).
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // Operand tile in shared memory, one pipeline stage.
 //   K-major  (rows = MN index, 64 k-elements = 128 B per row):   ROWS x 128 B, SBO = 1024 B (8 rows)
 //   MN-major (rows = k index,  64 mn-elements = 128 B per row):  ROWS/64 boxes of [64 k][128 B];
 //            LBO = 8192 B (next 64-wide MN atom), SBO = 1024 B (next 8 k-rows)
+// Either way the 64-row half `h` of a tile starts 8192 B in.
 template <bool KMAJOR, int ROWS>
 struct OperandTile {
   static constexpr int kBytes = ROWS * TC_BK * 2;
@@ -145,16 +141,16 @@ struct OperandTile {
     }
   }
   static __device__ __forceinline__ uint64_t desc(uint32_t saddr, int k_step /* 0..3 */) {
-    if (KMAJOR) return make_smem_desc(saddr + k_step * (TC_UMMA_K * 2), 16, 1024);
-    return make_smem_desc(saddr + k_step * (TC_UMMA_K * 128), 8192, 1024);
+    if (KMAJOR) return make_smem_desc(saddr + k_step * (TC_MMA_K * 2), 16, 1024);
+    return make_smem_desc(saddr + k_step * (TC_MMA_K * 128), 8192, 1024);
   }
 };
 
 // ---- epilogues ------------------------------------------------------------------------------
-// Each epilogue warp owns TMEM lanes [32q, 32q+32) = output rows m0+32q.. of the tile.
-// run() is called once per warp after the accumulator is complete; `scratch` is the (now idle)
-// operand ring, 1024-byte aligned, at least 32 KB.
-// Coordinates of the work item an epilogue warp is draining.
+// run() gets one consumer thread's accumulator fragment of the m64n256 wgmma: for every 8-column group j, d[4j], d[4j+1]
+// are columns (8j + 2 (lane % 4), +1) of row `row`, and d[4j+2], d[4j+3] the same columns of row `row + 8`.  A quad of
+// lanes covers 8 consecutive columns of a row (one 32-byte sector of fp32).  prologue() is called by all 256 consumer
+// threads (`ct`) before the tile's main loop.
 // Work item w -> (row tile m, column tile n).  Row tiles are taken in groups of `group_m`; inside a group the order is
 // column-major (all rows of the group for column 0, then column 1, ...).  The CTAs running at the same time then cover
 // the whole group for a few columns: the group's A rows (group_m x 128 x K, re-read for every column) are a small,
@@ -173,32 +169,31 @@ struct TileCoord {
   int split;         // k-split index
 };
 
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
 struct TcEpiStore {
   float* C; int ldc; size_t split_stride; int M;
   int accumulate;        // 1: C += tile (cell chunks of the pipelined forward run one after the other: fixed summation order)
-  template <int BN, int NW>
-  __device__ __forceinline__ void prologue(const TileCoord&, int, int, int) const {}
-  __device__ __forceinline__ void finish(int, int, int) const {}
-  template <int BN, int NW>
-  __device__ __forceinline__ void run(uint32_t tmem_acc, int q, int, int lane, const TileCoord& t) const {
-    static_assert(NW == 4, "one warp per TMEM lane quarter");
-    const int row = t.m0 + q * 32 + lane;
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 16) {
-      float v[16];
-      tmem_ld16(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-      const int col = t.n0 + c;
-      if (row < M && col < ldc) {
-        float4* dst = reinterpret_cast<float4*>(C + (size_t)t.split * split_stride + (size_t)row * ldc + col);
-        if (accumulate) {
+  __device__ __forceinline__ void prologue(const TileCoord&, int) const {}
+  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane) const {
+    float* base = C + (size_t)t.split * split_stride;
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float4 o = dst[e];
-            v[4 * e] += o.x; v[4 * e + 1] += o.y; v[4 * e + 2] += o.z; v[4 * e + 3] += o.w;
-          }
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      if (r >= M) continue;
+#pragma unroll
+      for (int j = 0; j < TC_BN / 8; ++j) {
+        const int col = t.n0 + 8 * j + 2 * (lane & 3);
+        if (col < ldc) {
+          float2* dst = reinterpret_cast<float2*>(base + (size_t)r * ldc + col);
+          float2 v = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+          if (accumulate) { const float2 o = *dst; v.x += o.x; v.y += o.y; }
+          *dst = v;
         }
-#pragma unroll
-        for (int e = 0; e < 4; ++e) dst[e] = make_float4(v[4 * e], v[4 * e + 1], v[4 * e + 2], v[4 * e + 3]);
       }
     }
   }
@@ -208,61 +203,43 @@ struct TcEpiStore {
 // bf16, centred per row on the previous iteration's row-dot (dq_ij = bf16(dP_ij - c_i): the softmax-Jacobian only sees
 // dP_ij - r_i, so the bf16 rounding is relative to the deviation from the row mean, not to dP itself), and the same
 // epilogue accumulates this iteration's row-dot partials r'_i = sum_j Pt_ij dq_ij from the ROUNDED values (so that
-// sum_j g_ij = 0 holds for what the streaming Adam kernel consumes).  Thread = row (TMEM lane), one 32-byte sector of
-// Pt in and one of dq out per 16 columns; the Pt segment of the tile is prefetched into L2 before the wait on the MMAs.
+// sum_j g_ij = 0 holds for what the streaming Adam kernel consumes).  The Pt segment of the tile is prefetched into L2
+// before the main loop.
 struct TcEpiDpStore {
   __nv_bfloat16* dq; const __nv_bfloat16* Pt; int ld;     // both [rows][ld]
   const float* center;                                    // c_i (per row)
-  float* rpart;                                           // [tiles_n * (NW / 4)][M]
+  float* rpart;                                           // [tiles_n][M]
   int M;
-  // NW = 4: one warp per TMEM lane quarter takes all BN columns; NW = 8: two warps, BN / 2 columns each.  Four warps keep
-  // the CTA small (192 threads) so that two CTAs of the streaming Adam kernel fit next to it on the SM.
-  template <int BN, int NW>
-  __device__ __forceinline__ void prologue(const TileCoord& t, int q, int ew, int lane) const {
-    static_assert(NW == 4 || NW == 8, "one or two warps per TMEM lane quarter");
-    constexpr int W = BN / (NW / 4);
-    const int row = t.m0 + q * 32 + lane, col = t.n0 + (ew >> 2) * W;
-    if (row < M) {
-      const __nv_bfloat16* src = Pt + (size_t)row * ld + col;
+  __device__ __forceinline__ void prologue(const TileCoord& t, int ct) const {
 #pragma unroll
-      for (int b = 0; b < W; b += 64)           // 128-byte lines of this thread's row segment
-        if (col + b < ld) prefetch_l2(src + b);
+    for (int i = ct; i < TC_BM * (TC_BN / 64); i += 256) {      // 128-byte lines of the tile's Pt block
+      const int row = t.m0 + (i >> 2), col = t.n0 + (i & 3) * 64;
+      if (row < M && col < ld) prefetch_l2(Pt + (size_t)row * ld + col);
     }
   }
-  __device__ __forceinline__ void finish(int, int, int) const {}
-  template <int BN, int NW>
-  __device__ __forceinline__ void run(uint32_t tmem_acc, int q, int ew, int lane, const TileCoord& t) const {
-    constexpr int PARTS = NW / 4, W = BN / PARTS, NCH = W / 16;
-    const int part = ew >> 2;
-    const int row = t.m0 + q * 32 + lane;
-    const int cbase = t.n0 + part * W;
-    const bool live = row < M;
-    const float c = live ? center[row] : 0.f;
-    const __nv_bfloat16* prow = Pt + (size_t)row * ld;
-    __nv_bfloat16* drow = dq + (size_t)row * ld;
-    uint32_t pw[2][8];
-    if (live && cbase < ld) ldg256(prow + cbase, pw[0]);
-    float racc = 0.f;
+  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane) const {
 #pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-      const int col0 = cbase + i * 16;
-      if (i + 1 < NCH && live && col0 + 16 < ld) ldg256(prow + col0 + 16, pw[(i + 1) & 1]);
-      float v[16];
-      tmem_ld16(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(col0 - t.n0), v);
-      if (live && col0 < ld) {
-        uint32_t w[8];
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      const bool live = r < M;
+      const float c = live ? center[r] : 0.f;
+      const __nv_bfloat16* prow = Pt + (size_t)r * ld;
+      __nv_bfloat16* drow = dq + (size_t)r * ld;
+      float racc = 0.f;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const __nv_bfloat162 d2 = __floats2bfloat162_rn(v[2 * e] - c, v[2 * e + 1] - c);
-          const __nv_bfloat162 p2 = *reinterpret_cast<const __nv_bfloat162*>(&pw[i & 1][e]);
+      for (int j = 0; j < TC_BN / 8; ++j) {
+        const int col = t.n0 + 8 * j + 2 * (lane & 3);
+        if (live && col < ld) {
+          const __nv_bfloat162 d2 = __floats2bfloat162_rn(d[4 * j + 2 * h] - c, d[4 * j + 2 * h + 1] - c);
+          const __nv_bfloat162 p2 = *reinterpret_cast<const __nv_bfloat162*>(prow + col);
           racc = fmaf(__low2float(p2), __low2float(d2), racc);
           racc = fmaf(__high2float(p2), __high2float(d2), racc);
-          w[e] = *reinterpret_cast<const uint32_t*>(&d2);
+          *reinterpret_cast<__nv_bfloat162*>(drow + col) = d2;
         }
-        stg256(drow + col0, w);
       }
+      racc = quad_sum(racc);
+      if (live && (lane & 3) == 0) rpart[(size_t)t.tile_n * M + r] = racc;
     }
-    if (live) rpart[((size_t)t.tile_n * PARTS + part) * M + row] = racc;
   }
 };
 
@@ -271,62 +248,42 @@ struct TcEpiDpStore {
 struct TcEpiDpStoreF32 {
   float* dp; int ld;                       // [rows][ld] fp32
   const __nv_bfloat16* P3; size_t plane;   // three planes of [rows][ld] bf16
-  float* rpart;                            // [tiles_n * (NW / 4)][M]
+  float* rpart;                            // [tiles_n][M]
   int M;
-  template <int BN, int NW>
-  __device__ __forceinline__ void prologue(const TileCoord& t, int q, int ew, int lane) const {
-    static_assert(NW == 4 || NW == 8, "one or two warps per TMEM lane quarter");
-    constexpr int W = BN / (NW / 4);
-    const int row = t.m0 + q * 32 + lane, col = t.n0 + (ew >> 2) * W;
-    if (row < M) {
+  __device__ __forceinline__ void prologue(const TileCoord& t, int ct) const {
 #pragma unroll
-      for (int pl = 0; pl < 3; ++pl) {
-        const __nv_bfloat16* src = P3 + pl * plane + (size_t)row * ld + col;
-#pragma unroll
-        for (int b = 0; b < W; b += 64)
-          if (col + b < ld) prefetch_l2(src + b);
-      }
+    for (int i = ct; i < 3 * TC_BM * (TC_BN / 64); i += 256) {
+      const int pl = i / (TC_BM * (TC_BN / 64)), li = i - pl * (TC_BM * (TC_BN / 64));
+      const int row = t.m0 + (li >> 2), col = t.n0 + (li & 3) * 64;
+      if (row < M && col < ld) prefetch_l2(P3 + pl * plane + (size_t)row * ld + col);
     }
   }
-  __device__ __forceinline__ void finish(int, int, int) const {}
-  template <int BN, int NW>
-  __device__ __forceinline__ void run(uint32_t tmem_acc, int q, int ew, int lane, const TileCoord& t) const {
-    constexpr int PARTS = NW / 4, W = BN / PARTS, NCH = W / 16;
-    const int part = ew >> 2;
-    const int row = t.m0 + q * 32 + lane;
-    const int cbase = t.n0 + part * W;
-    const bool live = row < M;
-    const __nv_bfloat16* prow = P3 + (size_t)row * ld;
-    float* drow = dp + (size_t)row * ld;
-    float racc = 0.f;
-#pragma unroll 1
-    for (int i = 0; i < NCH; ++i) {
-      const int col0 = cbase + i * 16;
-      uint32_t ph[8], pm[8], pl[8];
-      if (live && col0 < ld) { ldg256(prow + col0, ph); ldg256(prow + plane + col0, pm); ldg256(prow + 2 * plane + col0, pl); }
-      float v[16];
-      tmem_ld16(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(col0 - t.n0), v);
-      if (live && col0 < ld) {
+  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane) const {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(&ph[e]);
-          const __nv_bfloat162 m2 = *reinterpret_cast<const __nv_bfloat162*>(&pm[e]);
-          const __nv_bfloat162 l2 = *reinterpret_cast<const __nv_bfloat162*>(&pl[e]);
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      const bool live = r < M;
+      const __nv_bfloat16* prow = P3 + (size_t)r * ld;
+      float* drow = dp + (size_t)r * ld;
+      float racc = 0.f;
+#pragma unroll
+      for (int j = 0; j < TC_BN / 8; ++j) {
+        const int col = t.n0 + 8 * j + 2 * (lane & 3);
+        if (live && col < ld) {
+          const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(prow + col);
+          const __nv_bfloat162 m2 = *reinterpret_cast<const __nv_bfloat162*>(prow + plane + col);
+          const __nv_bfloat162 l2 = *reinterpret_cast<const __nv_bfloat162*>(prow + 2 * plane + col);
           const float p0 = (__low2float(l2) + __low2float(m2)) + __low2float(h2);
           const float p1 = (__high2float(l2) + __high2float(m2)) + __high2float(h2);
-          racc = fmaf(p0, v[2 * e], racc);
-          racc = fmaf(p1, v[2 * e + 1], racc);
+          const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+          racc = fmaf(p0, v0, racc);
+          racc = fmaf(p1, v1, racc);
+          *reinterpret_cast<float2*>(drow + col) = make_float2(v0, v1);
         }
-        uint32_t w[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) w[e] = __float_as_uint(v[e]);
-        stg256(drow + col0, w);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) w[e] = __float_as_uint(v[8 + e]);
-        stg256(drow + col0 + 8, w);
       }
+      racc = quad_sum(racc);
+      if (live && (lane & 3) == 0) rpart[(size_t)t.tile_n * M + r] = racc;
     }
-    if (live) rpart[((size_t)t.tile_n * PARTS + part) * M + row] = racc;
   }
 };
 
@@ -338,19 +295,11 @@ __device__ __forceinline__ float fast_ex2(float x) { float y; asm("ex2.approx.ft
 __device__ __forceinline__ float fast_rcp(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float fast_sqrt(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-// Blackwell packed-fp32 arithmetic (fma/add/mul .f32x2): two elements per instruction on the FMA pipe.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float a, float b) { f32x2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { f32x2 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-
 // ---- split-precision operands -------------------------------------------------------------------
 // Parity mode on tensor cores ("bf16x3"): every fp32 operand value x is stored as three bf16 planes
 // hi + mid + lo (x reconstructed to ~2^-24), and a*b is accumulated in fp32 from the six partial products
 // whose magnitude is >= 2^-24 relative: (l,h) (h,l) (m,m) (m,h) (h,m) (h,h), smallest first.  The kernel
-// simply runs its k-loop once per pair into the same TMEM accumulator; with n_pairs == 1 only (h,h) runs
+// simply runs its k-loop once per pair into the same accumulator; with n_pairs == 1 only (h,h) runs
 // (plain bf16 mode).
 struct TcMaps { CUtensorMap m[3]; };
 __device__ __constant__ int kPairA[6] = {2, 0, 1, 1, 0, 0};
@@ -359,53 +308,44 @@ __device__ __constant__ int kPairB[6] = {0, 2, 1, 0, 1, 0};
 // ---- the kernel -------------------------------------------------------------------------------
 // Work item w -> (split z, row tile, column tile), column tile fastest so that CTAs running at the
 // same time share A rows and stream B through L2.
-template <bool A_KMAJOR, bool B_KMAJOR, int BN, int STAGES, int EPI_WARPS, class Epi>
-__global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1)
+template <bool A_KMAJOR, bool B_KMAJOR, int STAGES, class Epi>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps maps_b, int n_pairs,
           int k_total, int k_per_split, int tiles_m, int tiles_n, int splits, int group_m, uint64_t policy_a,
           uint64_t policy_b, int tm_off, int k_off, const Epi epi) {
   using TileA = OperandTile<A_KMAJOR, TC_BM>;
-  using TileB = OperandTile<B_KMAJOR, BN>;
+  using TileB = OperandTile<B_KMAJOR, TC_BN>;
   constexpr int kStageBytes = TileA::kBytes + TileB::kBytes;
-  constexpr uint32_t kTmemCols = 2 * BN;     // two accumulator buffers (256 or 512 columns)
-  static_assert(kTmemCols == 256 || kTmemCols == 512, "TMEM allocation must be a power of two <= 512");
-  constexpr uint32_t kIdesc = make_idesc(TC_BM, BN, !A_KMAJOR, !B_KMAJOR);
+  constexpr int kTA = A_KMAJOR ? 0 : 1, kTB = B_KMAJOR ? 0 : 1;
+  constexpr uint32_t kConsumerWarps = 8;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int total = tiles_m * tiles_n * splits;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps_a.m[0]);
     tma_prefetch_desc(&maps_b.m[0]);
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-#pragma unroll
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    setmaxnreg_producer();
+    if (threadIdx.x == 0) {
       uint32_t kbg = 0;                         // k-blocks issued so far (ring position)
       for (int w = blockIdx.x; w < total; w += gridDim.x) {
         const int z = w / (tiles_n * tiles_m);
         int tm_i, tn_i;
         tile_mn(w - z * tiles_n * tiles_m, tiles_m, tiles_n, group_m, tm_i, tn_i);
-        const int n0 = tn_i * BN, m0 = (tm_off + tm_i) * TC_BM;
+        const int n0 = tn_i * TC_BN, m0 = (tm_off + tm_i) * TC_BM;
         const int k_begin = k_off + z * k_per_split;
         const int k_end = min(k_total, k_begin + k_per_split);
         const int num_kb = (k_end - k_begin + TC_BK - 1) / TC_BK;
@@ -426,252 +366,53 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one thread) =====
-    if (lane == 0) {
-      uint32_t kbg = 0;
-      int it = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-        const int z = w / (tiles_n * tiles_m);
-        const int k_begin = k_off + z * k_per_split;
-        const int k_end = min(k_total, k_begin + k_per_split);
-        const int num_kb = (k_end - k_begin + TC_BK - 1) / TC_BK;
-        const int b = it & 1;
-        mbar_wait(&tempty_bar[b], (((uint32_t)it >> 1) & 1) ^ 1);   // epilogue has drained this buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(b * BN);
-        const int total_kb = num_kb * n_pairs;
-        for (int kb = 0; kb < total_kb; ++kb, ++kbg) {
-          const int s = kbg % STAGES;
-          const uint32_t ph = (kbg / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * kStageBytes);
-          const uint32_t sb = sa + TileA::kBytes;
-#pragma unroll
-          for (int k = 0; k < TC_BK / TC_UMMA_K; ++k)
-            umma_bf16(d_tmem, TileA::desc(sa, k), TileB::desc(sb, k), kIdesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[s]);           // frees the smem stage when these MMAs retire
-        }
-        umma_commit(&tfull_bar[b]);             // accumulator of this tile complete
-      }
-    }
   } else {
-    // ===== epilogue warps: TMEM -> registers -> fused epilogue =====
-    const int q = warp & 3;                     // TMEM lane quarter this warp may access
-    const int ew = warp - 2;
-    int it = 0;
-    for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
+    // ===== consumers: wgmma main loop, then the fused epilogue on the accumulator registers =====
+    setmaxnreg_consumer();
+    const int cw = wg - 1;                      // rows [64 cw, 64 cw + 64) of the tile
+    const int ct = threadIdx.x - 128;
+    const int row_in_tile = 64 * cw + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+    float acc[TC_ACC];
+#pragma unroll
+    for (int i = 0; i < TC_ACC; ++i) acc[i] = 0.f;
+    uint32_t kbg = 0;
+    for (int w = blockIdx.x; w < total; w += gridDim.x) {
       TileCoord t;
       t.split = w / (tiles_n * tiles_m);
       int tm_i;
       tile_mn(w - t.split * tiles_n * tiles_m, tiles_m, tiles_n, group_m, tm_i, t.tile_n);
       t.tiles_n = tiles_n;
-      t.n0 = t.tile_n * BN;
+      t.n0 = t.tile_n * TC_BN;
       t.m0 = (tm_off + tm_i) * TC_BM;
-      const int b = it & 1;
+      const int k_begin = k_off + t.split * k_per_split;
+      const int k_end = min(k_total, k_begin + k_per_split);
+      const int total_kb = (k_end - k_begin + TC_BK - 1) / TC_BK * n_pairs;
 #ifndef TGB_SKIP_EPI
-      epi.template prologue<BN, EPI_WARPS>(t, q, ew, lane);
+      epi.prologue(t, ct);
 #endif
-      mbar_wait(&tfull_bar[b], ((uint32_t)it >> 1) & 1);
-      tc_fence_after();
-#ifndef TGB_SKIP_EPI
-      epi.template run<BN, EPI_WARPS>(tmem_base + (uint32_t)(b * BN), q, ew, lane, t);
-#endif
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[b]);
-    }
-    epi.finish(ew, lane, 0);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
-}
-
-// ---- CTA-pair variant (tcgen05 cta_group::2) ----------------------------------------------------
-// Two CTAs of a cluster (ranks 0/1, adjacent SMs) compute one 256 x BN tile: each stages ITS 128 rows of A and
-// HALF of the B tile, rank 0's MMA thread issues M=256 instructions that read both CTAs' shared memory and write
-// rows 0-127 / 128-255 of the tile into the two CTAs' TMEM.  B crosses L2->SM once per 256 output rows instead
-// of once per 128, and a stage is 16 KB smaller per CTA -- room for a deeper epilogue staging pipeline.
-// Protocol (cf. the cluster/2-SM notes in blackwell_cuda_programming.md):
-//   full[s]   lives in rank 0: armed there with both CTAs' bytes; both producers' bulk loads complete_tx on it
-//   empty[s]  one multicast tcgen05.commit per use arrives on BOTH CTAs' barriers (each producer waits locally)
-//   tfull[b]  multicast commit -> each CTA's epilogue waits on its own copy
-//   tempty[b] lives in rank 0: the epilogue warps of both CTAs arrive on it remotely
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* map, uint32_t leader_bar, uint32_t dst, int c0, int c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// K-major A and B only (the backward contraction).  tiles_m counts 256-row pair tiles; grid = 2 x clusters.
-template <int BN, int STAGES, int EPI_WARPS, class Epi>
-__global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1)
-k_gemm_tc_pair(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps maps_b, int n_pairs, int k_total, int tiles_m, int tiles_n, int group_m,
-               uint64_t policy_a, uint64_t policy_b, int tm_off, const Epi epi) {
-  using TileA = OperandTile<true, TC_BM>;         // this CTA's 128 rows
-  using TileB = OperandTile<true, BN / 2>;        // this CTA's half of the B tile
-  constexpr int kStageBytes = TileA::kBytes + TileB::kBytes;
-  constexpr uint32_t kTmemCols = 2 * BN;
-  static_assert(kTmemCols == 256 || kTmemCols == 512, "TMEM allocation must be a power of two <= 512");
-  constexpr uint32_t kIdesc = make_idesc(2 * TC_BM, BN, false, false);
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES];
-  __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-  const int total = tiles_m * tiles_n;
-  const int num_kb = (k_total + TC_BK - 1) / TC_BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&maps_a.m[0]);
-    tma_prefetch_desc(&maps_b.m[0]);
+      acc_fence(acc);
+      for (int kb = 0; kb < total_kb; ++kb, ++kbg) {
+        const int s = kbg % STAGES;
+        const uint32_t ph = (kbg / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sa = smem_u32(smem + s * kStageBytes) + cw * 8192;
+        const uint32_t sb = smem_u32(smem + s * kStageBytes) + TileA::kBytes;
+        wgmma_fence();
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-#pragma unroll
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 2 * EPI_WARPS); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_pair(&tmem_base_smem, kTmemCols);
-  tc_fence_before();
-  cluster_sync_all();                           // barriers of both CTAs initialised before any remote arrive / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp == 0) {
-    // ===== TMA producer (both CTAs): own A rows + own half of B, completing on rank 0's full barrier =====
-#ifdef TGB_SKIP_MAINLOOP
-    if (false) {
-#else
-    if (lane == 0) {
-#endif
-      uint32_t kbg = 0;
-      for (int w = cid; w < total; w += ncl) {
-        int tm_i, tn_i;
-        tile_mn(w, tiles_m, tiles_n, group_m, tm_i, tn_i);
-        const int n0 = tn_i * BN + (int)rank * (BN / 2);
-        const int m0 = (tm_off + tm_i) * (2 * TC_BM) + (int)rank * TC_BM;
-        for (int pr = 6 - n_pairs; pr < 6; ++pr) {
-          const CUtensorMap* ma = &maps_a.m[kPairA[pr]];
-          const CUtensorMap* mb = &maps_b.m[kPairB[pr]];
-          for (int kb = 0; kb < num_kb; ++kb, ++kbg) {
-            const int s = kbg % STAGES;
-            const uint32_t ph = (kbg / STAGES) & 1;
-            mbar_wait(&empty_bar[s], ph ^ 1);
-            const uint32_t sa = smem_u32(smem + s * kStageBytes);
-            const uint32_t sb = sa + TileA::kBytes;
-            if (rank == 0) mbar_expect_tx(&full_bar[s], 2 * kStageBytes);
-            const uint32_t lbar = mapa_shared(smem_u32(&full_bar[s]), 0);
-            tma_load_2d_pair(ma, lbar, sa, kb * TC_BK, m0, policy_a);
-            tma_load_2d_pair(mb, lbar, sb, kb * TC_BK, n0, policy_b);
-          }
-        }
+        for (int k = 0; k < TC_BK / TC_MMA_K; ++k)
+          wgmma_m64n256k16<kTA, kTB>(acc, TileA::desc(sa, k), TileB::desc(sb, k), (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                        // the MMAs of the previous k-block have retired: release its stage
+        if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(kbg - 1) % STAGES]);
       }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer: one thread of rank 0 drives both SMs' tensor cores =====
-    if (lane == 0 && rank == 0) {
-      uint32_t kbg = 0;
-      int it = 0;
-      for (int w = cid; w < total; w += ncl, ++it) {
-        const int b = it & 1;
-        mbar_wait(&tempty_bar[b], (((uint32_t)it >> 1) & 1) ^ 1);   // both epilogues have drained this buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(b * BN);
-#ifdef TGB_SKIP_MAINLOOP
-        const int total_kb = 0;
-#else
-        const int total_kb = num_kb * n_pairs;
-#endif
-        for (int kb = 0; kb < total_kb; ++kb, ++kbg) {
-          const int s = kbg % STAGES;
-          const uint32_t ph = (kbg / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * kStageBytes);
-          const uint32_t sb = sa + TileA::kBytes;
-#pragma unroll
-          for (int k = 0; k < TC_BK / TC_UMMA_K; ++k)
-            umma_bf16_pair(d_tmem, TileA::desc(sa, k), TileB::desc(sb, k), kIdesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit_pair(&empty_bar[s]);
-        }
-        umma_commit_pair(&tfull_bar[b]);
-      }
-    }
-  } else {
-    // ===== epilogue warps (both CTAs): each CTA owns 128 rows of the pair tile =====
-    const int q = warp & 3;
-    const int ew = warp - 2;
-    const uint32_t tempty_remote = mapa_shared(smem_u32(&tempty_bar[0]), 0);
-    int it = 0;
-    for (int w = cid; w < total; w += ncl, ++it) {
-      TileCoord t;
-      int tm_i;
-      tile_mn(w, tiles_m, tiles_n, group_m, tm_i, t.tile_n);
-      t.tiles_n = tiles_n;
-      t.n0 = t.tile_n * BN;
-      t.m0 = (tm_off + tm_i) * (2 * TC_BM) + (int)rank * TC_BM;
-      t.split = 0;
-      const int b = it & 1;
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (total_kb > 0 && lane == 0) mbar_arrive(&empty_bar[(kbg - 1) % STAGES]);
 #ifndef TGB_SKIP_EPI
-      epi.template prologue<BN, EPI_WARPS>(t, q, ew, lane);
+      epi.run(acc, t, t.m0 + row_in_tile, lane);
 #endif
-      mbar_wait(&tfull_bar[b], ((uint32_t)it >> 1) & 1);
-      tc_fence_after();
-#ifndef TGB_SKIP_EPI
-      epi.template run<BN, EPI_WARPS>(tmem_base + (uint32_t)(b * BN), q, ew, lane, t);
-#endif
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(tempty_remote + (uint32_t)b * 8u);
     }
-    epi.finish(ew, lane, 0);
   }
-  tc_fence_before();
-  cluster_sync_all();                           // the peer's shared memory and barriers stay valid until both are done
-  if (warp == 1) tmem_dealloc_pair(tmem_base, kTmemCols);
 }
 
 // ---- host side --------------------------------------------------------------------------------
@@ -681,9 +422,7 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 
 struct TcContext {
   PFN_encodeTiled encode = nullptr;
-  int num_sms = 148;
-  int pair_clusters = -1;   // co-resident 2-CTA clusters of the backward pair kernel (-1 = not queried yet, 0 = unavailable)
-  int dp_clusters = -1;     // same for the store-only backward kernel
+  int num_sms = 132;
   const void* smem_fn[16] = {};   // kernels whose dynamic shared-memory limit this handle has already raised
   int smem_bytes[16] = {};
 };
@@ -741,28 +480,13 @@ static inline int tc_check_launch(const char* name, char* err, size_t n) {
   return 0;
 }
 
-constexpr int TC_FWD_BN = 256, TC_FWD_STAGES = 4;
-#ifndef TGB_BWD_BN
-#define TGB_BWD_BN 256
-#endif
-constexpr int TC_BWD_BN = TGB_BWD_BN;
-// CTA-pair backward kernel (cta_group::2): used from TC_PAIR_MIN_ROWS cells up (smaller problems don't fill 74 pairs)
-#ifndef TGB_BWD_PAIR
-#define TGB_BWD_PAIR 1
-#endif
-constexpr int TC_PAIR_MIN_ROWS = 2048;
-// store-only backward (staged dP): no epilogue staging in shared memory, so the operand ring can be deeper
-#ifndef TGB_DP_STAGES
-#define TGB_DP_STAGES 6
-#endif
-#ifndef TGB_DP_EPI_WARPS
-#define TGB_DP_EPI_WARPS 4
-#endif
-constexpr int TC_DP_STAGES = TGB_DP_STAGES, TC_DP_SINGLE_STAGES = 4, TC_DP_EPI_WARPS = TGB_DP_EPI_WARPS;
-static inline int tc_dp_row_parts(int V) { return (int)ceil_div(V, TC_BWD_BN) * (TC_DP_EPI_WARPS / 4); }
-// (tile_mn's row-tile groups stay at 1: more CTAs pulling the same B tile at once hot-spot L2 slices -- measured in round 1.)
-static inline int tc_splits(long long tiles, long long k_total, int min_k) {
-  long long s = (2 * 148 + tiles - 1) / tiles;
+// 4 stages of 48 KB (128 x 64 A + 256 x 64 B, bf16): 193 KB of the 227 KB an H100 block may use
+constexpr int TC_STAGES = 4;
+constexpr int TC_SMEM = TC_STAGES * (TC_BM + TC_BN) * TC_BK * 2 + 1024;
+static inline int tc_dp_row_parts(int V) { return (int)ceil_div(V, TC_BN); }
+// (tile_mn's row-tile groups stay at 1: more CTAs pulling the same B tile at once hot-spot L2 slices.)
+static inline int tc_splits(int num_sms, long long tiles, long long k_total, int min_k) {
+  long long s = (2LL * num_sms + tiles - 1) / tiles;
   const long long max_s = (k_total + min_k - 1) / min_k;
   if (s > max_s) s = max_s;
   if (s < 1) s = 1;
@@ -771,17 +495,16 @@ static inline int tc_splits(long long tiles, long long k_total, int min_k) {
   return (int)((k_total + kps - 1) / kps);
 }
 // Parity mode: the tensor core accumulates in fp32 with truncation, a bias that grows with the length of the
-// accumulation chain (measured on real data: -5.6e-6 relative at 6.6k-deep chains, -0.9e-6 at 1.6k).  Chains are
-// therefore cut at `max_chain` contraction elements; the partial results are summed in fp32 (round-to-nearest) by
-// the kernels that consume them.
+// accumulation chain.  Chains are therefore cut at `max_chain` contraction elements; the partial results are summed
+// in fp32 (round-to-nearest) by the kernels that consume them.
 static inline int tc_splits_for_chain(long long k_total, int max_chain) {
   long long s = (k_total + max_chain - 1) / max_chain;
   if (s < 1) s = 1;
   const long long kps = ((k_total + s - 1) / s + TC_BK - 1) / TC_BK * TC_BK;
   return (int)((k_total + kps - 1) / kps);
 }
-static inline int tc_forward_splits(int N, int V, int Ke) {
-  return tc_splits((long long)ceil_div(V, TC_BM) * ceil_div(Ke, TC_FWD_BN), N, 512);
+static inline int tc_forward_splits(int num_sms, int N, int V, int Ke) {
+  return tc_splits(num_sms, (long long)ceil_div(V, TC_BM) * ceil_div(Ke, TC_BN), N, 512);
 }
 static inline int tc_kps(int k_total, int splits) {
   return (int)(round_up(ceil_div(k_total, splits), TC_BK));
@@ -804,7 +527,6 @@ static inline int tc_make_maps(TcContext& tc, TcMaps* maps, const __nv_bfloat16*
 // encodes each plan once (the buffers never move) instead of on every launch.
 struct TcPlan {
   TcMaps a, b;
-  bool pair = false;        // b is encoded for the CTA-pair kernel (half-tile boxes)
   bool ready = false;
 };
 
@@ -818,26 +540,24 @@ static inline int tc_forward_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16
 }
 static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int N, int V, int Ke, int splits,
                                     cudaStream_t s, char* err, size_t n) {
-  auto kern = k_gemm_tc<false, false, TC_FWD_BN, TC_FWD_STAGES, 4, TcEpiStore>;
-  const int smem = TC_FWD_STAGES * (TC_BM + TC_FWD_BN) * TC_BK * 2 + 1024;
-  if (tc_set_smem(tc, kern, smem, err, n)) return -2;
+  auto kern = k_gemm_tc<false, false, TC_STAGES, TcEpiStore>;
+  if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, 0};
-  const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_FWD_BN);
-  kern<<<tc_grid(tc, (long long)tm * tn * splits), 64 + 32 * 4, smem, s>>>(pl.a, pl.b, n_pairs, N, tc_kps(N, splits), tm, tn,
-                                                                         splits, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, 0, epi);
+  const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
+  kern<<<tc_grid(tc, (long long)tm * tn * splits), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, N, tc_kps(N, splits), tm, tn,
+                                                                             splits, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, 0, epi);
   return tc_check_launch("tc_gemm_fwd", err, n);
 }
 // cells [row0, row1) only (row0 a multiple of 64): `out` = or += this chunk's partial sum -- the host pipelines cell chunks
 // behind the streaming Adam kernel; the chunks run one after the other on one stream, so the summation order is fixed
 static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, float* out, int accumulate, int row0, int row1, int V, int Ke,
                                          cudaStream_t s, char* err, size_t n) {
-  auto kern = k_gemm_tc<false, false, TC_FWD_BN, TC_FWD_STAGES, 4, TcEpiStore>;
-  const int smem = TC_FWD_STAGES * (TC_BM + TC_FWD_BN) * TC_BK * 2 + 1024;
-  if (tc_set_smem(tc, kern, smem, err, n)) return -2;
+  auto kern = k_gemm_tc<false, false, TC_STAGES, TcEpiStore>;
+  if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, accumulate};
-  const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_FWD_BN);
-  kern<<<tc_grid(tc, (long long)tm * tn), 64 + 32 * 4, smem, s>>>(pl.a, pl.b, 1, row1, (int)round_up(row1 - row0, TC_BK), tm, tn,
-                                                                1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
+  const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
+  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, 1, row1, (int)round_up(row1 - row0, TC_BK), tm, tn,
+                                                                    1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
   return tc_check_launch("tc_gemm_fwd", err, n);
 }
 // one-shot variant for temporary operands (tgb200_project)
@@ -849,75 +569,25 @@ static inline int tc_forward(TcContext& tc, const __nv_bfloat16* P, size_t p_pla
   return tc_forward_launch(tc, pl, n_pairs, out, N, V, Ke, splits, s, err, n);
 }
 
-// number of co-resident 2-CTA clusters of a pair kernel (persistent: never launch more), 0 = unavailable
-template <class Kern>
-static inline int tc_pair_clusters(TcContext& tc, Kern pk, int threads, int smem, cudaStream_t s) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  cfg.gridDim = dim3(tc.num_sms & ~1);
-  int mc = 0;
-  const int r = cudaOccupancyMaxActiveClusters(&mc, pk, &cfg) == cudaSuccess ? mc : 0;
-  (void)cudaGetLastError();
-  return r;
-}
-template <class Kern, class... Args>
-static inline cudaError_t tc_launch_pair(Kern pk, unsigned clusters, int threads, int smem, cudaStream_t s, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  cfg.gridDim = dim3(2 * clusters);
-  return cudaLaunchKernelEx(&cfg, pk, args...);
-}
-
 // Staged backward: dq = bf16(S_ext dY_ext^T - centre) (bf16 mode) or dP in fp32 (bf16x3 mode, three operand planes, six
 // partial products) to HBM + row-dot partials; the update itself is a streaming kernel (adam_rows.cuh).  Rows [row0, row1)
-// only (row0 a multiple of 256): the host pipelines row chunks.
-template <class Epi>
+// only (row0 a multiple of 128): the host pipelines row chunks.
 static inline int tc_dpstore_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16* Sxb, size_t s_plane, const __nv_bfloat16* dYb,
-                                  size_t dy_plane, int planes, int N, int V, int Ke, cudaStream_t s, char* err, size_t n) {
+                                  size_t dy_plane, int planes, int N, int V, int Ke, char* err, size_t n) {
   if (tc_make_maps(tc, &pl.a, Sxb, s_plane, planes, Ke, N, Ke, 64, TC_BM, err, n)) return -2;
-  pl.pair = false;
-#if TGB_BWD_PAIR
-  if (N >= TC_PAIR_MIN_ROWS) {
-    auto pk = k_gemm_tc_pair<TC_BWD_BN, TC_DP_STAGES, TC_DP_EPI_WARPS, Epi>;
-    const int psmem = TC_DP_STAGES * (TC_BM + TC_BWD_BN / 2) * TC_BK * 2 + 1024;
-    if (tc_set_smem(tc, pk, psmem, err, n)) return -2;
-    if (tc.dp_clusters < 0) tc.dp_clusters = tc_pair_clusters(tc, pk, 64 + 32 * TC_DP_EPI_WARPS, psmem, s);
-    pl.pair = tc.dp_clusters > 0;
-  }
-#endif
-  if (tc_make_maps(tc, &pl.b, dYb, dy_plane, planes, Ke, V, Ke, 64, pl.pair ? TC_BWD_BN / 2 : TC_BWD_BN, err, n)) return -2;
+  if (tc_make_maps(tc, &pl.b, dYb, dy_plane, planes, Ke, V, Ke, 64, TC_BN, err, n)) return -2;
   pl.ready = true;
   return 0;
 }
 template <class Epi>
 static inline int tc_dpstore_launch(TcContext& tc, const TcPlan& pl, int n_pairs, const Epi& epi, int row0, int row1, int V, int Ke,
                                     cudaStream_t s, char* err, size_t n) {
-  const int tn = (int)ceil_div(V, TC_BWD_BN);
-  if (pl.pair) {
-    auto pk = k_gemm_tc_pair<TC_BWD_BN, TC_DP_STAGES, TC_DP_EPI_WARPS, Epi>;
-    const int psmem = TC_DP_STAGES * (TC_BM + TC_BWD_BN / 2) * TC_BK * 2 + 1024;
-    const int tm0 = row0 / (2 * TC_BM), tmp = (int)ceil_div(row1, 2 * TC_BM) - tm0;
-    const long long pair_tiles = (long long)tmp * tn;
-    const unsigned clusters = (unsigned)(pair_tiles < tc.dp_clusters ? pair_tiles : tc.dp_clusters);
-    cudaError_t e = tc_launch_pair(pk, clusters, 64 + 32 * TC_DP_EPI_WARPS, psmem, s, pl.a, pl.b, n_pairs, Ke, tmp, tn, 1,
-                                   (uint64_t)kPolicyEvictNormal, (uint64_t)kPolicyEvictLast, tm0, epi);
-    if (e != cudaSuccess) { snprintf(err, n, "launch tc_gemm_bwd_dp (pair): %s", cudaGetErrorString(e)); return -2; }
-    return tc_check_launch("tc_gemm_bwd_dp", err, n);
-  }
-  auto kern = k_gemm_tc<true, true, TC_BWD_BN, TC_DP_SINGLE_STAGES, TC_DP_EPI_WARPS, Epi>;
-  const int smem = TC_DP_SINGLE_STAGES * (TC_BM + TC_BWD_BN) * TC_BK * 2 + 1024;
-  if (tc_set_smem(tc, kern, smem, err, n)) return -2;
+  const int tn = (int)ceil_div(V, TC_BN);
+  auto kern = k_gemm_tc<true, true, TC_STAGES, Epi>;
+  if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   const int tm0 = row0 / TC_BM, tm = (int)ceil_div(row1, TC_BM) - tm0;
-  kern<<<tc_grid(tc, (long long)tm * tn), 64 + 32 * TC_DP_EPI_WARPS, smem, s>>>(pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
-                                                                                kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
+  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
+                                                                    kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
   return tc_check_launch("tc_gemm_bwd_dp", err, n);
 }
 

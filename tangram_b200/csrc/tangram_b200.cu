@@ -1,5 +1,5 @@
-// C-ABI of the B200-native map_cells_to_space hot path (see include/tangram_b200.h).
-// Host orchestration only; every kernel is hand-written for sm_100a in the .cuh files.
+// C-ABI of the native map_cells_to_space hot path (see include/tangram_b200.h).
+// Host orchestration only; every kernel is hand-written for sm_90a (H100) in the .cuh files.
 #include "../../include/tangram_b200.h"
 
 #include <cmath>
@@ -123,7 +123,7 @@ struct tgb200_mapper {
   bool in_step = false;
   int64_t launches = 0;
   KernelTimer* timer = nullptr;
-  TcContext tc;                 // driver entry points etc. for the tcgen05 path
+  TcContext tc;                 // driver entry points etc. for the wgmma path
   TcPlan plan_fwd, plan_dp;     // tensor maps of the two contractions, encoded once (the buffers never move)
   // staged backward (bf16 mode): store-only contraction -> bf16 dq = dP - centre in HBM -> streaming Adam kernel;
   // two contractions per iteration instead of three (no separate row-dot GEMM)
@@ -250,7 +250,7 @@ extern "C" int tgb200_host_unpin(void* buf) {
   return TGB200_OK;
 }
 extern "C" const char* tgb200_last_error(void) { return g_err; }
-extern "C" const char* tgb200_version(void) { return "tangram_b200 0.2.0 (sm_100a)"; }
+extern "C" const char* tgb200_version(void) { return "tangram_b200 0.3.0 (sm_90a)"; }
 
 extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (!cfg || !out) return fail(TGB200_ERR_INVALID, "null argument");
@@ -278,7 +278,8 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (cfg->device < 0 || cfg->device >= ndev) return fail(TGB200_ERR_INVALID, "device %d out of range (%d devices)", cfg->device, ndev);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return fail(TGB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(TGB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major, prop.minor);
   CK(cudaSetDevice(cfg->device));
 
   tgb200_mapper* h = new tgb200_mapper();
@@ -350,14 +351,15 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
     h->pipelined = ok;
     h->l2_persist = getenv("TGB200_L2_PERSIST") && atoi(getenv("TGB200_L2_PERSIST")) != 0;
   }
-  // forward split over cells so that the grid covers the 148 SMs (deterministic partial planes)
+  // forward split over cells so that the grid covers the SMs twice (deterministic partial planes)
+  h->tc.num_sms = prop.multiProcessorCount;
   {
     const int tiles = (int)(ceil_div(h->V, 128) * ceil_div(h->Ke, 128));
-    int s = (int)ceil_div(2 * 148, tiles);
+    int s = (int)ceil_div(2 * h->tc.num_sms, tiles);
     const int max_s = (int)ceil_div(h->N, 512);
     if (s > max_s) s = max_s;
     if (s < 1) s = 1;
-    if (h->tcm) s = tc_forward_splits(h->N, h->V, h->Ke);
+    if (h->tcm) s = tc_forward_splits(h->tc.num_sms, h->N, h->V, h->Ke);
     if (h->x3) { const int c = tc_splits_for_chain(h->N, 2048); if (c > s) s = c; }
     if (h->nchunks > 1) s = 1;               // the cell chunks of the pipelined forward accumulate straight into Y_ext
     h->fwd_splits = s;
@@ -368,7 +370,7 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
     A(h->Fl.alloc(h->N)); A(h->mF.alloc(h->N)); A(h->vF.alloc(h->N)); A(h->fsig.alloc(h->N));
     A(h->Sf.alloc((size_t)h->N * h->Ke)); A(h->fscal.alloc(4));
   }
-  h->r_parts = h->tcm ? tc_dp_row_parts(h->V) : (int)ceil_div(h->Ke, SG_BN);                   // TcEpiDpStore: one partial per (voxel tile, epilogue warp of a lane quarter)
+  h->r_parts = h->tcm ? tc_dp_row_parts(h->V) : (int)ceil_div(h->Ke, SG_BN);                   // TcEpiDpStore: one partial per voxel tile
   A(h->rpart.alloc((size_t)h->r_parts * h->N));
   A(h->ngc.alloc(h->Ke)); A(h->ngr.alloc(h->V));
   // voxel rows per CTA of the loss reductions: enough CTAs for small V, bounded partial arrays for large V
@@ -940,7 +942,7 @@ static int filter_update(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
 // then one streaming pass does softmax-Jacobian + Adam + the next forward's P.  (mapping_optimizer.py:395-396)
 static int backward_staged(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, const AdamScalars& a) {
   if (!h->plan_dp.ready)
-    CKS(tc_dpstore_plan<TcEpiDpStore>(h->tc, h->plan_dp, h->Sxb.p, 0, h->dYb.p, 0, 1, h->N, h->V, h->Ke, s, g_err, sizeof(g_err)));
+    CKS(tc_dpstore_plan(h->tc, h->plan_dp, h->Sxb.p, 0, h->dYb.p, 0, 1, h->N, h->V, h->Ke, g_err, sizeof(g_err)));
   const bool two_streams = su != s;
   const bool prefetch = two_streams && h->prefetch_next && h->nchunks > 1 && !h->constrained;
   for (int c = 0; c < h->nchunks; ++c) {
@@ -985,7 +987,7 @@ static int backward_staged(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, co
 static int backward_staged_x3(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a) {
   const size_t nkp = (size_t)h->N * h->Ke, vkp = (size_t)h->V * h->Ke, nvp = (size_t)h->N * h->ld;
   if (!h->plan_dp.ready)
-    CKS(tc_dpstore_plan<TcEpiDpStoreF32>(h->tc, h->plan_dp, h->Sxb.p, nkp, h->dYb.p, vkp, 3, h->N, h->V, h->Ke, s, g_err, sizeof(g_err)));
+    CKS(tc_dpstore_plan(h->tc, h->plan_dp, h->Sxb.p, nkp, h->dYb.p, vkp, 3, h->N, h->V, h->Ke, g_err, sizeof(g_err)));
   TcEpiDpStoreF32 epi{h->dpf.p, h->ld, h->Pb.p, nvp, h->rpart.p, h->N};
   // all six partial products: with only the three or four largest the one-step tests leave their 1e-5 band (measured
   // 28.6 / 25.8 it/s at C3 instead of 21.2 -- not worth the parity-grade mode's point)
@@ -1297,7 +1299,7 @@ extern "C" int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, 
     if (!h->x3) { CKS(Pown.alloc(3 * pplane, false)); Pp = Pown.p; }   // bf16 mode: Pb carries the unnormalised P state
     CKS(launch_softmax_rows<float>(h, s, (float*)nullptr, 0, nullptr, Split3{Pp, pplane}));
     const int ldc = (int)round_up(n_cols < chunk ? n_cols : chunk, 64);
-    int splits = tc_forward_splits(h->N, h->V, ldc);
+    int splits = tc_forward_splits(h->tc.num_sms, h->N, h->V, ldc);
     { const int c = tc_splits_for_chain(h->N, 2048); if (c > splits) splits = c; }
     const size_t xplane = (size_t)h->N * ldc, oplane = (size_t)h->V * ldc;
     DevBuf<float> Xc, Opart, Oc;

@@ -1,12 +1,12 @@
 """
 Drop-in replacement for the reference optimizer class `Mapper`
-(/root/reference/tangram/mapping_optimizer.py:14-408), running on the sm_100a C-ABI
+(Tangram's tangram/mapping_optimizer.py:14-408), running on the sm_90a (H100) C-ABI
 library (include/tangram_b200.h).  Same constructor keywords, same `train()` signature,
 same return types and history conventions.  There is no CPU path: `device` must be a
-CUDA device with compute capability 10.x.
+CUDA device with compute capability 9.0.
 
 Additions (keyword-only, all optional):
-  precision   "bf16x3" (default: parity-grade fp32 results on tcgen05 tensor cores -- every operand is split into three
+  precision   "bf16x3" (default: parity-grade fp32 results on wgmma tensor cores -- every operand is split into three
               bf16 planes and the six significant partial products are accumulated in fp32) |
               "fp32" (FFMA contractions, the cross-check) | "bf16" (plain bf16 operands: throughput mode)
   M0          explicit initial mapping (ndarray N x V); default is the reference draw
@@ -40,7 +40,7 @@ def _device_index(device):
     if s.startswith("cuda"):
         return int(s.split(":")[1]) if ":" in s else 0
     raise ValueError(
-        f"tangram_b200.Mapper runs on B200 GPUs only (device={device!r}); "
+        f"tangram_b200.Mapper runs on H100 GPUs only (device={device!r}); "
         "use the reference implementation for device='cpu'")
 
 

@@ -1,6 +1,6 @@
 """
 `map_cells_to_space` with the reference's signature and output contract
-(/root/reference/tangram/mapping_utils.py:141-428), hosted over the B200 Mapper.
+(Tangram's tangram/mapping_utils.py:141-428), hosted over the H100 Mapper.
 AnnData in, AnnData out (duck-typed: `anndata` is optional).  `pp_adatas` and
 `adata_to_cluster_expression` are the small host-side preparations this entry needs
 (:20-139); squidpy's neighbour graph must be supplied by the caller in

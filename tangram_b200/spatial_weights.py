@@ -1,5 +1,5 @@
 """Sparse restatement of tangram/spatial_weights.py:5-30.  The reference densifies the
-~7-nnz/row neighbour graph to V x V (via libpysal / sklearn, absent here); the B200 path
+~7-nnz/row neighbour graph to V x V (via libpysal / sklearn, absent here); the GPU path
 keeps it as scipy CSR end to end (SURVEY.md 8(f) N4)."""
 import numpy as np
 

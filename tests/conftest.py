@@ -9,4 +9,4 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) GPU (run with -m gpu)")

@@ -5,11 +5,19 @@ import numpy as np
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 GOLDEN_CASES = ["cells_default", "cells_nodensity", "cells_regs", "clusters", "cells_spatial"]
-# The reference's one-file hot path: the tree itself where it exists (this container), else the verbatim copy that
-# oracle/build_ref.py left in oracle/_ref/ (git-ignored; it travels to the GPU box with the snapshot).
-_REF_CANDIDATES = ["/root/reference/tangram/mapping_optimizer.py",
-                   os.path.join(os.path.dirname(GOLDEN_DIR.rstrip(os.sep)), "..", "oracle", "_ref", "mapping_optimizer.py")]
-REFERENCE_FILE = next((os.path.abspath(p) for p in _REF_CANDIDATES if os.path.exists(p)), _REF_CANDIDATES[0])
+# Stand-in for tangram/mapping_optimizer.py of a Tangram checkout: the reference's two classes, restated by this repository's
+# oracle (which tests/test_oracle.py pins to stored runs of the reference)
+_STANDIN = ("from oracle.tangram_oracle import OracleMapper as Mapper  # noqa: F401\n"
+            "from oracle.tangram_oracle import OracleMapperConstrained as MapperConstrained  # noqa: F401\n")
+
+
+def standin_checkout(tmp_path):
+    """A directory shaped like a Tangram checkout, holding the oracle stand-in, for where no checkout of the original
+    project exists (oracle/build_ref.py finds one next to this repository or in TANGRAM_REFERENCE)."""
+    os.makedirs(os.path.join(tmp_path, "tangram"), exist_ok=True)
+    with open(os.path.join(tmp_path, "tangram", "mapping_optimizer.py"), "w") as f:
+        f.write(_STANDIN)
+    return str(tmp_path)
 
 
 def load_golden(name):
@@ -38,13 +46,6 @@ def max_rel(a, b):
     b = np.asarray(b, dtype=np.float64)
     return float(np.max(np.abs(a - b) / np.maximum(np.abs(b), 1e-12)))
 
-
-def load_reference_module():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("ref_mapping_optimizer", REFERENCE_FILE)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def assert_same_print(ours, ref):

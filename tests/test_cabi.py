@@ -32,7 +32,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in the header but not exported"
         assert name in _lib.SIGNATURES, f"{name} has no ctypes signature"
     assert set(_lib.SIGNATURES) == set(declared_symbols())
-    assert b"sm_100a" in lib.tgb200_version()
+    assert b"sm_90a" in lib.tgb200_version()
 
 
 def test_config_struct_layout_matches_c(tmp_path):
@@ -67,7 +67,7 @@ def test_no_gpu_fails_loudly_no_cpu_fallback():
     G = np.ones((5, 3), dtype=np.float32)
     with pytest.raises(_lib.TangramB200Error, match="no CPU fallback|CUDA"):
         Mapper(S, G, device="cuda:0", random_state=1)
-    with pytest.raises(ValueError, match="B200 GPUs only"):
+    with pytest.raises(ValueError, match="H100 GPUs only"):
         Mapper(S, G, device="cpu", random_state=1)
 
 

@@ -134,7 +134,7 @@ def test_mapper_refuses_unsupported_terms_and_cpu():
         tg.Mapper(S, G, lambda_geary=1.0)
     with pytest.raises(NotImplementedError):
         tg.Mapper(S, G, adata_map=object())
-    with pytest.raises(ValueError, match="B200 GPUs only"):
+    with pytest.raises(ValueError, match="H100 GPUs only"):
         tg.Mapper(S, G, device="cpu")
 
 
@@ -189,19 +189,26 @@ def test_process_group_needs_cells_mode():
         tg.map_cells_to_space(ad_sc, ad_sp, mode="clusters", cluster_label="lab", process_group=object())
 
 
-def test_bench_reference_arm_runs_the_unmodified_reference_on_the_host():
-    """`bench.py --impl reference`: the unmodified reference Mapper (oracle/_ref or the reference tree) on the host cores, full
-    workload, bounded epochs; the JSON line carries what was actually run."""
+def test_bench_reference_arm_runs_the_unmodified_reference_on_the_host(tmp_path):
+    """`bench.py --impl reference`: the reference Mapper that oracle/build_ref.load() runs (the copy in oracle/_ref, else the
+    Tangram checkout; where neither exists, the oracle stand-in of tests.helpers) on the host cores, full workload, bounded
+    epochs; the JSON line carries what was actually run, down to the sha256 of the file."""
+    import hashlib
     import json
     import os
     import subprocess
     import sys
-    from tests.helpers import REFERENCE_FILE
-    if not os.path.exists(REFERENCE_FILE):
-        pytest.skip("reference file not available (oracle/build_ref.py)")
+    from oracle import build_ref
+    from tests.helpers import standin_checkout
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ)
+    expected = build_ref.source()
+    if expected is None:
+        env["TANGRAM_REFERENCE"] = standin_checkout(tmp_path)
+        path = os.path.join(env["TANGRAM_REFERENCE"], "tangram", "mapping_optimizer.py")
+        expected = {"path": path, "sha256": hashlib.sha256(open(path, "rb").read()).hexdigest()}
     res = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--impl", "reference", "--workload", "tiny", "--steps", "5",
-                          "--warmup", "3"], capture_output=True, text=True, timeout=300)
+                          "--warmup", "3"], capture_output=True, text=True, timeout=300, env=env)
     assert res.returncode == 0, res.stderr[-2000:]
     line = json.loads(res.stdout.strip().splitlines()[-1])
     assert line["impl"] == "reference" and line["metric"] == "map_cells_to_space iterations/sec" and line["unit"] == "iterations/s"
@@ -210,16 +217,23 @@ def test_bench_reference_arm_runs_the_unmodified_reference_on_the_host():
     assert abs(line["value"] - 1e3 / line["ms_per_step"]) < 1e-6 * line["value"]
     assert line["e2e"] == {"value": line["value"], "unit": "iterations/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     assert line["config"]["cells"] == 300 and "unmodified reference" in line["cpu_baseline"]["sample"]
+    assert line["cpu_baseline"]["source"] == expected
 
 
-def test_oracle_ref_recipe_is_a_verbatim_copy():
-    """oracle/build_ref.py: oracle/_ref/mapping_optimizer.py is the reference file byte for byte (sha256 in SOURCE.txt) and loads
-    as a module with the reference's two classes."""
+def test_oracle_ref_recipe_is_a_verbatim_copy(tmp_path, monkeypatch):
+    """oracle/build_ref.py: the copy is the checkout's tangram/mapping_optimizer.py byte for byte (sha256 in SOURCE.txt) and
+    loads as a module with the reference's two classes.  The copy goes to tmp_path instead of oracle/_ref."""
     import hashlib
     import os
     from oracle import build_ref
-    if not os.path.exists(build_ref.REF_SRC) and not os.path.exists(build_ref.REF_DST):
-        pytest.skip("neither the reference tree nor a copy is present")
+    from tests.helpers import standin_checkout
+    src = build_ref.REF_SRC if os.path.exists(build_ref.REF_SRC) else \
+        os.path.join(standin_checkout(tmp_path / "checkout"), "tangram", "mapping_optimizer.py")
+    dst_dir = str(tmp_path / "_ref")
+    monkeypatch.setattr(build_ref, "REF_SRC", src)
+    monkeypatch.setattr(build_ref, "REF_DIR", dst_dir)
+    monkeypatch.setattr(build_ref, "REF_DST", os.path.join(dst_dir, "mapping_optimizer.py"))
+    monkeypatch.setattr(build_ref, "STAMP", os.path.join(dst_dir, "SOURCE.txt"))
     path = build_ref.build()
     assert path == build_ref.REF_DST and os.path.exists(path)
     digest = hashlib.sha256(open(path, "rb").read()).hexdigest()
@@ -228,23 +242,6 @@ def test_oracle_ref_recipe_is_a_verbatim_copy():
         assert open(path, "rb").read() == open(build_ref.REF_SRC, "rb").read()
     mod = build_ref.load()
     assert hasattr(mod, "Mapper") and hasattr(mod, "MapperConstrained")
-
-
-def test_profiles_traffic_json_matches_the_committed_ncu_capture():
-    """bench.py's roofline.traffic comes from profiles/traffic.json, which tools/ncu_traffic.py derives from the committed raw
-    `ncu --set full` page: re-derive it and compare (DRAM bytes of the streaming update = its algorithmic 24 B/element)."""
-    import csv
-    import json
-    import os
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    traffic = json.load(open(os.path.join(root, "profiles", "traffic.json")))["c3/bf16"]
-    rows = list(csv.reader(open(os.path.join(root, traffic["_source"]))))
-    hdr, units = rows[0], rows[1]
-    ki, ri, wi = hdr.index("Kernel Name"), hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-    scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-    per_launch = [float(r[ri]) * scale[units[ri]] + float(r[wi]) * scale[units[wi]] for r in rows[2:] if "k_adam_rows" in r[ki]]
-    assert per_launch and abs(4 * np.mean(per_launch) - traffic["adam_rows"]) < 1e-6 * traffic["adam_rows"]
-    assert abs(traffic["adam_rows"] - 24.0 * 100_000 * 10_000) < 0.02 * 24e9          # nothing is re-read
 
 
 def test_nccl_comm_cache_ignores_non_nccl_groups():

@@ -1,4 +1,4 @@
-"""The reference's own known-answer test for this path (/root/reference/tests/tangram_test.py:67-103):
+"""The reference's own known-answer test for this path (Tangram's tests/tangram_test.py:67-103):
 map_cells_to_space(mode='clusters', cluster_label='subclass_label', random_state=42, num_epochs=500) on
 data/test_ad_sc.h5ad x data/test_ad_sp.h5ad must give round(ad_map.X[0,0], 3) == round(e, 3) for nine
 hyper-parameter sets.  The inputs (cluster-aggregated S, G, priors) are committed as tests/golden/kat_clusters.npz

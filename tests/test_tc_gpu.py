@@ -1,4 +1,4 @@
-"""The tcgen05 / TMA tensor-core path (precision="bf16") against the fp32 path and the oracle.
+"""The wgmma / TMA tensor-core path (precision="bf16") against the fp32 path and the oracle.
 bf16 operands carry 2^-9 relative rounding, so buffers agree to ~1e-3 and the loss trajectory to
 ~1e-4 (SURVEY.md 7.3: bf16 operands give 3.6e-5 on the loss trajectory)."""
 import numpy as np

@@ -1,5 +1,5 @@
-"""Dev tool: a few iterations of every precision mode at shapes that hit the CTA-pair backward kernels (ragged in both
-dimensions, second CTA of the last pair fully out of range) and the single-CTA kernels -- for compute-sanitizer memcheck.
+"""Dev tool: a few iterations of every precision mode at shapes that hit the tensor-core kernels ragged in both
+dimensions (last row tile partly out of range) -- for compute-sanitizer memcheck.
 With TGB200_CHUNKS=2 in the environment the 2100-cell case also runs the chunked three-stream pipeline (store-only backward
 contraction per chunk, streaming Adam on the update stream, next forward's chunks on the third stream).
 `python tools/san_small.py rows` runs only the row-pass cases: one row width in every threads x slots bucket of
