@@ -217,7 +217,9 @@ TGB200_API int tgb200_profile_step(tgb200_mapper* h, float learning_rate, void* 
 TGB200_API int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, double* flops);
 
 /* Diagnostics: copy an internal device buffer to HOST memory after a step.  name: "Y" (V x Ke),
- * "dY" (V x Ke), "rdot" (n_cells), "Sx" (n_cells x Ke), "shape" (Ke, ld, fwd_splits, r_parts).
+ * "dY" (V x Ke), "rdot" (n_cells), "Sx" (n_cells x Ke), "shape" (Ke, ld, fwd_splits, r_parts); bf16 mode
+ * only: "Pb" (n_cells x ld, the resident unnormalised P the next backward consumes), "dq" (n_cells x ld, the
+ * backward's centred dP), "rcenter" (n_cells, the centre dq is stored relative to); bf16 buffers widened to float.
  * out_host may be NULL to query the size (*n). */
 TGB200_API int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* out_host, int64_t cap, int64_t* n);
 

@@ -1,6 +1,6 @@
 // wgmma / TMA tensor-core contraction path (sm_90a): bf16 operands staged in shared memory by
 // TMA (128B swizzle), wgmma.mma_async issued by two consumer warpgroups, fp32 accumulators in
-// registers, fused epilogues straight from the accumulator fragments.
+// registers, fused epilogues on the accumulator fragments (the bf16 backward's through a shared-memory tile).
 //
 //   forward   Y_ext[z] = P[z]^T S_ext[z]        A = P  (MN-major), B = S_ext (MN-major), split over cells / cell chunks
 //   backward  dP = S_ext dY_ext^T  -> stored (bf16 centred / fp32) + row-dot partials in the epilogue (A, B K-major).
@@ -62,6 +62,31 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+// shared -> global tensor store, completion tracked by the issuing thread's bulk groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
+      ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the committed stores have finished reading shared memory (their global writes may still be in flight)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// generic-proxy writes to shared memory become visible to the async proxy (TMA) of this CTA
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+template <int ID>
+__device__ __forceinline__ void named_bar_sync(int threads) {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(threads) : "memory");
+}
+// four 8 x 8 b16 matrices; lane l addresses row (l % 8) of matrix l / 8 and receives, from every matrix, the two
+// elements of row l / 4, columns 2 (l % 4), +1 -- the wgmma accumulator fragment layout
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
 }
 
 // register budget of the two roles (warpgroup-wide): 128 x 40 + 256 x 232 <= 64K registers
@@ -151,6 +176,15 @@ struct OperandTile {
 // are columns (8j + 2 (lane % 4), +1) of row `row`, and d[4j+2], d[4j+3] the same columns of row `row + 8`.  A quad of
 // lanes covers 8 consecutive columns of a row (one 32-byte sector of fp32).  prologue() is called by all 256 consumer
 // threads (`ct`) before the tile's main loop.
+// An epilogue may also own kSmemBytes of shared memory after the operand ring (EpiSmem).  load() is then called by the
+// producer thread once per tile, after the tile's first STAGES k-blocks have been handed to the ring, to fill it.
+// Each consumer warpgroup `cw` owns one full / free mbarrier pair for its half; `parity` is the tile's phase of both.
+struct EpiSmem {
+  uint8_t* buf;          // 1024-byte aligned
+  uint64_t* full;        // [2] arrive count 1 + transaction bytes: the producer's load of half cw has landed
+  uint64_t* free;        // [2] arrive count 1: consumer warpgroup cw no longer needs its half
+  uint32_t parity;
+};
 // Work item w -> (row tile m, column tile n).  Row tiles are taken in groups of `group_m`; inside a group the order is
 // column-major (all rows of the group for column 0, then column 1, ...).  The CTAs running at the same time then cover
 // the whole group for a few columns: the group's A rows (group_m x 128 x K, re-read for every column) are a small,
@@ -176,10 +210,12 @@ __device__ __forceinline__ float quad_sum(float v) {
 }
 
 struct TcEpiStore {
+  static constexpr int kSmemBytes = 0;
   float* C; int ldc; size_t split_stride; int M;
   int accumulate;        // 1: C += tile (cell chunks of the pipelined forward run one after the other: fixed summation order)
   __device__ __forceinline__ void prologue(const TileCoord&, int) const {}
-  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane) const {
+  __device__ __forceinline__ void load(int, int, const EpiSmem&) const {}
+  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane, int, const EpiSmem&) const {
     float* base = C + (size_t)t.split * split_stride;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -203,42 +239,83 @@ struct TcEpiStore {
 // bf16, centred per row on the previous iteration's row-dot (dq_ij = bf16(dP_ij - c_i): the softmax-Jacobian only sees
 // dP_ij - r_i, so the bf16 rounding is relative to the deviation from the row mean, not to dP itself), and the same
 // epilogue accumulates this iteration's row-dot partials r'_i = sum_j Pt_ij dq_ij from the ROUNDED values (so that
-// sum_j g_ij = 0 holds for what the streaming Adam kernel consumes).  The Pt segment of the tile is prefetched into L2
-// before the main loop.
+// sum_j g_ij = 0 holds for what the streaming Adam kernel consumes).
+// The tile's Pt comes in by TMA during the main loop, into a 128 x 256 bf16 shared-memory tile (per 64-row half four
+// 64 x 64 boxes of 8 KB, 128-byte swizzle); the epilogue reads it with ldmatrix, writes dq over it with stmatrix and
+// each consumer warpgroup stores its half with TMA.  Both streams use evict_first: they pass through L2 once, beside the
+// dY_ext operand that every tile re-reads.
 struct TcEpiDpStore {
-  __nv_bfloat16* dq; const __nv_bfloat16* Pt; int ld;     // both [rows][ld]
+  static constexpr int kSmemBytes = TC_BM * TC_BN * 2;
+  static constexpr int kHalfBytes = kSmemBytes / 2;
+  static constexpr int kBoxBytes = 64 * 128;
+  CUtensorMap pt_map, dq_map;                             // Pt / dq [M][ld] bf16, box {64 columns, 64 rows}
+  int ld;                                                 // a multiple of 64
   const float* center;                                    // c_i (per row)
   float* rpart;                                           // [tiles_n][M]
   int M;
-  __device__ __forceinline__ void prologue(const TileCoord& t, int ct) const {
-#pragma unroll
-    for (int i = ct; i < TC_BM * (TC_BN / 64); i += 256) {      // 128-byte lines of the tile's Pt block
-      const int row = t.m0 + (i >> 2), col = t.n0 + (i & 3) * 64;
-      if (row < M && col < ld) prefetch_l2(Pt + (size_t)row * ld + col);
-    }
-  }
-  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane) const {
+  // boxes of the 64-row half starting at row r0 that hold data; with ld a multiple of 64 a box lies wholly inside
+  // [0, ld) or wholly past it, and TMA clips the rows >= M of a partly filled one
+  __device__ __forceinline__ int boxes(int r0, int n0) const { return r0 < M ? min(TC_BN / 64, (ld - n0) / 64) : 0; }
+  __device__ __forceinline__ void prologue(const TileCoord&, int) const {}
+  __device__ __forceinline__ void load(int m0, int n0, const EpiSmem& es) const {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int r = row + 8 * h;
-      const bool live = r < M;
-      const float c = live ? center[r] : 0.f;
-      const __nv_bfloat16* prow = Pt + (size_t)r * ld;
-      __nv_bfloat16* drow = dq + (size_t)r * ld;
-      float racc = 0.f;
+      mbar_wait(&es.free[h], es.parity ^ 1);
+      const int nb = boxes(m0 + 64 * h, n0);
+      mbar_expect_tx(&es.full[h], nb * kBoxBytes);
+      for (int b = 0; b < nb; ++b)
+        tma_load_2d(&pt_map, &es.full[h], es.buf + h * kHalfBytes + b * kBoxBytes, n0 + 64 * b, m0 + 64 * h, kPolicyEvictFirst);
+    }
+  }
+  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane, int cw,
+                                      const EpiSmem& es) const {
+    const int r0 = t.m0 + 64 * cw;
+    const int nb = boxes(r0, t.n0);
+    float c[2];
 #pragma unroll
-      for (int j = 0; j < TC_BN / 8; ++j) {
-        const int col = t.n0 + 8 * j + 2 * (lane & 3);
-        if (live && col < ld) {
-          const __nv_bfloat162 d2 = __floats2bfloat162_rn(d[4 * j + 2 * h] - c, d[4 * j + 2 * h + 1] - c);
-          const __nv_bfloat162 p2 = *reinterpret_cast<const __nv_bfloat162*>(prow + col);
-          racc = fmaf(__low2float(p2), __low2float(d2), racc);
-          racc = fmaf(__high2float(p2), __high2float(d2), racc);
-          *reinterpret_cast<__nv_bfloat162*>(drow + col) = d2;
+    for (int h = 0; h < 2; ++h) c[h] = row + 8 * h < M ? center[row + 8 * h] : 0.f;
+    // ldmatrix / stmatrix address of this lane: row (lane % 8) of matrix lane / 8, where matrices 0..3 are
+    // (rows +0, columns 8j), (rows +8, 8j), (rows +0, 8j + 8), (rows +8, 8j + 8) of the warp's 16 rows
+    const int mi = lane >> 3, rr = lane & 7;
+    const int arow = ((row - r0) & ~15) + 8 * (mi & 1) + rr;
+    const uint32_t half = smem_u32(es.buf + cw * kHalfBytes) + arow * 128;
+    mbar_wait(&es.full[cw], es.parity);
+    float racc[2] = {0.f, 0.f};
+#pragma unroll
+    for (int b = 0; b < TC_BN / 64; ++b) {
+      if (b >= nb) break;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {                       // columns 64 b + 16 q .. +16: j = 8 b + 2 q, +1
+        const uint32_t addr = half + b * kBoxBytes + (((2 * q + (mi >> 1)) ^ rr) << 4);
+        uint32_t p[4], o[4];
+        ldmatrix_x4(addr, p);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int j = 8 * b + 2 * q + e;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const __nv_bfloat162 d2 = __floats2bfloat162_rn(d[4 * j + 2 * h] - c[h], d[4 * j + 2 * h + 1] - c[h]);
+            const __nv_bfloat162 p2 = *reinterpret_cast<const __nv_bfloat162*>(&p[2 * e + h]);
+            racc[h] = fmaf(__low2float(p2), __low2float(d2), racc[h]);
+            racc[h] = fmaf(__high2float(p2), __high2float(d2), racc[h]);
+            o[2 * e + h] = *reinterpret_cast<const uint32_t*>(&d2);
+          }
         }
+        stmatrix_x4(addr, o);
       }
-      racc = quad_sum(racc);
-      if (live && (lane & 3) == 0) rpart[(size_t)t.tile_n * M + r] = racc;
+    }
+    fence_proxy_async_smem();
+    if (cw == 0) named_bar_sync<1>(128); else named_bar_sync<2>(128);    // this warpgroup's stmatrix writes are done
+    if ((threadIdx.x & 127) == 0) {
+      for (int b = 0; b < nb; ++b) tma_store_2d(&dq_map, es.buf + cw * kHalfBytes + b * kBoxBytes, t.n0 + 64 * b, r0, kPolicyEvictFirst);
+      bulk_commit();
+      bulk_wait_read_all();                               // the half may be refilled once the stores have read it
+      mbar_arrive(&es.free[cw]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float s = quad_sum(racc[h]);
+      if (row + 8 * h < M && (lane & 3) == 0) rpart[(size_t)t.tile_n * M + row + 8 * h] = s;
     }
   }
 };
@@ -246,6 +323,7 @@ struct TcEpiDpStore {
 // The same store-only backward for the parity mode (bf16x3): dP leaves the kernel in fp32 (nothing to centre) and the
 // row-dot partials use P reconstructed from its three bf16 planes (hi + mid + lo = the fp32 value the row pass computed).
 struct TcEpiDpStoreF32 {
+  static constexpr int kSmemBytes = 0;
   float* dp; int ld;                       // [rows][ld] fp32
   const __nv_bfloat16* P3; size_t plane;   // three planes of [rows][ld] bf16
   float* rpart;                            // [tiles_n][M]
@@ -258,7 +336,8 @@ struct TcEpiDpStoreF32 {
       if (row < M && col < ld) prefetch_l2(P3 + pl * plane + (size_t)row * ld + col);
     }
   }
-  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane) const {
+  __device__ __forceinline__ void load(int, int, const EpiSmem&) const {}
+  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane, int, const EpiSmem&) const {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = row + 8 * h;
@@ -312,7 +391,7 @@ template <bool A_KMAJOR, bool B_KMAJOR, int STAGES, class Epi>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps maps_b, int n_pairs,
           int k_total, int k_per_split, int tiles_m, int tiles_n, int splits, int group_m, uint64_t policy_a,
-          uint64_t policy_b, int tm_off, int k_off, const Epi epi) {
+          uint64_t policy_b, int tm_off, int k_off, const __grid_constant__ Epi epi) {
   using TileA = OperandTile<A_KMAJOR, TC_BM>;
   using TileB = OperandTile<B_KMAJOR, TC_BN>;
   constexpr int kStageBytes = TileA::kBytes + TileB::kBytes;
@@ -323,15 +402,20 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
+  __shared__ __align__(8) uint64_t epi_full[2], epi_free[2];
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int total = tiles_m * tiles_n * splits;
+  EpiSmem es{smem + STAGES * kStageBytes, epi_full, epi_free, 0};
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps_a.m[0]);
     tma_prefetch_desc(&maps_b.m[0]);
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+    if constexpr (Epi::kSmemBytes > 0) {
+      for (int h = 0; h < 2; ++h) { mbar_init(&epi_full[h], 1); mbar_init(&epi_free[h], 1); }
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -341,7 +425,7 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
     setmaxnreg_producer();
     if (threadIdx.x == 0) {
       uint32_t kbg = 0;                         // k-blocks issued so far (ring position)
-      for (int w = blockIdx.x; w < total; w += gridDim.x) {
+      for (int w = blockIdx.x; w < total; w += gridDim.x, es.parity ^= 1) {
         const int z = w / (tiles_n * tiles_m);
         int tm_i, tn_i;
         tile_mn(w - z * tiles_n * tiles_m, tiles_m, tiles_n, group_m, tm_i, tn_i);
@@ -362,6 +446,10 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
             const int k0 = k_begin + kb * TC_BK;
             TileA::load(ma, &full_bar[s], sa, m0, k0, policy_a);
             TileB::load(mb, &full_bar[s], sb, n0, k0, policy_b);
+#ifndef TGB_SKIP_EPI
+            // not before: waiting for the previous tile's epilogue to free its buffer would hold up the ring's prefill
+            if (Epi::kSmemBytes > 0 && pr == 6 - n_pairs && kb + 1 == min(STAGES, num_kb)) epi.load(m0, n0, es);
+#endif
           }
         }
       }
@@ -376,7 +464,7 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
 #pragma unroll
     for (int i = 0; i < TC_ACC; ++i) acc[i] = 0.f;
     uint32_t kbg = 0;
-    for (int w = blockIdx.x; w < total; w += gridDim.x) {
+    for (int w = blockIdx.x; w < total; w += gridDim.x, es.parity ^= 1) {
       TileCoord t;
       t.split = w / (tiles_n * tiles_m);
       int tm_i;
@@ -409,7 +497,7 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
       acc_fence(acc);
       if (total_kb > 0 && lane == 0) mbar_arrive(&empty_bar[(kbg - 1) % STAGES]);
 #ifndef TGB_SKIP_EPI
-      epi.run(acc, t, t.m0 + row_in_tile, lane);
+      epi.run(acc, t, t.m0 + row_in_tile, lane, cw, es);
 #endif
     }
   }
@@ -480,9 +568,19 @@ static inline int tc_check_launch(const char* name, char* err, size_t n) {
   return 0;
 }
 
-// 4 stages of 48 KB (128 x 64 A + 256 x 64 B, bf16): 193 KB of the 227 KB an H100 block may use
-constexpr int TC_STAGES = 4;
-constexpr int TC_SMEM = TC_STAGES * (TC_BM + TC_BN) * TC_BK * 2 + 1024;
+// Operand ring of up to 4 stages of 48 KB (128 x 64 A + 256 x 64 B, bf16), as many as fit beside the epilogue's buffer
+// in the 227 KB an H100 block may use (1 KB of it kept for the alignment of the dynamic buffer, 1 KB for the static
+// barriers): 4 stages (193 KB) without an epilogue buffer, 3 (209 KB) beside TcEpiDpStore's 64 KB.
+constexpr int TC_STAGE_BYTES = (TC_BM + TC_BN) * TC_BK * 2;
+constexpr int TC_SMEM_LIMIT = 227 * 1024;
+template <class Epi>
+constexpr int tc_stages() {
+  const int fit = (TC_SMEM_LIMIT - 2048 - Epi::kSmemBytes) / TC_STAGE_BYTES;
+  return fit < 4 ? fit : 4;
+}
+template <class Epi>
+constexpr int tc_smem() { return tc_stages<Epi>() * TC_STAGE_BYTES + Epi::kSmemBytes + 1024; }
+constexpr int TC_SMEM = tc_smem<TcEpiStore>();     // the forward
 static inline int tc_dp_row_parts(int V) { return (int)ceil_div(V, TC_BN); }
 // (tile_mn's row-tile groups stay at 1: more CTAs pulling the same B tile at once hot-spot L2 slices.)
 static inline int tc_splits(int num_sms, long long tiles, long long k_total, int min_k) {
@@ -527,6 +625,7 @@ static inline int tc_make_maps(TcContext& tc, TcMaps* maps, const __nv_bfloat16*
 // encodes each plan once (the buffers never move) instead of on every launch.
 struct TcPlan {
   TcMaps a, b;
+  CUtensorMap pt, dq;     // bf16 store-only backward: its epilogue's Pt input and dq output
   bool ready = false;
 };
 
@@ -540,7 +639,7 @@ static inline int tc_forward_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16
 }
 static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int N, int V, int Ke, int splits,
                                     cudaStream_t s, char* err, size_t n) {
-  auto kern = k_gemm_tc<false, false, TC_STAGES, TcEpiStore>;
+  auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
   if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, 0};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
@@ -552,7 +651,7 @@ static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs
 // behind the streaming Adam kernel; the chunks run one after the other on one stream, so the summation order is fixed
 static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, float* out, int accumulate, int row0, int row1, int V, int Ke,
                                          cudaStream_t s, char* err, size_t n) {
-  auto kern = k_gemm_tc<false, false, TC_STAGES, TcEpiStore>;
+  auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
   if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, accumulate};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
@@ -579,15 +678,22 @@ static inline int tc_dpstore_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16
   pl.ready = true;
   return 0;
 }
+// TcEpiDpStore's Pt and dq, both [N][ld] bf16, in 64 x 64 boxes
+static inline int tc_dpstore_epi_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16* Pt, const __nv_bfloat16* dq, int N, int ld,
+                                      char* err, size_t n) {
+  if (tc_make_map(tc, &pl.pt, Pt, ld, N, ld, 64, 64, err, n)) return -2;
+  return tc_make_map(tc, &pl.dq, dq, ld, N, ld, 64, 64, err, n);
+}
 template <class Epi>
 static inline int tc_dpstore_launch(TcContext& tc, const TcPlan& pl, int n_pairs, const Epi& epi, int row0, int row1, int V, int Ke,
                                     cudaStream_t s, char* err, size_t n) {
   const int tn = (int)ceil_div(V, TC_BN);
-  auto kern = k_gemm_tc<true, true, TC_STAGES, Epi>;
-  if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
+  auto kern = k_gemm_tc<true, true, tc_stages<Epi>(), Epi>;
+  constexpr int smem = tc_smem<Epi>();
+  if (tc_set_smem(tc, kern, smem, err, n)) return -2;
   const int tm0 = row0 / TC_BM, tm = (int)ceil_div(row1, TC_BM) - tm0;
-  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
-                                                                    kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
+  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, smem, s>>>(pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
+                                                                 kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
   return tc_check_launch("tc_gemm_bwd_dp", err, n);
 }
 

@@ -941,13 +941,15 @@ static int filter_update(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
 // Staged backward (bf16 mode): dq = bf16(S_ext dY_ext^T - centre) + row-dot partials from the store-only contraction,
 // then one streaming pass does softmax-Jacobian + Adam + the next forward's P.  (mapping_optimizer.py:395-396)
 static int backward_staged(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, const AdamScalars& a) {
-  if (!h->plan_dp.ready)
+  if (!h->plan_dp.ready) {
+    CKS(tc_dpstore_epi_plan(h->tc, h->plan_dp, h->Pb.p, h->dq.p, h->N, h->ld, g_err, sizeof(g_err)));
     CKS(tc_dpstore_plan(h->tc, h->plan_dp, h->Sxb.p, 0, h->dYb.p, 0, 1, h->N, h->V, h->Ke, g_err, sizeof(g_err)));
+  }
   const bool two_streams = su != s;
   const bool prefetch = two_streams && h->prefetch_next && h->nchunks > 1 && !h->constrained;
   for (int c = 0; c < h->nchunks; ++c) {
     const int r0 = h->nchunks > 1 ? h->chunk_row[c] : 0, r1 = h->nchunks > 1 ? h->chunk_row[c + 1] : h->N;
-    TcEpiDpStore epi{h->dq.p, h->Pb.p, h->ld, h->rcenter.p, h->rpart.p, h->N};
+    TcEpiDpStore epi{h->plan_dp.pt, h->plan_dp.dq, h->ld, h->rcenter.p, h->rpart.p, h->N};
     CKS(tc_dpstore_launch(h->tc, h->plan_dp, 1, epi, r0, r1, h->V, h->Ke, s, g_err, sizeof(g_err)));
     mark(h, s, "tc_gemm_bwd_dp");
     if (two_streams) {
@@ -1487,6 +1489,18 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
       return TGB200_OK;
     }
   }
+  else if ((nm == "dq" && h->staged) || (nm == "Pb" && h->bf16)) {    // N x ld bf16, widened
+    cnt = (int64_t)h->N * h->ld;
+    *n = cnt;
+    if (out_host) {
+      if (cap < cnt) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)cnt);
+      std::vector<__nv_bfloat16> tmp((size_t)cnt);
+      CK(cudaMemcpy(tmp.data(), nm == "dq" ? h->dq.p : h->Pb.p, (size_t)cnt * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
+      for (int64_t i = 0; i < cnt; ++i) out_host[i] = __bfloat162float(tmp[(size_t)i]);
+    }
+    return TGB200_OK;
+  }
+  else if (nm == "rcenter" && h->staged) { src = h->rcenter.p; cnt = h->N; }
   else if (nm == "rdot") { src = h->rdot.p; cnt = h->N; }
   else if (nm == "Sx") { src = h->Sx.p; cnt = (int64_t)h->N * h->Ke; }
   else if (nm == "shape") {   // Ke, ld, fwd_splits, r_parts
