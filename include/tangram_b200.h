@@ -140,6 +140,29 @@ TGB200_API int tgb200_init_mapping_normal(tgb200_mapper* h, uint64_t seed, void*
  * cell does not depend on how the cells are sharded over ranks (tgb200_init_mapping_normal == first_row 0). */
 TGB200_API int tgb200_init_mapping_normal_rows(tgb200_mapper* h, uint64_t seed, int64_t first_row, void* stream);
 
+/* State of numpy's legacy generator, as np.random.get_state() returns it:
+ * ('MT19937', key[624], pos, has_gauss, cached_gaussian). */
+typedef struct tgb200_mt_state {
+  uint32_t key[624];
+  int32_t pos;          /* 0 .. 624 */
+  int32_t has_gauss;    /* 0 or 1 */
+  double gauss;
+} tgb200_mt_state;
+
+/* The reference's initial draw on the device, bit for bit: M = float32(np.random.normal(0, 1, (n_rows, n_voxels))) after
+ * np.random.seed (:147-157), from the generator state `start`.  The handle receives rows [first_row, first_row + n_cells)
+ * of a draw that begins `skip` normals into the stream (MapperConstrained discards a first draw of N x V: skip = N V,
+ * :472-493); pad columns are zero.  `end_out` (may be NULL) receives the generator state after `end_normal` normals of the
+ * stream, as numpy leaves it after the host draw (end_normal >= skip + (first_row + n_cells) n_voxels).  The few values
+ * whose float32 rounding could depend on the last bit of log are recomputed on the host with libm's log, as numpy does;
+ * *n_fixed_out (may be NULL) is their number.  Resets the Adam state like tgb200_set_mapping.  Synchronous. */
+TGB200_API int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_state* start, int64_t skip, int64_t first_row,
+                                          int64_t end_normal, tgb200_mt_state* end_out, int64_t* n_fixed_out, void* stream);
+/* Host only, no device: the state after n_words more 32-bit words (numpy's state after random_raw(n_words)); has_gauss and
+ * gauss are copied.  tgb200_mt19937_jump_pow2 jumps by 2^log2_words words, log2_words <= 128. */
+TGB200_API int tgb200_mt19937_jump(const tgb200_mt_state* in, uint64_t n_words, tgb200_mt_state* out);
+TGB200_API int tgb200_mt19937_jump_pow2(const tgb200_mt_state* in, uint32_t log2_words, tgb200_mt_state* out);
+
 /* A fresh optimizer on the current mapping: what every Mapper.train call does when it builds torch.optim.Adam([M])
  * anew (:373, :607) -- zero moments, bias correction restarts at t = 1.  M, F, the history and its length are kept. */
 TGB200_API int tgb200_reset_adam(tgb200_mapper* h, void* stream);
@@ -220,6 +243,8 @@ TGB200_API int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, doub
  * "dY" (V x Ke), "rdot" (n_cells), "Sx" (n_cells x Ke), "shape" (Ke, ld, fwd_splits, r_parts); bf16 mode
  * only: "Pb" (n_cells x ld, the resident unnormalised P the next backward consumes), "dq" (n_cells x ld, the
  * backward's centred dP), "rcenter" (n_cells, the centre dq is stored relative to); bf16 buffers widened to float.
+ * "legacy_init": the last tgb200_init_mapping_legacy's ms of jump, count + scan, emit and fix-up (CUDA events), ms of host
+ * polynomial work, draw blocks, values recomputed on the host, values that recomputation changed.
  * out_host may be NULL to query the size (*n). */
 TGB200_API int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* out_host, int64_t cap, int64_t* n);
 

@@ -30,6 +30,27 @@ class Config(ctypes.Structure):
     ]
 
 
+class MtState(ctypes.Structure):
+    """tgb200_mt_state: numpy's legacy generator state, np.random.get_state()[1:]."""
+    _fields_ = [("key", ctypes.c_uint32 * 624), ("pos", ctypes.c_int32), ("has_gauss", ctypes.c_int32),
+                ("gauss", ctypes.c_double)]
+
+    @classmethod
+    def from_numpy(cls, state):
+        """From np.random.get_state() (or RandomState.get_state()): ('MT19937', key, pos, has_gauss, cached_gaussian)."""
+        name, key, pos, has_gauss, gauss = state
+        if name != "MT19937":
+            raise ValueError(f"not an MT19937 state: {name!r}")
+        st = cls()
+        np.ctypeslib.as_array(st.key)[:] = np.asarray(key, dtype=np.uint32)
+        st.pos, st.has_gauss, st.gauss = int(pos), int(has_gauss), float(gauss)
+        return st
+
+    def to_numpy(self):
+        """-> the tuple np.random.set_state() takes."""
+        return ("MT19937", np.ctypeslib.as_array(self.key).copy(), int(self.pos), int(self.has_gauss), float(self.gauss))
+
+
 class TangramB200Error(RuntimeError):
     pass
 
@@ -50,6 +71,10 @@ SIGNATURES = {
     "tgb200_set_mapping": (ctypes.c_int, [_P, _P, _P]),
     "tgb200_init_mapping_normal": (ctypes.c_int, [_P, ctypes.c_uint64, _P]),
     "tgb200_init_mapping_normal_rows": (ctypes.c_int, [_P, ctypes.c_uint64, ctypes.c_int64, _P]),
+    "tgb200_init_mapping_legacy": (ctypes.c_int, [_P, ctypes.POINTER(MtState), ctypes.c_int64, ctypes.c_int64,
+                                                  ctypes.c_int64, ctypes.POINTER(MtState), _I64, _P]),
+    "tgb200_mt19937_jump": (ctypes.c_int, [ctypes.POINTER(MtState), ctypes.c_uint64, ctypes.POINTER(MtState)]),
+    "tgb200_mt19937_jump_pow2": (ctypes.c_int, [ctypes.POINTER(MtState), ctypes.c_uint32, ctypes.POINTER(MtState)]),
     "tgb200_reset_adam": (ctypes.c_int, [_P, _P]),
     "tgb200_set_filter": (ctypes.c_int, [_P, _P, _P]),
     "tgb200_get_filter": (ctypes.c_int, [_P, _P, _P, _P]),

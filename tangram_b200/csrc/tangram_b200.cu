@@ -2,11 +2,13 @@
 // Host orchestration only; every kernel is hand-written for sm_90a (H100) in the .cuh files.
 #include "../../include/tangram_b200.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
@@ -16,6 +18,8 @@
 #include "gemm_simt.cuh"
 #include "gemm_tc.cuh"
 #include "adam_rows.cuh"
+#include "legacy_rng.cuh"
+#include "mt19937_jump.h"
 #include "nccl_dl.h"
 
 using namespace tgb;
@@ -122,6 +126,9 @@ struct tgb200_mapper {
   bool have_expr = false, have_density = false, have_ct = false, have_mapping = false;
   bool in_step = false;
   int64_t launches = 0;
+  // last tgb200_init_mapping_legacy: ms of jump, count + scan, emit, fix-up (device, CUDA events), host polynomials,
+  // then draw blocks, values recomputed on the host, values the recomputation changed
+  float legacy_stats[8] = {0};
   KernelTimer* timer = nullptr;
   TcContext tc;                 // driver entry points etc. for the wgmma path
   TcPlan plan_fwd, plan_dp;     // tensor maps of the two contractions, encoded once (the buffers never move)
@@ -658,6 +665,240 @@ extern "C" int tgb200_init_mapping_normal_rows(tgb200_mapper* h, uint64_t seed, 
   LAUNCH_CHECK("init_normal");
   CKS(reset_optimizer(h, s));
   h->have_mapping = true;
+  return TGB200_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// numpy's legacy normal stream on the device (legacy_rng.cuh; skip-ahead in mt19937_jump.h)
+
+static bool valid_mt_state(const tgb200_mt_state* st) {
+  return st->pos >= 0 && st->pos <= mtj::kN && (st->has_gauss == 0 || st->has_gauss == 1);
+}
+
+extern "C" int tgb200_mt19937_jump(const tgb200_mt_state* in, uint64_t n_words, tgb200_mt_state* out) {
+  if (!in || !out) return fail(TGB200_ERR_INVALID, "null argument");
+  if (!valid_mt_state(in)) return fail(TGB200_ERR_INVALID, "bad generator state (pos %d, has_gauss %d)", in->pos, in->has_gauss);
+  if (!mtj::field().ok()) return fail(TGB200_ERR_STATE, "MT19937 characteristic polynomial not found");
+  tgb200_mt_state r = *in;
+  if (n_words) mtj::jump(in->key, in->pos, (unsigned __int128)n_words - 1, r.key, &r.pos);
+  *out = r;
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_mt19937_jump_pow2(const tgb200_mt_state* in, uint32_t log2_words, tgb200_mt_state* out) {
+  if (!in || !out) return fail(TGB200_ERR_INVALID, "null argument");
+  if (!valid_mt_state(in)) return fail(TGB200_ERR_INVALID, "bad generator state (pos %d, has_gauss %d)", in->pos, in->has_gauss);
+  if (log2_words > 128) return fail(TGB200_ERR_INVALID, "log2_words > 128");
+  if (!mtj::field().ok()) return fail(TGB200_ERR_STATE, "MT19937 characteristic polynomial not found");
+  const unsigned __int128 n_minus_1 = log2_words == 128 ? ~(unsigned __int128)0 : ((unsigned __int128)1 << log2_words) - 1;
+  tgb200_mt_state r = *in;
+  mtj::jump(in->key, in->pos, n_minus_1, r.key, &r.pos);
+  *out = r;
+  return TGB200_OK;
+}
+
+// numpy's legacy_gauss on the four words of one accepted attempt, with libm's log and sqrt: the value numpy computes in
+// this process.  comp 0 is f x2 (returned first), 1 is f x1 (cached).  The squares go through volatile temporaries so
+// that no compiler contracts x1 x1 + x2 x2 into an FMA; every other product is exact or cannot be contracted.
+static double polar_value_host(const uint32_t w[4], int comp) {
+  const double d1 = ((w[0] >> 5) * 67108864.0 + (w[1] >> 6)) / 9007199254740992.0;
+  const double d2 = ((w[2] >> 5) * 67108864.0 + (w[3] >> 6)) / 9007199254740992.0;
+  const double x1 = 2.0 * d1 - 1.0, x2 = 2.0 * d2 - 1.0;
+  volatile double s1 = x1 * x1, s2 = x2 * x2;
+  const double r2 = s1 + s2;
+  const double f = std::sqrt(-2.0 * std::log(r2) / r2);
+  return f * (comp ? x1 : x2);
+}
+
+// Jump polynomials of the device draw, computed once per process and kept: [0] x^(L - 624), [1 + j] x^(2^j L) for the
+// draw-block length L.  *ms: host time spent here (phi included when this call found it).
+static int legacy_polys(int levels, std::vector<uint64_t>& flat, double* ms) {
+  static std::mutex mu;
+  static std::vector<std::vector<uint64_t>> polys;
+  std::lock_guard<std::mutex> lock(mu);
+  const auto t0 = std::chrono::steady_clock::now();
+  const mtj::Field& F = mtj::field();
+  if (!F.ok()) return fail(TGB200_ERR_STATE, "MT19937 characteristic polynomial not found");
+  if (polys.empty()) {
+    polys.push_back(F.x_pow(lrng::kWordsPerCta - lrng::kN));
+    polys.push_back(F.x_pow(lrng::kWordsPerCta));
+  }
+  while ((int)polys.size() < 1 + levels) {
+    std::vector<uint64_t> p = polys.back();
+    F.square(p);
+    polys.push_back(std::move(p));
+  }
+  flat.clear();
+  for (int i = 0; i < 1 + levels; ++i) flat.insert(flat.end(), polys[i].begin(), polys[i].end());
+  *ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  return TGB200_OK;
+}
+
+struct EventSet {
+  cudaEvent_t e[5] = {};
+  ~EventSet() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+  float ms(int a, int b) const { float t = 0.f; cudaEventElapsedTime(&t, e[a], e[b]); return t; }
+};
+
+extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_state* start, int64_t skip, int64_t first_row,
+                                          int64_t end_normal, tgb200_mt_state* end_out, int64_t* n_fixed_out, void* stream) {
+  using namespace lrng;
+  if (!h || !start) return fail(TGB200_ERR_INVALID, "null argument");
+  if (!valid_mt_state(start))
+    return fail(TGB200_ERR_INVALID, "bad generator state (pos %d, has_gauss %d)", start->pos, start->has_gauss);
+  if (skip < 0 || first_row < 0) return fail(TGB200_ERR_INVALID, "skip and first_row must be >= 0");
+  const int64_t V = h->V, N = h->N;
+  const int64_t t_lo = skip + first_row * V, t_hi = t_lo + N * V;       // stream normals that land in this handle
+  if (end_normal < t_hi) return fail(TGB200_ERR_INVALID, "end_normal < skip + (first_row + n_cells) * n_voxels");
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(h->cfg.device));
+  const int hg = start->has_gauss;
+  const int64_t a_end = end_normal > hg ? (end_normal - hg + 1) / 2 - 1 : -1;   // last accepted attempt consumed
+  const int64_t a_lo = t_lo > hg ? (t_lo - hg) / 2 : 0;                        // first one this handle needs
+  float* stats = h->legacy_stats;
+  std::fill(stats, stats + 8, 0.f);
+  EventSet ev;
+  for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
+  CK(cudaMemsetAsync(h->M.p, 0, h->M.n * sizeof(float), s));
+  EndRecord end_h{-1, {0, 0, 0, 0}};
+  int64_t n_fixed = 0, n_changed = 0;
+  std::vector<float> patch_vals;
+  if (a_end >= 0) {
+    CK(cudaFuncSetAttribute(k_mt_jump, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kJumpSmem));   // per device
+    // draw blocks: the expected attempts (a_end + 1) / (pi / 4) plus 10 standard deviations; doubled if ever short
+    const double pa = 0.78539816339744831, na = (double)(a_end + 1);
+    int64_t nb = (int64_t)((na / pa + 10.0 * std::sqrt(na * (1.0 - pa)) / pa) / kAttemptsPerCta) + 2;
+    DevBuf<uint32_t> key0, starts;
+    DevBuf<uint64_t> polys;
+    DevBuf<long long> counts, offs;
+    CKS(key0.alloc(kN, false));
+    CK(cudaMemcpy(key0.p, start->key, kN * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    std::vector<long long> offs_h;
+    std::vector<uint64_t> flat;
+    for (;;) {
+      if (nb > (1LL << 30)) return fail(TGB200_ERR_INVALID, "draw of %lld normals is too large", (long long)end_normal);
+      int levels = 0;
+      while ((1LL << levels) + 1 < nb) ++levels;
+      double host_ms = 0.0;
+      CKS(legacy_polys(levels, flat, &host_ms));
+      stats[4] += (float)host_ms;
+      CKS(polys.alloc(flat.size(), false));
+      CK(cudaMemcpy(polys.p, flat.data(), flat.size() * sizeof(uint64_t), cudaMemcpyHostToDevice));
+      CKS(starts.alloc((size_t)nb * kN, false));
+      CKS(counts.alloc(nb, false));
+      CKS(offs.alloc(nb + 1, false));
+      CK(cudaEventRecord(ev.e[0], s));
+      // level -1: start 1 = the window 624 words before MT block B + kBlocksPerCta; level j: starts
+      // [1 + 2^j, 1 + 2^(j+1)) = starts [1, 1 + 2^j) jumped by 2^j draw blocks
+      if (nb > 1) {
+        CK(cudaMemcpyAsync(starts.p, key0.p, kN * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+        k_mt_jump<<<1, kN, kJumpSmem, s>>>(starts.p, starts.p + kN, polys.p);
+        LAUNCH_CHECK("mt_jump");
+        for (int j = 0; j < levels; ++j) {
+          const int64_t stride = 1LL << j, cnt = std::min<int64_t>(stride, nb - 1 - stride);
+          k_mt_jump<<<(unsigned)cnt, kN, kJumpSmem, s>>>(starts.p + kN, starts.p + (1 + stride) * kN,
+                                                          polys.p + (size_t)(1 + j) * kPolyWords);
+          LAUNCH_CHECK("mt_jump");
+        }
+      }
+      CK(cudaEventRecord(ev.e[1], s));
+      DrawParams p{};
+      p.key0 = key0.p;
+      p.starts = starts.p;
+      p.pos0 = start->pos;
+      p.counts = counts.p;
+      k_legacy_pass<false><<<(unsigned)nb, kN, 0, s>>>(p);
+      LAUNCH_CHECK("legacy_count");
+      k_scan_counts<<<1, 1024, 0, s>>>(counts.p, (int)nb, offs.p);
+      LAUNCH_CHECK("legacy_scan");
+      CK(cudaEventRecord(ev.e[2], s));
+      offs_h.resize(nb + 1);
+      CK(cudaMemcpyAsync(offs_h.data(), offs.p, (nb + 1) * sizeof(long long), cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      if (offs_h[nb] > a_end) break;
+      nb *= 2;
+    }
+    stats[5] = (float)nb;
+    // draw blocks [b_lo, b_hi] hold accepted attempts a_lo .. a_end
+    const int64_t b_lo = std::upper_bound(offs_h.begin(), offs_h.end(), (long long)a_lo) - offs_h.begin() - 1;
+    const int64_t b_hi = std::upper_bound(offs_h.begin(), offs_h.end(), (long long)a_end) - offs_h.begin() - 1;
+    const int flag_cap = (int)std::min<int64_t>(4096 + ((N * V) >> 16), 1 << 24);
+    DevBuf<Flagged> flags;
+    DevBuf<int> n_flags;
+    DevBuf<EndRecord> end_d;
+    CKS(flags.alloc(flag_cap, false));
+    CKS(n_flags.alloc(1, true));
+    CKS(end_d.alloc(1, true));
+    DrawParams p{};
+    p.key0 = key0.p;
+    p.starts = starts.p;
+    p.pos0 = start->pos;
+    p.b_first = (int)b_lo;
+    p.offs = offs.p;
+    p.t_lo = t_lo;
+    p.t_hi = t_hi;
+    p.has_gauss = hg;
+    p.V = h->V;
+    p.ld = h->ld;
+    p.M = h->M.p;
+    p.a_end = a_end;
+    p.end = end_d.p;
+    p.flags = flags.p;
+    p.n_flags = n_flags.p;
+    p.flag_cap = flag_cap;
+    k_legacy_pass<true><<<(unsigned)(b_hi - b_lo + 1), kN, 0, s>>>(p);
+    LAUNCH_CHECK("legacy_emit");
+    CK(cudaEventRecord(ev.e[3], s));
+    int nf = 0;
+    CK(cudaMemcpyAsync(&nf, n_flags.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&end_h, end_d.p, sizeof(EndRecord), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (nf > flag_cap) return fail(TGB200_ERR_STATE, "%d values near a float32 rounding midpoint (room for %d)", nf, flag_cap);
+    if (end_h.attempt < 0) return fail(TGB200_ERR_STATE, "legacy draw: the last attempt was not found");
+    // host fix-up: libm's log for every value whose float32 rounding could depend on the last bit of log
+    std::vector<Flagged> fl(nf);
+    std::vector<float> dev_vals(nf);
+    if (nf) CK(cudaMemcpy(fl.data(), flags.p, nf * sizeof(Flagged), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < nf; ++i) CK(cudaMemcpyAsync(&dev_vals[i], h->M.p + fl[i].idx, sizeof(float), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    patch_vals.resize(nf);
+    for (int i = 0; i < nf; ++i) {
+      patch_vals[i] = (float)polar_value_host(fl[i].w, fl[i].comp);
+      if (std::memcmp(&patch_vals[i], &dev_vals[i], sizeof(float)) != 0) {
+        CK(cudaMemcpyAsync(h->M.p + fl[i].idx, &patch_vals[i], sizeof(float), cudaMemcpyHostToDevice, s));
+        ++n_changed;
+      }
+    }
+    n_fixed = nf;
+  }
+  float cached = (float)start->gauss;
+  if (hg && t_lo == 0) CK(cudaMemcpyAsync(h->M.p, &cached, sizeof(float), cudaMemcpyHostToDevice, s));   // normal 0
+  if (a_end >= 0) CK(cudaEventRecord(ev.e[4], s));
+  CKS(reset_optimizer(h, s));
+  h->have_mapping = true;
+  CK(cudaStreamSynchronize(s));
+  if (a_end >= 0) {
+    stats[0] = ev.ms(0, 1);
+    stats[1] = ev.ms(1, 2);
+    stats[2] = ev.ms(2, 3);
+    stats[3] = ev.ms(3, 4);
+  }
+  stats[6] = (float)n_fixed;
+  stats[7] = (float)n_changed;
+  if (end_out) {
+    tgb200_mt_state e = *start;
+    e.has_gauss = 0;
+    e.gauss = 0.0;
+    if (a_end >= 0) {                          // 4 (attempt + 1) words consumed; an odd count leaves f x1 cached
+      mtj::jump(start->key, start->pos, (unsigned __int128)(4 * end_h.attempt + 3), e.key, &e.pos);
+      if ((end_normal - hg) & 1) {
+        e.has_gauss = 1;
+        e.gauss = polar_value_host(end_h.w, 1);
+      }
+    }
+    *end_out = e;
+  }
+  if (n_fixed_out) *n_fixed_out = n_fixed;
   return TGB200_OK;
 }
 
@@ -1509,6 +1750,12 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
     if (cap < 4) return fail(TGB200_ERR_INVALID, "cap < 4");
     out_host[0] = (float)h->Ke; out_host[1] = (float)h->ld; out_host[2] = (float)h->fwd_splits; out_host[3] = (float)h->r_parts;
     *n = 4;
+    return TGB200_OK;
+  } else if (nm == "legacy_init") {
+    *n = 8;
+    if (!out_host) return TGB200_OK;
+    if (cap < 8) return fail(TGB200_ERR_INVALID, "cap < 8");
+    for (int i = 0; i < 8; ++i) out_host[i] = h->legacy_stats[i];
     return TGB200_OK;
   } else return fail(TGB200_ERR_INVALID, "unknown debug buffer '%s'", name);
   *n = cnt;

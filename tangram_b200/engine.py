@@ -70,6 +70,15 @@ class Engine:
     def init_mapping_normal(self, seed, stream=None, first_row=0):
         _lib.check(self._lib.tgb200_init_mapping_normal_rows(self._h, seed, first_row, self._s(stream)))
 
+    def init_mapping_legacy(self, state, skip=0, first_row=0, end_normal=None, stream=None):
+        """The reference draw np.random.normal(0, 1, ...) from the numpy generator state `state` (get_state() tuple):
+        rows [first_row, first_row + n_cells) of a draw that starts `skip` normals into the stream.  Returns (the state
+        after end_normal normals, default the end of these rows; values recomputed on the host)."""
+        from . import legacy_rng
+        if end_normal is None:
+            end_normal = skip + (first_row + self.cfg.n_cells) * self.cfg.n_voxels
+        return legacy_rng.init_mapping(self._lib, self._h, state, skip, first_row, end_normal, self._s(stream))
+
     def run(self, n_steps, lr=0.1, stream=None):
         _lib.check(self._lib.tgb200_run(self._h, n_steps, lr, self._s(stream)))
 

@@ -9,7 +9,8 @@ Additions (keyword-only, all optional):
   precision   "bf16x3" (default: parity-grade fp32 results on wgmma tensor cores -- every operand is split into three
               bf16 planes and the six significant partial products are accumulated in fp32) |
               "fp32" (FFMA contractions, the cross-check) | "bf16" (plain bf16 operands: throughput mode)
-  M0          explicit initial mapping (ndarray N x V); default is the reference draw
+  M0          explicit initial mapping (ndarray N x V); default is the reference draw, made on the device bit for bit
+              (legacy_rng), leaving numpy's global generator where the host draw leaves it
   process_group / shard  cell-sharded multi-GPU operation (one process per GPU): every rank passes the
               full S (/ M0) and keeps rows shard_rows(N, rank, world); with a NCCL process group the handle gets its own
               NCCL communicator (tgb200_comm_init_rank) and the per-iteration exchange runs inside tgb200_run
@@ -21,7 +22,7 @@ import ctypes
 
 import numpy as np
 
-from . import _lib
+from . import _lib, legacy_rng
 from .sharded import shard_rows, sharded_steps
 
 _HIST_KEYS = ["total_loss", "main_loss", "vg_reg", "kl_reg", "entropy_reg"]
@@ -206,9 +207,11 @@ class Mapper:
         sharded = (r1 - r0) != n_cells_global
         # initial mapping: legacy numpy RNG, float64 draw, f32 cast; seeded only if truthy (:147-157).  A rank of a
         # sharded run draws the same stream and keeps only its rows (pre-sharded callers pass M0 or get a per-rank draw).
-        if M0 is None:
+        # The draw runs on the device (legacy_rng) unless this numpy's arithmetic differs from the device formula.
+        device_draw = M0 is None and not presharded and legacy_rng.device_draw_supported()
+        if M0 is None and not device_draw:
             M0 = legacy_normal_rows(self.random_state, n_rows_given, n_voxels, r0, r1)
-        else:
+        elif M0 is not None:
             M0 = M0[r0:r1]
 
         cfg = _lib.Config()
@@ -256,9 +259,14 @@ class Mapper:
             if ct_encode is None:
                 raise ValueError("ct_encode is required when lambda_ct_islands > 0")
             _lib.check(L.tgb200_set_ct_encode(h, _lib.ptr(np.ascontiguousarray(ct_encode[r0:r1])), None))
-        M0 = np.ascontiguousarray(M0, dtype=np.float32)
-        _lib.check(L.tgb200_set_mapping(h, _lib.ptr(M0), None))
-        del M0
+        if device_draw:
+            if self.random_state:
+                np.random.seed(seed=self.random_state)
+            legacy_rng.draw_global(L, h, 0, r0, r1 * n_voxels)      # the generator ends after row r1, as on the host
+        else:
+            M0 = np.ascontiguousarray(M0, dtype=np.float32)
+            _lib.check(L.tgb200_set_mapping(h, _lib.ptr(M0), None))
+            del M0
         self._own_comm = False
         if sharded and process_group is not None:
             self._init_comm(process_group)
@@ -434,7 +442,9 @@ class MapperConstrained:
         G = np.ascontiguousarray(np.asarray(G, dtype=np.float32))
         n_cells, n_voxels, n_genes = S.shape[0], G.shape[0], S.shape[1]
         self.target_density_enabled = d is not None
-        if M0 is None or F0 is None:
+        draw = M0 is None or F0 is None
+        device_draw = draw and legacy_rng.device_draw_supported()
+        if draw and not device_draw:
             # :472-493 -- M is drawn twice (the second draw is used), F after it, legacy numpy RNG
             if self.random_state:
                 np.random.seed(seed=self.random_state)
@@ -463,7 +473,14 @@ class MapperConstrained:
         if self.target_density_enabled:
             dd = np.ascontiguousarray(np.asarray(d, dtype=np.float32))
             _lib.check(L.tgb200_set_density(h, _lib.ptr(dd), None, None))
-        _lib.check(L.tgb200_set_mapping(h, _lib.ptr(np.ascontiguousarray(M0, dtype=np.float32)), None))
+        if device_draw:
+            # the same three draws: the first N x V normals are skipped, the second N x V land in M, F follows on the host
+            if self.random_state:
+                np.random.seed(seed=self.random_state)
+            legacy_rng.draw_global(L, h, n_cells * n_voxels, 0, 2 * n_cells * n_voxels)
+            F0 = np.random.normal(0, 1, n_cells)
+        else:
+            _lib.check(L.tgb200_set_mapping(h, _lib.ptr(np.ascontiguousarray(M0, dtype=np.float32)), None))
         _lib.check(L.tgb200_set_filter(h, _lib.ptr(np.ascontiguousarray(F0, dtype=np.float32)), None))
 
     def __del__(self):
