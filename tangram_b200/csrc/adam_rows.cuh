@@ -175,8 +175,8 @@ k_adam_rows(const AdamRowsArgs p) {
 
 // ---- parity mode (bf16x3): the same streaming pass in the reference's arithmetic ---------------------------------------------
 // IEEE expf / div / sqrt, torch's single-tensor Adam op order (adam_update), P from the row-pass statistics (softmax_prob) --
-// element for element what the fused epilogue of round 1 (TcEpiAdam, exact path) computed, now fed by the fp32 dP the
-// store-only contraction left in HBM.  16 B/element in (M, m, v, dP), 12 B/element out.
+// element for element what the fp32 mode's fused epilogue (EpiAdam) computes, here fed by the fp32 dP the store-only
+// contraction left in HBM.  16 B/element in (M, m, v, dP), 12 B/element out.
 struct AdamRowsExactArgs {
   float* M; float* m; float* v;          // [rows][ld]
   const float* dp;                       // [rows][ld]

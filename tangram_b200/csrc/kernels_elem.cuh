@@ -641,12 +641,6 @@ __global__ void k_pack_rows(const float* __restrict__ src, int rows, int cols, f
   const int r = (int)(i / cols), c = (int)(i % cols);
   dst[(size_t)r * ld + col_off + c] = src[i];
 }
-__global__ void k_unpack_rows(const float* __restrict__ src, int ld, int rows, int cols, float* __restrict__ dst) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)rows * cols) return;
-  const int r = (int)(i / cols), c = (int)(i % cols);
-  dst[i] = src[(size_t)r * ld + c];
-}
 // density columns of S_ext: cells mode (1, 0); clusters mode (w, 0) in fp32 or (hi, lo) split for bf16
 __global__ void k_fill_density_cols(float* __restrict__ Sx, int rows, int ld, int col, const float* __restrict__ w,
                                     int split_bf16) {
@@ -689,17 +683,17 @@ __global__ void k_init_normal(float* __restrict__ M, int rows, int V, int ld, un
   reinterpret_cast<float4*>(M + (size_t)r * ld)[c >> 2] = n;
 }
 // ---- tensor-core path: row normalisation carried across iterations -------------------------
-// The backward epilogue of iteration t writes, for iteration t+1, Pt_ij = exp(Mnew_ij - lseA_i)
-// (bf16) where lseA_i is the exact log-sum-exp of the OLD row, plus per-row partial sums of Pt
+// The streaming update of iteration t writes, for iteration t+1, Pt_ij = exp(Mnew_ij - lseA_i)
+// (bf16) where lseA_i is the exact log-sum-exp of the OLD row, plus per-row sums of Pt
 // (and Pt*M, |M|, M^2 when those terms are on).  This kernel turns them into the exact statistics
 // of the new row:  zt_i = sum_j Pt_ij,  lseT_i = lseA_i + log zt_i,  P_ij = Pt_ij / zt_i,
 // h_i = sum_j P log P = px_i / zt_i - lseT_i.   `fresh` = P was just produced by the row pass
 // (already normalised: zt = 1, lseT = mx + log Z).
-__global__ void k_row_norm(int n_rows, int fresh, const float* __restrict__ zpart, const float* __restrict__ pxpart,
-                           const float* __restrict__ l1part, const float* __restrict__ l2part, int nparts,
+__global__ void k_row_norm(int fresh, const float* __restrict__ zsum, const float* __restrict__ pxsum,
+                           const float* __restrict__ l1sum, const float* __restrict__ l2sum,
                            const float* __restrict__ lseA, float* __restrict__ lseT, float* __restrict__ inv_zt,
                            RowStat* __restrict__ stats, float* __restrict__ rowaux, int row0, int row1) {
-  const int i = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // rows [row0, row1) of n_rows
+  const int i = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // rows [row0, row1)
   if (i >= row1) return;
   if (fresh) {
     const RowStat st = stats[i];
@@ -707,21 +701,15 @@ __global__ void k_row_norm(int n_rows, int fresh, const float* __restrict__ zpar
     inv_zt[i] = 1.f;
     return;   // stats[i].h and rowaux were written by the row pass
   }
-  float z = 0.f, px = 0.f, a = 0.f, b = 0.f;
-  for (int p = 0; p < nparts; ++p) {
-    const size_t o = (size_t)p * n_rows + i;
-    z += zpart[o];
-    if (pxpart) px += pxpart[o];
-    if (l1part) { a += l1part[o]; b += l2part[o]; }
-  }
+  const float z = zsum[i];
   const float lt = lseA[i] + logf(z);
   lseT[i] = lt;
   inv_zt[i] = 1.f / z;
   RowStat st;
   st.mx = lt; st.inv_z = 1.f; st.log_z = 0.f;
-  st.h = pxpart ? px / z - lt : 0.f;
+  st.h = pxsum ? pxsum[i] / z - lt : 0.f;
   stats[i] = st;
-  if (rowaux && l1part) { rowaux[2 * i] = a; rowaux[2 * i + 1] = b; }
+  if (rowaux && l1sum) { rowaux[2 * i] = l1sum[i]; rowaux[2 * i + 1] = l2sum[i]; }
 }
 // Sxs[i][:] = bf16(Sx[i][:] * inv_zt[i]): the forward B operand carries the row normalisation
 __global__ void k_scale_rows_bf16(const float* __restrict__ Sx, const float* __restrict__ inv_zt, int row0, int row1, int ld,
@@ -760,19 +748,13 @@ __global__ void k_sum_planes(const float* __restrict__ part, int nplanes, size_t
   for (int z = 0; z < nplanes; ++z) s += part[(size_t)z * plane + i];
   out[i] = s;
 }
-// r_i = sum over partial arrays (deterministic order); also packs the per-row constants the
-// tensor-core backward epilogue needs (lse, r, h) into one float4.
-__global__ void k_rowdot_finalize(const float* __restrict__ rpart, int nparts, int n_rows, float* __restrict__ r,
-                                  const RowStat* __restrict__ stats, float4* __restrict__ rowc) {
+// r_i = sum over partial arrays (deterministic order)
+__global__ void k_rowdot_finalize(const float* __restrict__ rpart, int nparts, int n_rows, float* __restrict__ r) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_rows) return;
   float s = 0.f;
   for (int p = 0; p < nparts; ++p) s += rpart[(size_t)p * n_rows + i];
   r[i] = s;
-  if (rowc != nullptr) {
-    const RowStat st = stats[i];
-    rowc[i] = make_float4(st.mx + st.log_z, s, st.h, 0.f);
-  }
 }
 
 }  // namespace tgb

@@ -73,7 +73,19 @@ struct CsrDev {
   Csr view() const { return Csr{indptr.p, indices.p, vals.p}; }
 };
 
-struct KernelTimer;  // fwd
+// what the bf16-mode operand Pb holds
+enum class PState {
+  stale,                        // nothing valid: the next forward runs the row pass
+  fresh,                        // normalised P from the row pass
+  updated,                      // exp(Mnew - lse) from the streaming update; k_row_norm normalises it
+};
+
+// one launch while recording is on (tgb200_profile_step / tgb200_debug_timeline): stream 0 caller, 1 hi, 2 lo, 3 sf
+struct LaunchRecord {
+  const char* name;
+  int stream;
+  cudaEvent_t ev;
+};
 
 struct tgb200_mapper {
   tgb200_config cfg;
@@ -82,7 +94,6 @@ struct tgb200_mapper {
   bool bf16;                    // throughput mode: bf16 operands
   bool x3;                      // parity mode on tensor cores: three bf16 planes per operand, six partial products
   bool tcm;                     // either tensor-core mode
-  int n_pairs = 1;
   // state
   DevBuf<float> M, m, v;        // N x ld
   int64_t step = 0;
@@ -98,21 +109,21 @@ struct tgb200_mapper {
   DevBuf<float4> rowc;          // (lse, r, h, 0) per row for the tensor-core backward epilogue
   // tensor-core path: row normalisation carried across iterations (see k_row_norm)
   DevBuf<__nv_bfloat16> Sxs;    // N x Ke  bf16(S_ext / zt): forward B operand
-  DevBuf<float> lse0, lse1, inv_zt, zpart, pxpart, l1part, l2part;
+  DevBuf<float> lse0, lse1, inv_zt;
+  DevBuf<float> zsum, pxsum, l1sum, l2sum;   // per row, left by the streaming update (AdamRowsArgs); px / l1 / l2 only when used
   float* lseA = nullptr;        // offset the current Pb was produced with
   float* lseT = nullptr;        // exact log-sum-exp of the current rows
-  int z_parts = 0;
   // constrained mode (MapperConstrained): filter logits, their Adam state, f = sigmoid(F), S_f = f o S_ext
   bool constrained = false, have_filter = false;
   DevBuf<float> Fl, mF, vF, fsig, Sf, fscal;
-  int p_state = 0;              // 0: Pb invalid, 1: fresh from the row pass (normalised), 2: written by backward
+  PState p_state = PState::stale;
   int r_parts = 0;
   // forward / loss
   int fwd_splits = 1;
   DevBuf<float> Ypart;          // splits x V x Ke (only when splits > 1)
   DevBuf<float> Y;              // V x Ke + kTail (exchange buffer)
-  DevBuf<float> dY;             // V x Ke
-  DevBuf<__nv_bfloat16> dYb;
+  DevBuf<float> dY;             // V x Ke (fp32 mode)
+  DevBuf<__nv_bfloat16> dYb;    // the tensor-core modes' dY: one bf16 plane, or three in bf16x3 mode
   DevBuf<float> ngc, ngr, WG, nwg, AG, nag, sgnG, Z, Zg, H;
   DevBuf<float> colpart, colpart_nb, colpart_go, rowpart, ctpart;
   DevBuf<float> coefA, coefB, coefAn, coefBn, coefAg, coefBg, coefAr, coefBr, densg;
@@ -129,21 +140,18 @@ struct tgb200_mapper {
   // last tgb200_init_mapping_legacy: ms of jump, count + scan, emit, fix-up (device, CUDA events), host polynomials,
   // then draw blocks, values recomputed on the host, values the recomputation changed
   float legacy_stats[8] = {0};
-  KernelTimer* timer = nullptr;
   TcContext tc;                 // driver entry points etc. for the wgmma path
   TcPlan plan_fwd, plan_dp;     // tensor maps of the two contractions, encoded once (the buffers never move)
-  // staged backward (bf16 mode): store-only contraction -> bf16 dq = dP - centre in HBM -> streaming Adam kernel;
+  // backward of the bf16 mode: store-only contraction -> bf16 dq = dP - centre in HBM -> streaming Adam kernel;
   // two contractions per iteration instead of three (no separate row-dot GEMM)
-  bool staged = false;
   DevBuf<__nv_bfloat16> dq;     // N x ld
-  DevBuf<__nv_bfloat16> mb;     // N x ld: Adam's first moment in bf16 (staged mode only; `m` is then not allocated).  It is an
+  DevBuf<__nv_bfloat16> mb;     // N x ld: Adam's first moment in bf16 (bf16 mode only; `m` is then not allocated).  It is an
                                 // exponential average with a 10-iteration memory: bf16 rounding noise does not accumulate, and
                                 // next to bf16 operands it is invisible in every parity metric (DESIGN.md); v stays fp32.
   DevBuf<float> rcenter;        // per row: last iteration's row-dot, the centre dq is stored relative to
   // the same staging for the parity mode (bf16x3): dP in fp32, exact streaming update (no chunk pipeline)
-  bool staged_x3 = false;
   DevBuf<float> dpf;            // N x ld
-  // Pipelining of the staged backward over cell chunks (rows [chunk_row[c], chunk_row[c+1]), multiples of 256):
+  // Pipelining of the bf16 backward over cell chunks (rows [chunk_row[c], chunk_row[c+1]), multiples of 256):
   //   hi (high-priority stream): forward(c) ... loss ... backward contraction(c)        -- tensor-core bound
   //   lo (low-priority stream):  row-dot finalize(c), streaming Adam(c)                 -- HBM bound
   // Adam(c) runs under the contraction of chunk c+1 and, across the iteration boundary, under the next forward's
@@ -151,20 +159,21 @@ struct tgb200_mapper {
   // start of an API call and joins hi + lo at its end (tgb200_run joins once, after its last iteration).
   bool pipelined = false;
   int nchunks = 1, chunk_row[9] = {0};
-  cudaStream_t hi = nullptr, lo = nullptr, sf = nullptr;     // sf: the NEXT iteration's forward chunks (see backward_staged)
+  cudaStream_t hi = nullptr, lo = nullptr, sf = nullptr;     // sf: the NEXT iteration's forward chunks (see backward_bf16)
   cudaEvent_t ev_fork = nullptr, ev_join_hi = nullptr, ev_join_lo = nullptr, ev_join_sf = nullptr, ev_loss = nullptr;
   cudaEvent_t ev_g[8] = {}, ev_a[8] = {}, ev_f[8] = {};
   bool a_valid = false;         // ev_a[] were recorded by an earlier step_end and guard the rows of the next forward
   bool prefetch_next = false;   // tgb200_run, not its last iteration: issue the NEXT forward's chunks between this backward's chunks
   bool fwd_ahead = false;       // ... and they have been issued: the next step_begin skips its chunk loop
-  bool l2_persist = false;      // dY_ext pinned in L2 (access-policy window on the contraction stream)
   bool defer_join = false;      // inside tgb200_run: no fork / join between its iterations
   bool serial = false;          // tgb200_profile_step: everything on the caller's stream, one kernel at a time
-  // diagnostics (tgb200_debug_timeline): completion time of every launch on its stream
-  bool timeline_on = false;
-  std::vector<const char*> tl_names;
-  std::vector<int> tl_streams;
-  std::vector<cudaEvent_t> tl_events;
+  // diagnostics: an event after every launch while recording is on
+  bool recording = false;
+  std::vector<LaunchRecord> records;
+  void drop_records(size_t from) {
+    for (size_t i = from; i < records.size(); ++i) cudaEventDestroy(records[i].ev);
+    records.resize(from);
+  }
   // cell-sharded operation: NCCL communicator of the ranks that share the voxels (tgb200_comm_init_rank / tgb200_set_comm)
   void* comm = nullptr;
   bool comm_owned = false;
@@ -189,31 +198,17 @@ struct tgb200_mapper {
     for (cudaEvent_t e : {ev_fork, ev_join_hi, ev_join_lo, ev_join_sf, ev_loss}) if (e) cudaEventDestroy(e);
     for (int i = 0; i < 8; ++i)
       for (cudaEvent_t e : {ev_g[i], ev_a[i], ev_f[i]}) if (e) cudaEventDestroy(e);
+    drop_records(0);
   }
 };
 
-// Optional per-kernel CUDA-event timing (tgb200_profile_step).
-struct KernelTimer {
-  std::vector<const char*> names;
-  std::vector<cudaEvent_t> ev;
-};
 static void mark(tgb200_mapper* h, cudaStream_t s, const char* name) {
   h->launches++;
-  if (h->timeline_on) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, s);
-    h->tl_names.push_back(name);
-    h->tl_streams.push_back(s == h->hi ? 1 : (s == h->lo ? 2 : (s == h->sf ? 3 : 0)));
-    h->tl_events.push_back(e);
-  }
-  if (h->timer) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, s);
-    h->timer->names.push_back(name);
-    h->timer->ev.push_back(e);
-  }
+  if (!h->recording) return;
+  cudaEvent_t e;
+  cudaEventCreate(&e);
+  cudaEventRecord(e, s);
+  h->records.push_back({name, s == h->hi ? 1 : (s == h->lo ? 2 : (s == h->sf ? 3 : 0)), e});
 }
 #define LAUNCH_CHECK(name)                                                                  \
   do {                                                                                      \
@@ -300,35 +295,33 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   h->bf16 = cfg->precision == TGB200_PREC_BF16;
   h->x3 = cfg->precision == TGB200_PREC_BF16X3;
   h->tcm = h->bf16 || h->x3;
-  h->n_pairs = h->x3 ? 6 : 1;
   h->ct_off = h->K + 2;
   h->Ke = (int)round_up(h->K + 2 + h->T, 64);
   h->ld = (int)round_up(h->V, 64);
   const size_t nv = (size_t)h->N * h->ld, vk = (size_t)h->V * h->Ke;
   int st = TGB200_OK;
   auto A = [&](int s) { if (st == TGB200_OK) st = s; };
-  h->staged = h->bf16;           // both tensor-core modes stage the backward contraction's result in HBM
-  h->staged_x3 = h->x3;
-  if (h->staged_x3) A(h->dpf.alloc(nv, false));
+  if (h->x3) A(h->dpf.alloc(nv, false));
   A(h->M.alloc(nv)); A(h->v.alloc(nv));
-  if (h->staged) A(h->mb.alloc(nv)); else A(h->m.alloc(nv));
+  if (h->bf16) A(h->mb.alloc(nv)); else A(h->m.alloc(nv));
   if (h->bf16) {
-    h->z_parts = 1;              // k_adam_rows: one warp per row, complete row sums
     A(h->Sxs.alloc((size_t)h->N * h->Ke)); A(h->lse0.alloc(h->N)); A(h->lse1.alloc(h->N)); A(h->inv_zt.alloc(h->N));
-    A(h->zpart.alloc((size_t)h->z_parts * h->N));
-    if (cfg->lambda_r != 0.f) A(h->pxpart.alloc((size_t)h->z_parts * h->N));
-    if (cfg->lambda_l1 != 0.f || cfg->lambda_l2 != 0.f) { A(h->l1part.alloc((size_t)h->z_parts * h->N)); A(h->l2part.alloc((size_t)h->z_parts * h->N)); }
+    A(h->zsum.alloc(h->N));
+    if (cfg->lambda_r != 0.f) A(h->pxsum.alloc(h->N));
+    if (cfg->lambda_l1 != 0.f || cfg->lambda_l2 != 0.f) { A(h->l1sum.alloc(h->N)); A(h->l2sum.alloc(h->N)); }
     h->lseA = h->lse0.p; h->lseT = h->lse1.p;
+    A(h->rowc.alloc(h->N)); A(h->Pb.alloc(nv)); A(h->Sxb.alloc((size_t)h->N * h->Ke)); A(h->dYb.alloc(vk));
+    A(h->dq.alloc(nv, false)); A(h->rcenter.alloc(h->N));
+  } else if (h->x3) {
+    A(h->Pb.alloc(3 * nv)); A(h->Sxb.alloc((size_t)3 * h->N * h->Ke)); A(h->dYb.alloc(3 * vk));
+  } else {
+    A(h->Pf.alloc(nv));
   }
-  if (h->bf16) { A(h->rowc.alloc(h->N)); A(h->Pb.alloc(nv)); A(h->Sxb.alloc((size_t)h->N * h->Ke)); A(h->dYb.alloc(vk)); }
-  if (h->staged) { A(h->dq.alloc(nv, false)); A(h->rcenter.alloc(h->N)); }
-  else if (h->x3) { A(h->Pb.alloc(3 * nv)); A(h->Sxb.alloc((size_t)3 * h->N * h->Ke)); A(h->dYb.alloc(3 * vk)); }
-  else A(h->Pf.alloc(nv));
   A(h->Sx.alloc((size_t)h->N * h->Ke));
   A(h->G.alloc(vk));
   A(h->d.alloc(h->V)); A(h->dsrc.alloc(h->N));
   A(h->stats.alloc(h->N)); A(h->rowaux.alloc((size_t)2 * h->N)); A(h->rdot.alloc(h->N));
-  if (h->staged) {
+  if (h->bf16) {
     // cell chunks of the pipelined backward: 4 from 32k cells up, 2 from 8k (a rank of an 8-way sharded 100k-cell run):
     // each chunk still fills the GPU several times over
     int nc = h->N >= 32768 ? 4 : (h->N >= 8192 ? 2 : 1);
@@ -340,7 +333,7 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
     h->nchunks = nc;
     for (int c = 0; c <= nc; ++c) h->chunk_row[c] = c == nc ? h->N : (int)round_up((int64_t)c * h->N / nc, 256);
   }
-  if (h->staged && h->nchunks > 1) {          // one chunk: nothing to overlap, everything stays on the caller's stream
+  if (h->nchunks > 1) {                      // one chunk: nothing to overlap, everything stays on the caller's stream
     int lo_p = 0, hi_p = 0;
     cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p);
     // priorities: backward contractions (they feed the streaming update) > next forward's chunks > the update itself
@@ -356,23 +349,21 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
            cudaEventCreateWithFlags(&h->ev_f[c], cudaEventDisableTiming) == cudaSuccess;
     if (!ok) A(fail(TGB200_ERR_CUDA, "stream / event creation failed: %s", cudaGetErrorString(cudaGetLastError())));
     h->pipelined = ok;
-    h->l2_persist = getenv("TGB200_L2_PERSIST") && atoi(getenv("TGB200_L2_PERSIST")) != 0;
   }
-  // forward split over cells so that the grid covers the SMs twice (deterministic partial planes)
+  // forward split over cells (deterministic partial planes)
   h->tc.num_sms = prop.multiProcessorCount;
-  {
+  if (h->nchunks > 1) {
+    h->fwd_splits = 1;                       // the cell chunks of the pipelined forward accumulate straight into Y_ext
+  } else if (h->tcm) {
+    h->fwd_splits = tc_forward_splits(h->tc.num_sms, h->N, h->V, h->Ke);
+    if (h->x3) h->fwd_splits = std::max(h->fwd_splits, tc_splits_for_chain(h->N, 2048));
+  } else {                                   // the SIMT grid covers the SMs twice
     const int tiles = (int)(ceil_div(h->V, 128) * ceil_div(h->Ke, 128));
-    int s = (int)ceil_div(2 * h->tc.num_sms, tiles);
-    const int max_s = (int)ceil_div(h->N, 512);
-    if (s > max_s) s = max_s;
-    if (s < 1) s = 1;
-    if (h->tcm) s = tc_forward_splits(h->tc.num_sms, h->N, h->V, h->Ke);
-    if (h->x3) { const int c = tc_splits_for_chain(h->N, 2048); if (c > s) s = c; }
-    if (h->nchunks > 1) s = 1;               // the cell chunks of the pipelined forward accumulate straight into Y_ext
-    h->fwd_splits = s;
-    if (s > 1) A(h->Ypart.alloc((size_t)s * vk));
+    h->fwd_splits = std::clamp((int)ceil_div(2 * h->tc.num_sms, tiles), 1, (int)ceil_div(h->N, 512));
   }
-  A(h->Y.alloc(vk + kTail)); A(h->dY.alloc(vk));
+  if (h->fwd_splits > 1) A(h->Ypart.alloc((size_t)h->fwd_splits * vk));
+  A(h->Y.alloc(vk + kTail));
+  if (!h->tcm) A(h->dY.alloc(vk));
   if (h->constrained) {
     A(h->Fl.alloc(h->N)); A(h->mF.alloc(h->N)); A(h->vF.alloc(h->N)); A(h->fsig.alloc(h->N));
     A(h->Sf.alloc((size_t)h->N * h->Ke)); A(h->fscal.alloc(4));
@@ -402,22 +393,6 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (cfg->lambda_ct_islands > 0.f) {
     h->n_ct_blocks = (int)ceil_div((int64_t)h->V * h->T, 256);
     A(h->H.alloc((size_t)h->V * h->T)); A(h->ctpart.alloc(h->n_ct_blocks));
-  }
-  if (st == TGB200_OK && h->l2_persist && h->pipelined) {
-    // keep dY_ext (the B operand every backward tile re-reads) resident in L2 while the state streams through it
-    const size_t bytes = (size_t)h->V * h->Ke * sizeof(__nv_bfloat16);
-    int max_persist = 0, max_window = 0;
-    cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, cfg->device);
-    cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, cfg->device);
-    const size_t want = bytes < (size_t)max_persist ? bytes : (size_t)max_persist;
-    cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want);
-    cudaStreamAttrValue attr = {};
-    attr.accessPolicyWindow.base_ptr = h->dYb.p;
-    attr.accessPolicyWindow.num_bytes = bytes < (size_t)max_window ? bytes : (size_t)max_window;
-    attr.accessPolicyWindow.hitRatio = want >= bytes ? 1.0f : (float)want / (float)bytes;
-    attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    if (cudaStreamSetAttribute(h->hi, cudaStreamAttributeAccessPolicyWindow, &attr) != cudaSuccess) { (void)cudaGetLastError(); h->l2_persist = false; }
   }
   if (st == TGB200_OK && h->tcm) st = tc_init(h->tc, g_err, sizeof(g_err));
   if (st != TGB200_OK) { delete h; return st; }
@@ -579,15 +554,20 @@ extern "C" int tgb200_set_graph(tgb200_mapper* h, int which, const int32_t* indp
   return TGB200_OK;
 }
 
-static int reset_optimizer(tgb200_mapper* h, cudaStream_t s) {
-  if (h->staged) CK(cudaMemsetAsync(h->mb.p, 0, h->mb.n * sizeof(__nv_bfloat16), s));
+static int zero_moments(tgb200_mapper* h, cudaStream_t s) {
+  if (h->bf16) CK(cudaMemsetAsync(h->mb.p, 0, h->mb.n * sizeof(__nv_bfloat16), s));
   else CK(cudaMemsetAsync(h->m.p, 0, h->m.n * sizeof(float), s));
   CK(cudaMemsetAsync(h->v.p, 0, h->v.n * sizeof(float), s));
-  if (h->staged) CK(cudaMemsetAsync(h->rcenter.p, 0, h->rcenter.n * sizeof(float), s));
+  return TGB200_OK;
+}
+
+static int reset_optimizer(tgb200_mapper* h, cudaStream_t s) {
+  CKS(zero_moments(h, s));
+  if (h->bf16) CK(cudaMemsetAsync(h->rcenter.p, 0, h->rcenter.n * sizeof(float), s));
   h->step = 0;
   h->hist_len = 0;
   h->in_step = false;
-  h->p_state = 0;
+  h->p_state = PState::stale;
   h->fwd_ahead = false;
   return TGB200_OK;
 }
@@ -599,9 +579,7 @@ extern "C" int tgb200_reset_adam(tgb200_mapper* h, void* stream) {
   if (h->in_step) return fail(TGB200_ERR_STATE, "reset_adam inside a step");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
-  if (h->staged) CK(cudaMemsetAsync(h->mb.p, 0, h->mb.n * sizeof(__nv_bfloat16), s));
-  else CK(cudaMemsetAsync(h->m.p, 0, h->m.n * sizeof(float), s));
-  CK(cudaMemsetAsync(h->v.p, 0, h->v.n * sizeof(float), s));
+  CKS(zero_moments(h, s));
   if (h->constrained) {
     CK(cudaMemsetAsync(h->mF.p, 0, h->mF.n * sizeof(float), s));
     CK(cudaMemsetAsync(h->vF.p, 0, h->vF.n * sizeof(float), s));
@@ -675,10 +653,15 @@ static bool valid_mt_state(const tgb200_mt_state* st) {
   return st->pos >= 0 && st->pos <= mtj::kN && (st->has_gauss == 0 || st->has_gauss == 1);
 }
 
-extern "C" int tgb200_mt19937_jump(const tgb200_mt_state* in, uint64_t n_words, tgb200_mt_state* out) {
+static int check_jump_args(const tgb200_mt_state* in, const tgb200_mt_state* out) {
   if (!in || !out) return fail(TGB200_ERR_INVALID, "null argument");
   if (!valid_mt_state(in)) return fail(TGB200_ERR_INVALID, "bad generator state (pos %d, has_gauss %d)", in->pos, in->has_gauss);
   if (!mtj::field().ok()) return fail(TGB200_ERR_STATE, "MT19937 characteristic polynomial not found");
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_mt19937_jump(const tgb200_mt_state* in, uint64_t n_words, tgb200_mt_state* out) {
+  CKS(check_jump_args(in, out));
   tgb200_mt_state r = *in;
   if (n_words) mtj::jump(in->key, in->pos, (unsigned __int128)n_words - 1, r.key, &r.pos);
   *out = r;
@@ -686,10 +669,8 @@ extern "C" int tgb200_mt19937_jump(const tgb200_mt_state* in, uint64_t n_words, 
 }
 
 extern "C" int tgb200_mt19937_jump_pow2(const tgb200_mt_state* in, uint32_t log2_words, tgb200_mt_state* out) {
-  if (!in || !out) return fail(TGB200_ERR_INVALID, "null argument");
-  if (!valid_mt_state(in)) return fail(TGB200_ERR_INVALID, "bad generator state (pos %d, has_gauss %d)", in->pos, in->has_gauss);
   if (log2_words > 128) return fail(TGB200_ERR_INVALID, "log2_words > 128");
-  if (!mtj::field().ok()) return fail(TGB200_ERR_STATE, "MT19937 characteristic polynomial not found");
+  CKS(check_jump_args(in, out));
   const unsigned __int128 n_minus_1 = log2_words == 128 ? ~(unsigned __int128)0 : ((unsigned __int128)1 << log2_words) - 1;
   tgb200_mt_state r = *in;
   mtj::jump(in->key, in->pos, n_minus_1, r.key, &r.pos);
@@ -775,6 +756,16 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
     CK(cudaMemcpy(key0.p, start->key, kN * sizeof(uint32_t), cudaMemcpyHostToDevice));
     std::vector<long long> offs_h;
     std::vector<uint64_t> flat;
+    DrawParams p{};
+    p.key0 = key0.p;
+    p.pos0 = start->pos;
+    p.t_lo = t_lo;
+    p.t_hi = t_hi;
+    p.has_gauss = hg;
+    p.V = h->V;
+    p.ld = h->ld;
+    p.M = h->M.p;
+    p.a_end = a_end;
     for (;;) {
       if (nb > (1LL << 30)) return fail(TGB200_ERR_INVALID, "draw of %lld normals is too large", (long long)end_normal);
       int levels = 0;
@@ -802,11 +793,9 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
         }
       }
       CK(cudaEventRecord(ev.e[1], s));
-      DrawParams p{};
-      p.key0 = key0.p;
       p.starts = starts.p;
-      p.pos0 = start->pos;
       p.counts = counts.p;
+      p.offs = offs.p;
       k_legacy_pass<false><<<(unsigned)nb, kN, 0, s>>>(p);
       LAUNCH_CHECK("legacy_count");
       k_scan_counts<<<1, 1024, 0, s>>>(counts.p, (int)nb, offs.p);
@@ -829,19 +818,7 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
     CKS(flags.alloc(flag_cap, false));
     CKS(n_flags.alloc(1, true));
     CKS(end_d.alloc(1, true));
-    DrawParams p{};
-    p.key0 = key0.p;
-    p.starts = starts.p;
-    p.pos0 = start->pos;
     p.b_first = (int)b_lo;
-    p.offs = offs.p;
-    p.t_lo = t_lo;
-    p.t_hi = t_hi;
-    p.has_gauss = hg;
-    p.V = h->V;
-    p.ld = h->ld;
-    p.M = h->M.p;
-    p.a_end = a_end;
     p.end = end_d.p;
     p.flags = flags.p;
     p.n_flags = n_flags.p;
@@ -913,7 +890,7 @@ static int launch_softmax_rows(tgb200_mapper* h, cudaStream_t s, PT* P, int want
   RowStat* st = h->stats.p + row0;
   // One CTA per row, the row cached in registers between the max / exp-sum / emit passes.  Wide rows use more threads with
   // fewer float4 slots each: registers/thread stay <= 40..64, so 48-64 warps stay resident per SM (256 x 12 slots held 24,
-  // and the row pass was latency-bound at 0.46 of the HBM peak; profiles/README.md).  Rows wider than 6144 float4 re-read M.
+  // and the row pass was latency-bound at 0.46 of the HBM peak).  Rows wider than 6144 float4 re-read M.
 #define SMX(T, ITEMS, MINB)                                                                         \
   k_softmax_rows<PT, T, ITEMS, MINB><<<nrows, T, 0, s>>>(Mp, h->ld, h->V, P, h->ld, st, rowaux, want_entropy, split)
   if (nvec <= 256 * 1) SMX(256, 1, 1);
@@ -997,7 +974,7 @@ static int forward_chunk(tgb200_mapper* h, cudaStream_t s, int c, int fresh, con
   const int r0 = h->nchunks > 1 ? h->chunk_row[c] : 0, r1 = h->nchunks > 1 ? h->chunk_row[c + 1] : h->N;
   // rows of this chunk: the streaming Adam kernel of the previous iteration must have written their P and row sums
   if (h->a_valid && h->pipelined && !h->serial) CK(cudaStreamWaitEvent(s, h->ev_a[c], 0));
-  k_row_norm<<<(unsigned)ceil_div(r1 - r0, 256), 256, 0, s>>>(h->N, fresh, h->zpart.p, h->pxpart.p, h->l1part.p, h->l2part.p, h->z_parts,
+  k_row_norm<<<(unsigned)ceil_div(r1 - r0, 256), 256, 0, s>>>(fresh, h->zsum.p, h->pxsum.p, h->l1sum.p, h->l2sum.p,
                                                              lseA, lseT, h->inv_zt.p, h->stats.p, rowaux, r0, r1);
   LAUNCH_CHECK("row_norm");
   const long long nq = (long long)(r1 - r0) * (h->Ke / 4);
@@ -1017,16 +994,16 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
   if (h->bf16) {
     // The row pass runs only when P is not already resident (first iteration / after a state load):
     // in steady state the previous backward epilogue has written P and its row sums.
-    if (h->p_state == 0) {
+    if (h->p_state == PState::stale) {
       CKS(launch_softmax_rows<__nv_bfloat16>(h, s, h->Pb.p, 1, rowaux));
-      h->p_state = 1;
+      h->p_state = PState::fresh;
     }
     if (h->fwd_ahead) {           // issued by the previous iteration's backward (forward_chunk under the streaming Adam kernel)
       h->fwd_ahead = false;
       for (int c = 0; c < h->nchunks; ++c) CK(cudaStreamWaitEvent(s, h->ev_f[c], 0));
       if (h->nchunks > 1) return TGB200_OK;
     } else {
-      for (int c = 0; c < h->nchunks; ++c) CKS(forward_chunk(h, s, c, h->p_state == 1 ? 1 : 0, h->lseA, h->lseT));
+      for (int c = 0; c < h->nchunks; ++c) CKS(forward_chunk(h, s, c, h->p_state == PState::fresh ? 1 : 0, h->lseA, h->lseT));
     }
     if (h->nchunks > 1) return TGB200_OK;
   } else if (h->x3) {
@@ -1043,7 +1020,7 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
       CKS(tc_forward_plan(h->tc, h->plan_fwd, h->Pb.p, (size_t)h->N * h->ld, sB, (size_t)h->N * h->Ke, h->x3 ? 3 : 1, h->N, h->V, h->Ke,
                           h->ld, g_err, sizeof(g_err)));
     }
-    CKS(tc_forward_launch(h->tc, h->plan_fwd, h->n_pairs, out, h->N, h->V, h->Ke, h->fwd_splits, s, g_err, sizeof(g_err)));
+    CKS(tc_forward_launch(h->tc, h->plan_fwd, h->x3 ? 6 : 1, out, h->N, h->V, h->Ke, h->fwd_splits, s, g_err, sizeof(g_err)));
     mark(h, s, "tc_gemm_fwd");
   } else {
     GemmArgs g;
@@ -1115,20 +1092,26 @@ static int ensure_history(tgb200_mapper* h, int64_t need, cudaStream_t s) {
   return TGB200_OK;
 }
 
+// Y_ext (first summed over the forward's partial planes when `from_partials`) -> finalised per-gene sums in colfin;
+// p.colpart then points at them for k_loss_scalars
+static int reduce_columns(tgb200_mapper* h, cudaStream_t s, LossParams& p, bool from_partials, int with_g2) {
+  const bool planes = from_partials && h->fwd_splits > 1;
+  dim3 vgrid(h->nredchunk, h->nchunk);          // four columns per thread
+  k_loss_reduce<<<vgrid, kLossCols, 0, s>>>(p, planes ? h->Ypart.p : h->Y.p, planes ? h->fwd_splits : 1, with_g2, h->loss_rows);
+  LAUNCH_CHECK("loss_reduce");
+  k_col_finalize<<<dim3((unsigned)ceil_div(h->Ke, 128), 3), 128, 0, s>>>(h->colpart.p, h->nchunk, 3, h->Ke, h->colfin.p);
+  LAUNCH_CHECK("col_finalize");
+  p.colpart = h->colfin.p;
+  return TGB200_OK;
+}
+
 // everything on V x Ke: reductions, scalars + history row, dY_ext
 static int loss_stage(tgb200_mapper* h, cudaStream_t s, float* hist_row, bool reduce_partials_first) {
   LossParams p = make_loss_params(h);
   const tgb200_config& c = h->cfg;
   dim3 rgrid(h->ncolchunk, h->nchunk);          // spatial kernels: one column per thread
-  dim3 vgrid(h->nredchunk, h->nchunk);          // reduction kernel: four columns per thread
-  const float* part = (h->fwd_splits > 1 && reduce_partials_first) ? h->Ypart.p : h->Y.p;
-  const int nsplit = (h->fwd_splits > 1 && reduce_partials_first) ? h->fwd_splits : 1;
-  k_loss_reduce<<<vgrid, kLossCols, 0, s>>>(p, part, nsplit, c.lambda_g2 != 0.f ? 1 : 0, h->loss_rows);
-  LAUNCH_CHECK("loss_reduce");
-  const dim3 fgrid3((unsigned)ceil_div(h->Ke, 128), 3), fgrid2((unsigned)ceil_div(h->Ke, 128), 2);
-  k_col_finalize<<<fgrid3, 128, 0, s>>>(h->colpart.p, h->nchunk, 3, h->Ke, h->colfin.p);
-  LAUNCH_CHECK("col_finalize");
-  p.colpart = h->colfin.p;
+  CKS(reduce_columns(h, s, p, reduce_partials_first, c.lambda_g2 != 0.f ? 1 : 0));
+  const dim3 fgrid2((unsigned)ceil_div(h->Ke, 128), 2);
   if (c.lambda_neighborhood_g1 > 0.f) {
     k_spatial_colstats<<<rgrid, kLossCols, 0, s>>>(h->V, h->K, h->Ke, h->W.view(), h->Y.p, h->WG.p, h->Z.p, h->colpart_nb.p, h->loss_rows);
     LAUNCH_CHECK("spatial_colstats");
@@ -1150,8 +1133,8 @@ static int loss_stage(tgb200_mapper* h, cudaStream_t s, float* hist_row, bool re
   k_loss_scalars<<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist_row);
   LAUNCH_CHECK("loss_scalars");
   dim3 dgrid(h->V, h->nredchunk);                       // voxels on x: gridDim.y is limited to 65535
-  // the tensor-core path consumes only the bf16 copy of dY_ext
-  k_dy_assemble<<<dgrid, kLossCols, 0, s>>>(p, h->tcm ? nullptr : h->dY.p, h->bf16 ? h->dYb.p : nullptr,
+  // fp32 dY_ext in fp32 mode (dY is not allocated otherwise), its bf16 copy or three bf16 planes on tensor cores
+  k_dy_assemble<<<dgrid, kLossCols, 0, s>>>(p, h->dY.p, h->bf16 ? h->dYb.p : nullptr,
                                             h->x3 ? Split3{h->dYb.p, (size_t)h->V * h->Ke} : Split3{nullptr, 0});
   LAUNCH_CHECK("dy_assemble");
   return TGB200_OK;
@@ -1179,9 +1162,9 @@ static int filter_update(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
   return TGB200_OK;
 }
 
-// Staged backward (bf16 mode): dq = bf16(S_ext dY_ext^T - centre) + row-dot partials from the store-only contraction,
+// Backward of the bf16 mode: dq = bf16(S_ext dY_ext^T - centre) + row-dot partials from the store-only contraction,
 // then one streaming pass does softmax-Jacobian + Adam + the next forward's P.  (mapping_optimizer.py:395-396)
-static int backward_staged(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, const AdamScalars& a) {
+static int backward_bf16(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, const AdamScalars& a) {
   if (!h->plan_dp.ready) {
     CKS(tc_dpstore_epi_plan(h->tc, h->plan_dp, h->Pb.p, h->dq.p, h->N, h->ld, g_err, sizeof(g_err)));
     CKS(tc_dpstore_plan(h->tc, h->plan_dp, h->Sxb.p, 0, h->dYb.p, 0, 1, h->N, h->V, h->Ke, g_err, sizeof(g_err)));
@@ -1202,7 +1185,7 @@ static int backward_staged(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, co
     { cudaStream_t s = su; LAUNCH_CHECK("rowdot_finalize"); }
     if (h->constrained) CKS(filter_update(h, su, a));
     AdamRowsArgs ar{h->M.p, h->mb.p, h->v.p, h->dq.p, h->Pb.p, reinterpret_cast<const RowConst*>(h->rowc.p),
-                    h->zpart.p, h->pxpart.p, h->l1part.p, h->l2part.p, h->ld, h->V, r0, r1,
+                    h->zsum.p, h->pxsum.p, h->l1sum.p, h->l2sum.p, h->ld, h->V, r0, r1,
                     h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
     if (adam_rows_launch(ar, su)) return fail(TGB200_ERR_CUDA, "launch adam_rows: %s", cudaGetErrorString(cudaGetLastError()));
     mark(h, su, "adam_rows");
@@ -1221,13 +1204,13 @@ static int backward_staged(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, co
   h->fwd_ahead = prefetch;
   // Pb now holds exp(Mnew - lseT): lseT becomes the offset of the resident P
   float* t = h->lseA; h->lseA = h->lseT; h->lseT = t;
-  h->p_state = 2;
+  h->p_state = PState::updated;
   return TGB200_OK;
 }
 
-// Staged backward of the parity mode (bf16x3): six partial products of S_ext dY_ext^T into fp32 dP + exact row-dot partials,
+// Backward of the parity mode (bf16x3): six partial products of S_ext dY_ext^T into fp32 dP + exact row-dot partials,
 // then the exact streaming update.  Two contractions per iteration instead of three here too.  (mapping_optimizer.py:395-396)
-static int backward_staged_x3(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a) {
+static int backward_bf16x3(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a) {
   const size_t nkp = (size_t)h->N * h->Ke, vkp = (size_t)h->V * h->Ke, nvp = (size_t)h->N * h->ld;
   if (!h->plan_dp.ready)
     CKS(tc_dpstore_plan(h->tc, h->plan_dp, h->Sxb.p, nkp, h->dYb.p, vkp, 3, h->N, h->V, h->Ke, g_err, sizeof(g_err)));
@@ -1236,13 +1219,35 @@ static int backward_staged_x3(tgb200_mapper* h, cudaStream_t s, const AdamScalar
   // 28.6 / 25.8 it/s at C3 instead of 21.2 -- not worth the parity-grade mode's point)
   CKS(tc_dpstore_launch(h->tc, h->plan_dp, 6, epi, 0, h->N, h->V, h->Ke, s, g_err, sizeof(g_err)));
   mark(h, s, "tc_gemm_bwd_dp");
-  k_rowdot_finalize<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->rpart.p, h->r_parts, h->N, h->rdot.p, h->stats.p, nullptr);
+  k_rowdot_finalize<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->rpart.p, h->r_parts, h->N, h->rdot.p);
   LAUNCH_CHECK("rowdot_finalize");
   if (h->constrained) CKS(filter_update(h, s, a));
   AdamRowsExactArgs ar{h->M.p, h->m.p, h->v.p, h->dpf.p, h->stats.p, h->rdot.p, h->ld, h->V, 0, h->N,
                        h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
   if (adam_rows_exact_launch(ar, s)) return fail(TGB200_ERR_CUDA, "launch adam_rows_exact: %s", cudaGetErrorString(cudaGetLastError()));
   mark(h, s, "adam_rows");
+  return TGB200_OK;
+}
+
+// Backward of the fp32 cross-check mode: FFMA contractions (row-dot GEMM, then the backward GEMM with the fused exact
+// epilogue)
+static int backward_fp32(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a) {
+  GemmArgs g;
+  g.A = h->Pf.p; g.lda = h->ld; g.B = h->dY.p; g.ldb = h->Ke;
+  g.M = h->N; g.N = h->Ke; g.K = h->V; g.k_per_split = (int)round_up(h->V, 16);
+  EpiRowDot epi_r{s_act(h), h->Ke, h->rpart.p};
+  dim3 grid_r((unsigned)ceil_div(h->Ke, SG_BN), (unsigned)ceil_div(h->N, SG_BM), 1);
+  k_gemm_simt<true, false, EpiRowDot><<<grid_r, SG_THREADS, 0, s>>>(g, epi_r);
+  LAUNCH_CHECK("simt_gemm_rowdot");
+  k_rowdot_finalize<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->rpart.p, h->r_parts, h->N, h->rdot.p);
+  LAUNCH_CHECK("rowdot_finalize");
+  if (h->constrained) CKS(filter_update(h, s, a));
+  g.A = s_act(h); g.lda = h->Ke; g.B = h->dY.p; g.ldb = h->Ke;
+  g.M = h->N; g.N = h->V; g.K = h->Ke; g.k_per_split = h->Ke;
+  EpiAdam epi{h->M.p, h->m.p, h->v.p, h->ld, h->V, h->stats.p, h->rdot.p, h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
+  dim3 grid((unsigned)ceil_div(h->V, SG_BN), (unsigned)ceil_div(h->N, SG_BM), 1);
+  k_gemm_simt<true, true, EpiAdam><<<grid, SG_THREADS, 0, s>>>(g, epi);
+  LAUNCH_CHECK("simt_gemm_bwd_adam");
   return TGB200_OK;
 }
 
@@ -1261,29 +1266,9 @@ extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
   if (h->pipelined && !h->serial) CK(cudaEventRecord(h->ev_loss, s));
 
   const AdamScalars a = adam_scalars(h->cfg, h->step + 1, lr);
-  if (h->staged) {
-    CKS(backward_staged(h, s, update_stream(h, caller), a));
-  } else if (h->staged_x3) {
-    CKS(backward_staged_x3(h, s, a));
-  } else {
-    // fp32 cross-check mode: FFMA contractions (row-dot GEMM, then the backward GEMM with the fused exact epilogue)
-    GemmArgs g;
-    g.A = h->Pf.p; g.lda = h->ld; g.B = h->dY.p; g.ldb = h->Ke;
-    g.M = h->N; g.N = h->Ke; g.K = h->V; g.k_per_split = (int)round_up(h->V, 16);
-    EpiRowDot epi_r{s_act(h), h->Ke, h->rpart.p};
-    dim3 grid_r((unsigned)ceil_div(h->Ke, SG_BN), (unsigned)ceil_div(h->N, SG_BM), 1);
-    k_gemm_simt<true, false, EpiRowDot><<<grid_r, SG_THREADS, 0, s>>>(g, epi_r);
-    LAUNCH_CHECK("simt_gemm_rowdot");
-    k_rowdot_finalize<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->rpart.p, h->r_parts, h->N, h->rdot.p, h->stats.p, nullptr);
-    LAUNCH_CHECK("rowdot_finalize");
-    if (h->constrained) CKS(filter_update(h, s, a));
-    g.A = s_act(h); g.lda = h->Ke; g.B = h->dY.p; g.ldb = h->Ke;
-    g.M = h->N; g.N = h->V; g.K = h->Ke; g.k_per_split = h->Ke;
-    EpiAdam epi{h->M.p, h->m.p, h->v.p, h->ld, h->V, h->stats.p, h->rdot.p, h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
-    dim3 grid((unsigned)ceil_div(h->V, SG_BN), (unsigned)ceil_div(h->N, SG_BM), 1);
-    k_gemm_simt<true, true, EpiAdam><<<grid, SG_THREADS, 0, s>>>(g, epi);
-    LAUNCH_CHECK("simt_gemm_bwd_adam");
-  }
+  if (h->bf16) CKS(backward_bf16(h, s, update_stream(h, caller), a));
+  else if (h->x3) CKS(backward_bf16x3(h, s, a));
+  else CKS(backward_fp32(h, s, a));
   CKS(join_streams(h, caller));
   h->step++;
   h->hist_len++;
@@ -1298,17 +1283,15 @@ static int exchange_partials(tgb200_mapper* h, cudaStream_t s) {
   const size_t count = (size_t)h->V * h->Ke + kTail;
   const int r = api->AllReduce(h->Y.p, h->Y.p, count, kNcclFloat32, kNcclSum, h->comm, s);
   if (r != 0) return fail(TGB200_ERR_CUDA, "ncclAllReduce: %s", api->GetErrorString(r));
-  if (h->timer) { mark(h, s, "nccl_all_reduce"); h->launches--; }   // timed when profiling; not one of OUR kernels
   return TGB200_OK;
 }
 
 // With a communicator in hand, move the exchange buffer into memory NCCL allocated itself and register it: the in-place
 // all-reduce then runs as an in-switch (NVLS) reduction on user buffers.  Best effort: any failure keeps the plain buffer.
 static void register_exchange_buffer(tgb200_mapper* h) {
-  static const bool kOn = !(getenv("TGB200_NCCL_REGISTER") && atoi(getenv("TGB200_NCCL_REGISTER")) == 0);
   char e[128];
   NcclApi* a = nccl_api(e, sizeof(e));
-  if (!kOn || !a || !a->MemAlloc || !a->MemFree || !a->CommRegister || !a->CommDeregister || h->y_nccl || !h->comm) return;
+  if (!a || !a->MemAlloc || !a->MemFree || !a->CommRegister || !a->CommDeregister || h->y_nccl || !h->comm) return;
   cudaSetDevice(h->cfg.device);
   cudaDeviceSynchronize();
   void* buf = nullptr;
@@ -1334,23 +1317,6 @@ extern "C" int tgb200_comm_unique_id(void* id_out, int64_t cap) {
   return TGB200_OK;
 }
 
-extern "C" int tgb200_comm_init_rank(tgb200_mapper* h, const void* unique_id, int32_t rank, int32_t world) {
-  if (!h || !unique_id) return fail(TGB200_ERR_INVALID, "null argument");
-  if (world < 1 || rank < 0 || rank >= world) return fail(TGB200_ERR_INVALID, "bad rank %d of %d", rank, world);
-  if (h->comm) return fail(TGB200_ERR_STATE, "this handle already has a communicator");
-  NcclApi* api = nccl_api(g_err, sizeof(g_err));
-  if (!api) return TGB200_ERR_STATE;
-  CK(cudaSetDevice(h->cfg.device));
-  NcclUniqueId id;
-  memcpy(&id, unique_id, sizeof(id));
-  void* comm = nullptr;
-  const int r = api->CommInitRank(&comm, world, id, rank);
-  if (r != 0) return fail(TGB200_ERR_CUDA, "ncclCommInitRank: %s", api->GetErrorString(r));
-  h->comm = comm; h->comm_owned = true; h->comm_rank = rank; h->comm_world = world;
-  register_exchange_buffer(h);
-  return TGB200_OK;
-}
-
 // A communicator that outlives handles: created once per process and group of ranks, lent to handles with tgb200_set_comm
 // (ncclCommInitRank costs a second or more at 8 ranks -- too much to pay in every Mapper constructor).
 extern "C" int tgb200_comm_create(const void* unique_id, int32_t rank, int32_t world, int32_t device, void** comm_out) {
@@ -1365,6 +1331,16 @@ extern "C" int tgb200_comm_create(const void* unique_id, int32_t rank, int32_t w
   const int r = api->CommInitRank(&comm, world, id, rank);
   if (r != 0) return fail(TGB200_ERR_CUDA, "ncclCommInitRank: %s", api->GetErrorString(r));
   *comm_out = comm;
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_comm_init_rank(tgb200_mapper* h, const void* unique_id, int32_t rank, int32_t world) {
+  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
+  if (h->comm) return fail(TGB200_ERR_STATE, "this handle already has a communicator");
+  void* comm = nullptr;
+  CKS(tgb200_comm_create(unique_id, rank, world, h->cfg.device, &comm));
+  h->comm = comm; h->comm_owned = true; h->comm_rank = rank; h->comm_world = world;
+  register_exchange_buffer(h);
   return TGB200_OK;
 }
 extern "C" int tgb200_comm_destroy(void* comm) {
@@ -1397,9 +1373,7 @@ extern "C" int tgb200_set_comm(tgb200_mapper* h, void* nccl_comm, int32_t rank, 
 extern "C" int tgb200_run(tgb200_mapper* h, int32_t n_steps, float lr, void* stream) {
   if (!h) return fail(TGB200_ERR_INVALID, "null handle");
   if (n_steps < 0) return fail(TGB200_ERR_INVALID, "n_steps < 0");
-  // TGB200_SKIP_EXCHANGE=1 (dev only): run one rank's share of a sharded iteration on a single GPU without its collective
-  static const bool kSkipExchange = getenv("TGB200_SKIP_EXCHANGE") && atoi(getenv("TGB200_SKIP_EXCHANGE")) != 0;
-  const bool sharded = h->cfg.n_cells_global != h->N && !kSkipExchange;
+  const bool sharded = h->cfg.n_cells_global != h->N;
   if (sharded && !h->comm)
     return fail(TGB200_ERR_STATE, "cell-sharded handle without a communicator: call tgb200_comm_init_rank / tgb200_set_comm, or drive "
                                   "step_begin / all-reduce / step_end yourself");
@@ -1409,9 +1383,8 @@ extern "C" int tgb200_run(tgb200_mapper* h, int32_t n_steps, float lr, void* str
   CKS(fork_streams(h, (cudaStream_t)stream));
   h->defer_join = true;                      // iterations chain through the handle's own streams and events
   int st = TGB200_OK;
-  static const bool kPrefetch = !(getenv("TGB200_PREFETCH_FWD") && atoi(getenv("TGB200_PREFETCH_FWD")) == 0);
   for (int i = 0; i < n_steps && st == TGB200_OK; ++i) {
-    h->prefetch_next = kPrefetch && i + 1 < n_steps;
+    h->prefetch_next = i + 1 < n_steps;
     st = tgb200_step_begin(h, stream);
     if (st == TGB200_OK && sharded) st = exchange_partials(h, work_stream(h, (cudaStream_t)stream));
     if (st == TGB200_OK) st = tgb200_step_end(h, lr, stream);
@@ -1448,16 +1421,16 @@ extern "C" int tgb200_get_mapping(tgb200_mapper* h, float* out, void* stream) {
   // softmax(M) in fp32 (:406-407), through device memory the iterations leave idle between calls -- no allocation here:
   //   fp32 mode          Pf (the forward operand itself)
   //   bf16x3 mode        the three bf16 P planes (6 B/element, rewritten by every forward pass)
-  //   bf16 staged mode   dq (2 B/element: half of the rows at a time)
+  //   bf16 mode          dq (2 B/element: half of the rows at a time)
   const size_t nv = (size_t)h->N * h->ld;
   DevBuf<float> tmp;
   float* scratch = h->Pf.p;
   size_t cap_elems = nv;
   if (h->x3) { scratch = reinterpret_cast<float*>(h->Pb.p); cap_elems = 3 * nv / 2; }
-  else if (h->staged) { scratch = reinterpret_cast<float*>(h->dq.p); cap_elems = nv / 2; }
+  else if (h->bf16) { scratch = reinterpret_cast<float*>(h->dq.p); cap_elems = nv / 2; }
   int blk = (int)(cap_elems / (size_t)h->ld);
   if (blk > h->N) blk = h->N;
-  if (blk < 1) { CKS(tmp.alloc((size_t)h->ld, false)); scratch = tmp.p; blk = 1; }     // one-row mapping in staged mode
+  if (blk < 1) { CKS(tmp.alloc((size_t)h->ld, false)); scratch = tmp.p; blk = 1; }     // one-row mapping in bf16 mode
   for (int r0 = 0; r0 < h->N; r0 += blk) {
     const int nr = h->N - r0 < blk ? h->N - r0 : blk;
     CKS(launch_softmax_rows<float>(h, s, scratch, 0, nullptr, Split3{nullptr, 0}, r0, nr));
@@ -1468,18 +1441,27 @@ extern "C" int tgb200_get_mapping(tgb200_mapper* h, float* out, void* stream) {
   return TGB200_OK;
 }
 
+// fp32 staging of the bf16 first moment between the caller and `mb`: the idle dq buffer, half of the rows at a time
+// (`one_row` for a one-row mapping)
+static int moment_scratch(tgb200_mapper* h, DevBuf<float>& one_row, float** scratch, int* blk) {
+  *scratch = reinterpret_cast<float*>(h->dq.p);
+  *blk = h->N / 2;
+  if (*blk < 1) { CKS(one_row.alloc((size_t)h->ld, false)); *scratch = one_row.p; *blk = 1; }
+  return TGB200_OK;
+}
+
 extern "C" int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream) {
   if (!h) return fail(TGB200_ERR_INVALID, "null handle");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
   const size_t w = (size_t)h->V * sizeof(float), pitch = (size_t)h->ld * sizeof(float);
   if (M) CK(cudaMemcpy2DAsync(M, w, h->M.p, pitch, w, h->N, cudaMemcpyDefault, s));
-  if (m && !h->staged) CK(cudaMemcpy2DAsync(m, w, h->m.p, pitch, w, h->N, cudaMemcpyDefault, s));
-  if (m && h->staged) {       // bf16 first moment -> fp32 for the caller, through the idle dq buffer (half of the rows at a time)
-    float* scratch = reinterpret_cast<float*>(h->dq.p);
+  if (m && !h->bf16) CK(cudaMemcpy2DAsync(m, w, h->m.p, pitch, w, h->N, cudaMemcpyDefault, s));
+  if (m && h->bf16) {         // bf16 first moment -> fp32 for the caller
+    float* scratch;
+    int blk;
     DevBuf<float> one_row;
-    int blk = h->N / 2;
-    if (blk < 1) { CKS(one_row.alloc((size_t)h->ld, false)); scratch = one_row.p; blk = 1; }
+    CKS(moment_scratch(h, one_row, &scratch, &blk));
     for (int r0 = 0; r0 < h->N; r0 += blk) {
       const int nr = h->N - r0 < blk ? h->N - r0 : blk;
       const long long n = (long long)nr * h->ld;
@@ -1501,16 +1483,16 @@ extern "C" int tgb200_set_state(tgb200_mapper* h, const float* M, const float* m
   CK(cudaSetDevice(h->cfg.device));
   const size_t w = (size_t)h->V * sizeof(float), pitch = (size_t)h->ld * sizeof(float);
   if (M) {
-    CK(cudaMemcpy2DAsync(h->M.p, pitch, M, w, w, h->N, cudaMemcpyDefault, s)); h->have_mapping = true; h->p_state = 0;
+    CK(cudaMemcpy2DAsync(h->M.p, pitch, M, w, w, h->N, cudaMemcpyDefault, s)); h->have_mapping = true; h->p_state = PState::stale;
     h->fwd_ahead = false;
-    if (h->staged) CK(cudaMemsetAsync(h->rcenter.p, 0, h->rcenter.n * sizeof(float), s));
+    if (h->bf16) CK(cudaMemsetAsync(h->rcenter.p, 0, h->rcenter.n * sizeof(float), s));
   }
-  if (m && !h->staged) CK(cudaMemcpy2DAsync(h->m.p, pitch, m, w, w, h->N, cudaMemcpyDefault, s));
-  if (m && h->staged) {       // fp32 from the caller -> bf16 (exact for values that came out of tgb200_get_state)
-    float* scratch = reinterpret_cast<float*>(h->dq.p);
+  if (m && !h->bf16) CK(cudaMemcpy2DAsync(h->m.p, pitch, m, w, w, h->N, cudaMemcpyDefault, s));
+  if (m && h->bf16) {         // fp32 from the caller -> bf16 (exact for values that came out of tgb200_get_state)
+    float* scratch;
+    int blk;
     DevBuf<float> one_row;
-    int blk = h->N / 2;
-    if (blk < 1) { CKS(one_row.alloc((size_t)h->ld)); scratch = one_row.p; blk = 1; }
+    CKS(moment_scratch(h, one_row, &scratch, &blk));
     for (int r0 = 0; r0 < h->N; r0 += blk) {
       const int nr = h->N - r0 < blk ? h->N - r0 : blk;
       const long long n = (long long)nr * h->ld;
@@ -1600,21 +1582,15 @@ extern "C" int tgb200_validation_terms(tgb200_mapper* h, float* out4, void* stre
   if (h->cfg.n_cells_global != h->N) return fail(TGB200_ERR_UNSUPPORTED, "validation_terms on a sharded handle");
   // _val_loss_fn (:311-356): a second forward on the train matrices.  bf16 mode: re-run the exact row pass so that the
   // per-row entropy exists whatever lambda_r is (in steady state it is only carried when the entropy term is on)
-  if (h->bf16) { h->p_state = 0; h->fwd_ahead = false; }
+  if (h->bf16) { h->p_state = PState::stale; h->fwd_ahead = false; }
   CKS(forward_pass(h, s, 1));
   LossParams p = make_loss_params(h);
-  DevBuf<float> rowpart, coefAr, coefBr, hist, gnz;
+  DevBuf<float> rowpart, coefAr, coefBr, hist;
   CKS(rowpart.alloc((size_t)h->ncolchunk * h->V * 2)); CKS(coefAr.alloc(h->V)); CKS(coefBr.alloc(h->V));
   CKS(hist.alloc(TGB200_HIST_COLS));
   p.rowpart = rowpart.p; p.coefAr = coefAr.p; p.coefBr = coefBr.p;
   p.lam_g2 = 1.f; p.lam_g1 = 1.f; p.lam_nb = 0.f; p.lam_go = 0.f; p.lam_ct = 0.f; p.density_mode = 0;
-  dim3 rgrid(h->nredchunk, h->nchunk);
-  const float* part = h->fwd_splits > 1 ? h->Ypart.p : h->Y.p;
-  k_loss_reduce<<<rgrid, kLossCols, 0, s>>>(p, part, h->fwd_splits, 1, h->loss_rows);
-  LAUNCH_CHECK("loss_reduce");
-  k_col_finalize<<<dim3((unsigned)ceil_div(h->Ke, 128), 3), 128, 0, s>>>(h->colpart.p, h->nchunk, 3, h->Ke, h->colfin.p);
-  LAUNCH_CHECK("col_finalize");
-  p.colpart = h->colfin.p;
+  CKS(reduce_columns(h, s, p, true, 1));
   k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, nullptr, nullptr, h->N, h->Y.p + (size_t)h->V * h->Ke);
   LAUNCH_CHECK("row_scalar_reduce");
   k_loss_scalars<<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist.p);
@@ -1659,28 +1635,30 @@ extern "C" int tgb200_profile_step(tgb200_mapper* h, float lr, void* stream, con
   if (!h || !names || !ms || !n) return fail(TGB200_ERR_INVALID, "null argument");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
-  KernelTimer t;
   cudaEvent_t e0;
   CK(cudaEventCreate(&e0));
   CK(cudaStreamSynchronize(s));
   CK(cudaEventRecord(e0, s));
-  h->timer = &t;
+  // the step's launches are appended to the records; a timeline recording in progress keeps them
+  const bool timeline = h->recording;
+  const size_t first = h->records.size();
+  h->recording = true;
   h->serial = true;                          // one stream, one kernel at a time: clean per-kernel durations
   int st = tgb200_step_begin(h, stream);
   if (st == TGB200_OK) st = tgb200_step_end(h, lr, stream);
   h->serial = false;
-  h->timer = nullptr;
+  h->recording = timeline;
   cudaStreamSynchronize(s);
   int cnt = 0;
   cudaEvent_t prev = e0;
-  for (size_t i = 0; i < t.ev.size(); ++i) {
+  for (size_t i = first; i < h->records.size(); ++i) {
     float f = 0.f;
-    cudaEventElapsedTime(&f, prev, t.ev[i]);
-    if (cnt < cap) { names[cnt] = t.names[i]; ms[cnt] = f; cnt++; }
-    prev = t.ev[i];
+    cudaEventElapsedTime(&f, prev, h->records[i].ev);
+    if (cnt < cap) { names[cnt] = h->records[i].name; ms[cnt] = f; cnt++; }
+    prev = h->records[i].ev;
   }
   cudaEventDestroy(e0);
-  for (auto e : t.ev) cudaEventDestroy(e);
+  if (!timeline) h->drop_records(first);
   *n = cnt;
   return st;
 }
@@ -1692,16 +1670,27 @@ extern "C" int tgb200_debug_timeline(tgb200_mapper* h, int32_t enable, const cha
   CK(cudaDeviceSynchronize());
   if (!enable) {
     int cnt = 0;
-    for (size_t i = 0; i < h->tl_events.size(); ++i) {
+    for (const LaunchRecord& r : h->records) {
       float f = 0.f;
-      cudaEventElapsedTime(&f, h->tl_events[0], h->tl_events[i]);
-      if (names && streams && end_ms && cnt < cap) { names[cnt] = h->tl_names[i]; streams[cnt] = h->tl_streams[i]; end_ms[cnt] = f; cnt++; }
+      cudaEventElapsedTime(&f, h->records[0].ev, r.ev);
+      if (names && streams && end_ms && cnt < cap) { names[cnt] = r.name; streams[cnt] = r.stream; end_ms[cnt] = f; cnt++; }
     }
     if (n) *n = cnt;
   }
-  for (cudaEvent_t e : h->tl_events) cudaEventDestroy(e);
-  h->tl_events.clear(); h->tl_names.clear(); h->tl_streams.clear();
-  h->timeline_on = enable != 0;
+  h->drop_records(0);
+  h->recording = enable != 0;
+  return TGB200_OK;
+}
+
+// n elements of `planes` bf16 planes, summed from the last plane to the first in fp32 on the host
+static int widen_bf16(const __nv_bfloat16* src, int64_t n, int planes, float* out) {
+  std::vector<__nv_bfloat16> tmp((size_t)n * planes);
+  CK(cudaMemcpy(tmp.data(), src, tmp.size() * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
+  for (int64_t i = 0; i < n; ++i) {
+    float acc = __bfloat162float(tmp[(size_t)(planes - 1) * n + i]);
+    for (int pl = planes - 2; pl >= 0; --pl) acc += __bfloat162float(tmp[(size_t)pl * n + i]);
+    out[i] = acc;
+  }
   return TGB200_OK;
 }
 
@@ -1717,31 +1706,22 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
   else if (nm == "dY") {
     src = h->dY.p; cnt = vk;
     if (h->tcm && out_host) {     // only the bf16 copy (or its three planes) exists on the tensor-core paths
-      const int planes = h->x3 ? 3 : 1;
-      std::vector<__nv_bfloat16> tmp((size_t)vk * planes);
       if (cap < cnt) return fail(TGB200_ERR_INVALID, "buffer 'dY' needs %lld floats", (long long)cnt);
-      CK(cudaMemcpy(tmp.data(), h->dYb.p, (size_t)vk * planes * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
-      for (int64_t i = 0; i < vk; ++i) {
-        float acc = 0.f;
-        for (int pl = planes - 1; pl >= 0; --pl) acc += __bfloat162float(tmp[(size_t)pl * vk + (size_t)i]);
-        out_host[i] = acc;
-      }
+      CKS(widen_bf16(h->dYb.p, vk, h->x3 ? 3 : 1, out_host));
       *n = cnt;
       return TGB200_OK;
     }
   }
-  else if ((nm == "dq" && h->staged) || (nm == "Pb" && h->bf16)) {    // N x ld bf16, widened
+  else if ((nm == "dq" || nm == "Pb") && h->bf16) {    // N x ld bf16, widened
     cnt = (int64_t)h->N * h->ld;
     *n = cnt;
     if (out_host) {
       if (cap < cnt) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)cnt);
-      std::vector<__nv_bfloat16> tmp((size_t)cnt);
-      CK(cudaMemcpy(tmp.data(), nm == "dq" ? h->dq.p : h->Pb.p, (size_t)cnt * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
-      for (int64_t i = 0; i < cnt; ++i) out_host[i] = __bfloat162float(tmp[(size_t)i]);
+      CKS(widen_bf16(nm == "dq" ? h->dq.p : h->Pb.p, cnt, 1, out_host));
     }
     return TGB200_OK;
   }
-  else if (nm == "rcenter" && h->staged) { src = h->rcenter.p; cnt = h->N; }
+  else if (nm == "rcenter" && h->bf16) { src = h->rcenter.p; cnt = h->N; }
   else if (nm == "rdot") { src = h->rdot.p; cnt = h->N; }
   else if (nm == "Sx") { src = h->Sx.p; cnt = (int64_t)h->N * h->Ke; }
   else if (nm == "shape") {   // Ke, ld, fwd_splits, r_parts
@@ -1772,8 +1752,8 @@ extern "C" int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, doub
   const double N = h->N, V = h->V, K = h->K, T = h->T;
   const double sS = h->bf16 ? 2.0 : 4.0;
   // SURVEY.md 8(d): 28 N V = M read in forward (4) + M, m, v read and written (24); with the first moment kept in bf16
-  // (staged bf16 mode) m costs 2 + 2 instead of 4 + 4 -> 24 N V ("if the moments are kept in BF16 ... state which")
-  if (hbm_bytes) *hbm_bytes = (h->staged ? 24.0 : 28.0) * N * V + 2.0 * sS * N * K + 8.0 * V * K;
+  // (bf16 mode) m costs 2 + 2 instead of 4 + 4 -> 24 N V ("if the moments are kept in BF16 ... state which")
+  if (hbm_bytes) *hbm_bytes = (h->bf16 ? 24.0 : 28.0) * N * V + 2.0 * sS * N * K + 8.0 * V * K;
   if (flops) *flops = 4.0 * N * V * K + (h->cfg.lambda_ct_islands > 0.f ? 4.0 * N * V * T : 0.0);
   return TGB200_OK;
 }

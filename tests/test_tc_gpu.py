@@ -166,10 +166,11 @@ def test_project_multi_chunk_matches_float64(precision):
 
 
 @pytest.mark.parametrize("precision,tol", [("fp32", 2e-6), ("bf16x3", 2e-6), ("bf16", 1e-4)])
-def test_pair_kernel_with_regularisers_matches_oracle(precision, tol):
-    """>= 2048 cells selects the CTA-pair backward kernel (cta_group::2); 2100 % 256 = 52 leaves the second CTA of the
-    last pair entirely out of range, 300 voxels leave a ragged column tile, and lambda_r / lambda_g2 take the epilogue
-    off its packed fast path.  Loss trajectory vs the oracle (observed: 2e-7 in fp32 / bf16x3, 1.2e-5 in bf16)."""
+def test_ragged_tiles_with_regularisers_matches_oracle(precision, tol):
+    """2100 cells leave a last 128-row tile of 52 rows in the backward contraction and a ragged k-block in the forward,
+    300 voxels leave a ragged 256-column tile, lambda_r takes the streaming update off its plain fast path, and
+    lambda_g2 adds the voxel-wise term to dY_ext.  Loss trajectory vs the oracle (observed: 2e-7 in fp32 / bf16x3,
+    1.2e-5 in bf16)."""
     from tangram_b200 import Mapper
     N, V, K = 2100, 300, 70
     inp = synthetic_inputs(N, V, K, seed=3)

@@ -1,4 +1,4 @@
-"""Dev tool: completion times of every launch of a few steady-state iterations on the handle's two streams
+"""Dev tool: completion times of every launch of a few steady-state iterations on the handle's three streams
 (tgb200_debug_timeline) -- shows whether the streaming Adam kernel really runs under the contractions."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -8,11 +8,9 @@ import bench
 from tangram_b200 import _lib
 from tangram_b200.engine import Engine
 name = sys.argv[1] if len(sys.argv) > 1 else "c3"
-world = int(sys.argv[2]) if len(sys.argv) > 2 else 1      # > 1: rank 0's share of a `world`-way sharded run (needs TGB200_SKIP_EXCHANGE=1)
-Ng, V, K, T, clusters, _ = bench.WORKLOADS[name]
-N = bench.shard_rows_for(Ng, 0, world)[1] if world > 1 else Ng
+N, V, K, T, clusters, _ = bench.WORKLOADS[name]
 inp = bench.gen_inputs(name, 0, N)
-eng = Engine(N, V, K, precision="bf16", density_mode=_lib.DENSITY_CELLS, n_cells_global=Ng)
+eng = Engine(N, V, K, precision="bf16", density_mode=_lib.DENSITY_CELLS)
 eng.set_expression(inp["S"], inp["G"]); eng.set_density(inp["d"])
 eng.init_mapping_normal(1234)
 eng.run(5)

@@ -12,9 +12,7 @@ import torch
 P = torch.softmax(torch.tensor(M0, dtype=torch.float64), dim=1)
 Y64 = (P.t() @ torch.tensor(S, dtype=torch.float64)).numpy()
 K = S.shape[1]
-for prec, env in (("fp32", None), ("bf16x3", None), ("bf16", None)):
-    if env: os.environ["TGB200_FWD_SPLITS"] = env
-    else: os.environ.pop("TGB200_FWD_SPLITS", None)
+for prec in ("fp32", "bf16x3", "bf16"):
     m = Mapper(S=S, G=G, d=d, lambda_d=1.0, M0=M0, precision=prec, device="cuda:0")
     m.train(1, print_each=None)
     Ke = int(m._debug("shape")[0]); splits = int(m._debug("shape")[2])
