@@ -223,6 +223,22 @@ TGB200_API int tgb200_validation_terms(tgb200_mapper* h, float* out4_host, void*
  * X (n_cells x n_cols) row-major f32, host or device; fp32 accumulate. */
 TGB200_API int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, float* out, void* stream);
 
+/* Run-to-run agreement of R equally shaped arrays (the hyper-parameter tuner's metrics,
+ * tangram/mapping_parameter_tuning.py:42-82), in one streaming pass that reads every element once and allocates
+ * O(rows) scratch.  `arrays`: a HOST array of R DEVICE pointers (all on `device`), each rows x cols row-major f32 with
+ * leading dimension ld; 1 <= R <= 8.
+ *   pearson_out            R(R-1)/2 doubles (host or device; NULL to skip): np.corrcoef of the flattened arrays at
+ *                          np.tril_indices(R, -1), i.e. pearson_corr (:42-53); sums in fp64, reduced in a fixed order
+ *   vote_entropy_out       rows floats (host or device; NULL to skip): per row, the entropy of the R runs' argmax votes
+ *                          (first column on ties) over log(cols), vote_entropy (:55-69)
+ *   consensus_entropy_out  rows floats (host or device; NULL to skip): per row, the entropy of p / sum(p) with
+ *                          p = mean over runs, over log(cols), consensus_entropy (:71-82)
+ * Fails with TGB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  Bit-reproducible on a given device.
+ * Synchronous on `stream`. */
+TGB200_API int tgb200_agreement(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                double* pearson_out, float* vote_entropy_out, float* consensus_entropy_out,
+                                int32_t device, void* stream);
+
 /* Checkpoint / resume (the reference stubs this: `raise NotImplemented`, :151-153).
  * Any pointer may be NULL to skip it.  M, m, v: n_cells x n_voxels f32, host or device. */
 TGB200_API int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream);

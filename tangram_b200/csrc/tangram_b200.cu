@@ -19,6 +19,7 @@
 #include "gemm_tc.cuh"
 #include "adam_rows.cuh"
 #include "legacy_rng.cuh"
+#include "agreement.cuh"
 #include "mt19937_jump.h"
 #include "nccl_dl.h"
 
@@ -1755,5 +1756,86 @@ extern "C" int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, doub
   // (bf16 mode) m costs 2 + 2 instead of 4 + 4 -> 24 N V ("if the moments are kept in BF16 ... state which")
   if (hbm_bytes) *hbm_bytes = (h->bf16 ? 24.0 : 28.0) * N * V + 2.0 * sS * N * K + 8.0 * V * K;
   if (flops) *flops = 4.0 * N * V * K + (h->cfg.lambda_ct_islands > 0.f ? 4.0 * N * V * T : 0.0);
+  return TGB200_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Agreement of R runs (tangram/mapping_parameter_tuning.py:42-82): stateless, no handle.
+template <int R>
+static void launch_agreement(const AgrArgs& a, int grid, bool rows, cudaStream_t s) {
+  if (rows) k_agreement<R, true><<<grid, kAgrThreads, 0, s>>>(a);
+  else k_agreement<R, false><<<grid, kAgrThreads, 0, s>>>(a);
+}
+
+extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                double* pearson_out, float* vote_out, float* cons_out, int32_t device, void* stream) {
+  if (!arrays) return fail(TGB200_ERR_INVALID, "null argument");
+  if (R < 1 || R > kAgrMaxRuns) return fail(TGB200_ERR_INVALID, "R=%d runs, supported 1..%d", R, kAgrMaxRuns);
+  if (rows <= 0 || cols <= 0 || ld < cols || cols > INT32_MAX)
+    return fail(TGB200_ERR_INVALID, "bad shape rows=%lld cols=%lld ld=%lld", (long long)rows, (long long)cols, (long long)ld);
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    return fail(TGB200_ERR_NO_DEVICE, "no CUDA device visible: tangram_b200 has no CPU fallback");
+  }
+  if (device < 0 || device >= ndev) return fail(TGB200_ERR_INVALID, "device %d out of range (%d devices)", device, ndev);
+  int major = 0, minor = 0, n_sms = 0;           // attribute queries: cudaGetDeviceProperties costs milliseconds
+  CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
+  CK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+  CK(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
+  if (major != 9 || minor != 0)
+    return fail(TGB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+  CK(cudaSetDevice(device));
+  AgrArgs a{};
+  a.rows = rows; a.cols = cols; a.ld = ld;
+  a.vec = ld % 4 == 0;
+  for (int r = 0; r < R; ++r) {
+    if (!arrays[r]) return fail(TGB200_ERR_INVALID, "array %d is null", r);
+    cudaPointerAttributes at;
+    CK(cudaPointerGetAttributes(&at, arrays[r]));
+    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != device)
+      return fail(TGB200_ERR_INVALID, "array %d is not device memory of device %d", r, device);
+    a.x[r] = arrays[r];
+    if (reinterpret_cast<uintptr_t>(arrays[r]) % 16) a.vec = 0;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const bool per_row = vote_out || cons_out;
+  const int NS = R + R * (R + 1) / 2;
+  int per_sm = 0;
+#define AGR_OCC(RR) \
+  case RR: CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, per_row ? k_agreement<RR, true> : k_agreement<RR, false>, kAgrThreads, 0)); break;
+  switch (R) { AGR_OCC(1) AGR_OCC(2) AGR_OCC(3) AGR_OCC(4) AGR_OCC(5) AGR_OCC(6) AGR_OCC(7) AGR_OCC(8) }
+#undef AGR_OCC
+  const int warps = kAgrThreads / kWarp;
+  const int64_t need = ceil_div(rows, warps);
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)std::max(per_sm, 1) * n_sms));
+  // scratch is O(R^2 grid + rows): the per-block partials, the shifts, the correlations, the per-row results
+  DevBuf<double> shift, part, corr;
+  DevBuf<float> vote, cons;
+  CKS(shift.alloc(R, false)); CKS(part.alloc((size_t)grid * NS, false)); CKS(corr.alloc(R > 1 ? R * (R - 1) / 2 : 1, false));
+  if (vote_out) CKS(vote.alloc(rows, false));
+  if (cons_out) CKS(cons.alloc(rows, false));
+  a.shift = shift.p; a.part = part.p; a.vote = vote.p; a.cons = cons.p;
+  k_agreement_shift<<<R, kAgrThreads, 0, s>>>(a, shift.p);
+  CK(cudaGetLastError());
+  switch (R) {
+    case 1: launch_agreement<1>(a, grid, per_row, s); break;
+    case 2: launch_agreement<2>(a, grid, per_row, s); break;
+    case 3: launch_agreement<3>(a, grid, per_row, s); break;
+    case 4: launch_agreement<4>(a, grid, per_row, s); break;
+    case 5: launch_agreement<5>(a, grid, per_row, s); break;
+    case 6: launch_agreement<6>(a, grid, per_row, s); break;
+    case 7: launch_agreement<7>(a, grid, per_row, s); break;
+    default: launch_agreement<8>(a, grid, per_row, s); break;
+  }
+  CK(cudaGetLastError());
+  if (R > 1) {
+    k_agreement_finish<<<1, 64, 0, s>>>(part.p, grid, R, (double)rows * (double)cols, corr.p);
+    CK(cudaGetLastError());
+    if (pearson_out) CK(cudaMemcpyAsync(pearson_out, corr.p, sizeof(double) * R * (R - 1) / 2, cudaMemcpyDefault, s));
+  }
+  if (vote_out) CK(cudaMemcpyAsync(vote_out, vote.p, sizeof(float) * rows, cudaMemcpyDefault, s));
+  if (cons_out) CK(cudaMemcpyAsync(cons_out, cons.p, sizeof(float) * rows, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
   return TGB200_OK;
 }

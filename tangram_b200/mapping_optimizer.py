@@ -17,6 +17,7 @@ Additions (keyword-only, all optional):
   n_cells_global         pre-sharded variant: S, M0, d_source, ct_encode already hold only this rank's rows
   train(..., resume=True)  continue with the Adam state of the previous train() call (the reference -- and the default
               here -- builds a fresh optimizer in every train() call, mapping_optimizer.py:373)
+  train(..., out=tensor)   write softmax(M) into a CUDA tensor instead of returning a host array
 """
 import ctypes
 
@@ -337,10 +338,12 @@ class Mapper:
         sharded_steps(_Eng(), n_steps, lr,
                       lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self._pg))   # the one exchange per step
 
-    def train(self, num_epochs, learning_rate=0.1, print_each=100, val_each=None, *, resume=False):
+    def train(self, num_epochs, learning_rate=0.1, print_each=100, val_each=None, *, resume=False, out=None):
         """mapping_optimizer.py:358-408.  Returns (softmax(M) as (N, V) f32 ndarray, history).
         Every call starts a fresh Adam (zero moments, t = 1) like the reference's `torch.optim.Adam([self.M])` at :373;
-        `resume=True` keeps the optimizer state of the previous call instead."""
+        `resume=True` keeps the optimizer state of the previous call instead.
+        `out`: a contiguous float32 CUDA tensor of shape (N, V) on this mapper's device; softmax(M) is written there
+        (device to device, no host copy) and `out` is returned in place of the ndarray."""
         import logging
         if print_each:
             logging.info(f"Printing scores every {print_each} epochs.")
@@ -351,13 +354,23 @@ class Mapper:
         _lib.check(self._lib.tgb200_history_len(self._h, ctypes.byref(first)))
         first = first.value
         lr = float(learning_rate)
+        if out is not None:
+            self._check_out(out)
+            return self._train_loop(num_epochs, lr, print_each, val_each, first, training_history, None, out)
         result = _ResultBuffer(self._lib, (self.n_cells, self.n_voxels), self._cfg.device)
         try:
             return self._train_loop(num_epochs, lr, print_each, val_each, first, training_history, result)
         finally:
             result.release()
 
-    def _train_loop(self, num_epochs, lr, print_each, val_each, first, training_history, result):
+    def _check_out(self, out):
+        import torch
+        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.device.index == self._cfg.device):
+            raise TypeError(f"out must be a CUDA tensor on cuda:{self._cfg.device}")
+        if out.dtype != torch.float32 or tuple(out.shape) != (self.n_cells, self.n_voxels) or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous float32 tensor of shape {(self.n_cells, self.n_voxels)}")
+
+    def _train_loop(self, num_epochs, lr, print_each, val_each, first, training_history, result, out=None):
         t = 0
         while t < num_epochs:
             if val_each is not None:
@@ -381,7 +394,7 @@ class Mapper:
         for c, key in enumerate(_HIST_KEYS[1:], start=1):
             training_history[key] = [float(x) for x in rows[:, c]]
         self.history_matrix = rows
-        output = result.ready()
+        output = result.ready() if out is None else out
         _lib.check(self._lib.tgb200_get_mapping(self._h, _lib.ptr(output), None))
         return output, training_history
 

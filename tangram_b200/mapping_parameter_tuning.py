@@ -1,0 +1,192 @@
+"""
+The hyper-parameter tuner's trial (Tangram's tangram/mapping_parameter_tuning.py:42-139) on the sm_90a (H100) library:
+the three run-to-run metrics and `train_multiple_Mapper`, which trains one configuration several times and scores how
+well the runs agree.
+
+    pearson_corr(cube)        (R(R-1)/2,) pairwise Pearson correlations of the flattened runs, np.tril_indices order
+    vote_entropy(cube)        (N,) normalised entropy of the runs' argmax votes per row
+    consensus_entropy(cube)   (N,) normalised entropy of the mean over runs per row
+
+`cube` is an (R, N, V) numpy array or CUDA tensor (or a sequence of R (N, V) ones); all three run on the device in one
+streaming pass each (tgb200_agreement), with no N x V scratch and no float64 copy of the cube.  There is no CPU path.
+
+    metrics = train_multiple_Mapper(config, data)     # the five numbers the reference reports to ray.train.report
+
+makes a Ray trainable a one-line wrapper.  The Ray / Optuna driver `mapping_hyperparameter_tuning` itself stays with the
+reference.
+"""
+import ctypes
+
+import numpy as np
+
+from . import _lib
+from .mapping_optimizer import Mapper, _VAL_KEYS
+
+_CONFIG_LAMBDAS = ["lambda_d", "lambda_g1", "lambda_g2", "lambda_neighborhood_g1", "lambda_r", "lambda_l1",
+                   "lambda_l2", "lambda_ct_islands", "lambda_getis_ord"]     # :97
+_GENE_SIM = _VAL_KEYS.index("val_gene_sim")
+# device bytes per mapping element one Mapper handle holds at most (M, m, v, operands, a projection's P planes)
+_HANDLE_BYTES_PER_ELEMENT = 28
+
+
+def _require_device(device):
+    """-> ordinal of a visible CUDA device, or TangramB200Error: there is no CPU fallback."""
+    import torch
+    s = str(device)
+    if not s.startswith("cuda"):
+        raise _lib.TangramB200Error(f"tangram_b200 runs on H100 GPUs only (device={device!r}); no CPU fallback")
+    if not torch.cuda.is_available():
+        raise _lib.TangramB200Error("no CUDA device visible: tangram_b200 has no CPU fallback")
+    return int(s.split(":")[1]) if ":" in s else torch.cuda.current_device()
+
+
+def _runs_on_device(cube, device):
+    """(R, N, V) ndarray / CUDA tensor / sequence of (N, V) -> (list of R CUDA tensors with unit column stride and equal
+    row stride, device ordinal).  Host data is copied to the device once, as float32."""
+    import torch
+    if isinstance(cube, torch.Tensor) and cube.is_cuda:
+        dev = cube.device.index
+        runs = list(cube.unbind(0)) if cube.dim() == 3 else None
+    elif isinstance(cube, (list, tuple)) and cube and all(isinstance(c, torch.Tensor) and c.is_cuda for c in cube):
+        dev = cube[0].device.index
+        runs = list(cube)
+    else:
+        dev = _require_device("cuda" if device is None else device)
+        arr = np.asarray(cube if not isinstance(cube, (list, tuple)) else np.stack([np.asarray(c) for c in cube]))
+        if arr.ndim != 3:
+            raise ValueError(f"expected an (R, N, V) cube, got shape {arr.shape}")
+        runs = list(torch.from_numpy(np.ascontiguousarray(arr, dtype=np.float32)).to(f"cuda:{dev}").unbind(0))
+    if runs is None or any(r.dim() != 2 for r in runs):
+        raise ValueError("expected an (R, N, V) cube or a sequence of R (N, V) arrays")
+    shape = tuple(runs[0].shape)
+    out = []
+    for r in runs:
+        if tuple(r.shape) != shape or r.device.index != dev:
+            raise ValueError("all runs must have the same shape and device")
+        r = r.float()
+        if r.stride(1) != 1 or (shape[0] > 1 and r.stride(0) != runs[0].stride(0)) or r.stride(0) < shape[1]:
+            r = r.contiguous()
+        out.append(r)
+    if len({r.stride(0) for r in out}) > 1:
+        out = [r.contiguous() for r in out]
+    return out, dev
+
+
+def agreement(cube, *, pearson=True, vote=False, consensus=False, device=None):
+    """One pass of tgb200_agreement over the R runs of `cube`: -> (pearson (R(R-1)/2,) float64 or None,
+    vote entropy (N,) float32 or None, consensus entropy (N,) float32 or None).  `device` places host data (default:
+    the current CUDA device); device data is read where it lives."""
+    import torch
+    runs, dev = _runs_on_device(cube, device)
+    R = len(runs)
+    rows, cols = runs[0].shape
+    lib = _lib.load()
+    ptrs = (_lib._P * R)(*[r.data_ptr() for r in runs])
+    p = np.empty(R * (R - 1) // 2, dtype=np.float64) if pearson else None
+    v = np.empty(rows, dtype=np.float32) if vote else None
+    c = np.empty(rows, dtype=np.float32) if consensus else None
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(lib.tgb200_agreement(ptrs, R, rows, cols, runs[0].stride(0), _lib.ptr(p), _lib.ptr(v), _lib.ptr(c),
+                                    dev, stream))
+    return p, v, c
+
+
+def pearson_corr(cube, *, device=None):
+    """:42-53 -- all pairwise Pearson correlations of the R flattened runs, (R(R-1)/2,) float64 in np.tril_indices(R, -1)
+    order, as np.corrcoef computes them (fp64 sums)."""
+    return agreement(cube, device=device)[0]
+
+
+def vote_entropy(pred_probs_cube, *, device=None):
+    """:55-69 -- per row, the entropy of the runs' argmax votes (first column on ties) normalised by log(V): (N,)."""
+    return agreement(pred_probs_cube, pearson=False, vote=True, device=device)[1]
+
+
+def consensus_entropy(pred_probs_cube, *, device=None):
+    """:71-82 -- per row, the entropy of the mean over runs (renormalised, 0 log 0 = 0) normalised by log(V): (N,)."""
+    return agreement(pred_probs_cube, pearson=False, consensus=True, device=device)[2]
+
+
+def _val_gene_sim(mapper):
+    vals = np.zeros(4, dtype=np.float32)
+    _lib.check(mapper._lib.tgb200_validation_terms(mapper._h, _lib.ptr(vals), None))
+    return float(vals[_GENE_SIM])
+
+
+def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details=None):
+    """:86-139 -- train the configuration `config` n_runs times (random_state = 0, 1, 2, ...) on `data`, the reference's
+    12-entry list [S, G, d_source, d, device, print_each, voxel_weights, ct_encode, neighborhood_filter, spatial_weights,
+    train_genes_idx, val_genes_idx], and return the five metrics the reference reports:
+        cell_map_consistency   mean pairwise Pearson correlation of the mappings
+        cell_map_agreement     1 - mean vote entropy of the mappings
+        cell_map_certainty     1 - mean consensus entropy of the mappings
+        gene_expr_consistency  mean pairwise Pearson correlation of the projected validation genes
+        gene_expr_correctness  mean over runs of the final validation gene score (val_gene_sim after the last update)
+    As in the reference, run 0 is unseeded (random_state=0 is falsy, mapping_optimizer.py:148) and continues numpy's
+    global generator.  The mappings stay on the device (an R x N x V cube), the validation genes are projected there,
+    and each run's handle is released before the next starts.  `details`, if a dict, receives the device cubes
+    ("cell_cube" R x N x V, "gene_cube" R x V x n_val), the per-run "val_gene_sim" and the seconds spent in "train_s",
+    "project_s" and "score_s"."""
+    import time
+
+    import torch
+    (S, G, d_source, d, device, print_each, voxel_weights, ct_encode, neighborhood_filter, spatial_weights,
+     train_genes_idx, val_genes_idx) = data
+    dev = _require_device(device)
+    hyperparameters = {"d_source": d_source}
+    for param in _CONFIG_LAMBDAS:
+        if param in config:
+            hyperparameters[param] = config[param]
+    learning_rate = config.get("learning_rate", 0.1)
+    num_epochs = config.get("num_epochs", 1000)
+
+    S = np.asarray(S, dtype=np.float32)
+    N, V = S.shape[0], np.shape(G)[0]
+    S_val = np.ascontiguousarray(S[:, val_genes_idx] if val_genes_idx is not None else S)
+    n_val = S_val.shape[1]
+    k_train = len(train_genes_idx) if train_genes_idx is not None else S.shape[1]
+    cube_bytes = 4 * n_runs * N * V + 4 * n_runs * V * n_val
+    handle_bytes = _HANDLE_BYTES_PER_ELEMENT * N * V + 16 * (N + V) * (k_train + n_val)
+    free, _ = torch.cuda.mem_get_info(dev)
+    if cube_bytes + handle_bytes > free:
+        raise _lib.TangramB200Error(
+            f"train_multiple_Mapper needs about {(cube_bytes + handle_bytes) / 2**30:.1f} GiB on cuda:{dev} "
+            f"({n_runs} mappings of {N} x {V} = {cube_bytes / 2**30:.1f} GiB, plus one mapper of "
+            f"{handle_bytes / 2**30:.1f} GiB); {free / 2**30:.1f} GiB are free")
+
+    t_train = t_proj = 0.0
+    cell_cube = torch.empty((n_runs, N, V), dtype=torch.float32, device=f"cuda:{dev}")
+    gene_cube = torch.empty((n_runs, V, n_val), dtype=torch.float32, device=f"cuda:{dev}")   # (S_val^T P)^T
+    val_gene_scores = []
+    for run in range(n_runs):
+        t0 = time.perf_counter()
+        mapper = Mapper(S=S, G=G, d=d, train_genes_idx=train_genes_idx, val_genes_idx=val_genes_idx,
+                        voxel_weights=voxel_weights, neighborhood_filter=neighborhood_filter, ct_encode=ct_encode,
+                        spatial_weights=spatial_weights, device=f"cuda:{dev}", random_state=run, precision=precision,
+                        **hyperparameters)
+        try:
+            # the reference validates after every update (val_each=1) and keeps only the last score: one evaluation
+            # after the final update is the same number
+            mapper.train(num_epochs, learning_rate=learning_rate, print_each=print_each, out=cell_cube[run])
+            val_gene_scores.append(_val_gene_sim(mapper))
+            t1 = time.perf_counter()
+            # :134 -- S[:, val]^T @ mapping, stored transposed: Pearson over flattened runs does not see the order
+            _lib.check(mapper._lib.tgb200_project(mapper._h, _lib.ptr(S_val), n_val, _lib.ptr(gene_cube[run]), None))
+            t2 = time.perf_counter()
+        finally:
+            mapper.release()
+        t_train += t1 - t0
+        t_proj += t2 - t1
+
+    t0 = time.perf_counter()
+    cell_p, cell_v, cell_c = agreement(cell_cube, vote=True, consensus=True)
+    gene_p = agreement(gene_cube)[0]
+    t_score = time.perf_counter() - t0
+    if isinstance(details, dict):
+        details.update(cell_cube=cell_cube, gene_cube=gene_cube, val_gene_sim=val_gene_scores, train_s=t_train,
+                       project_s=t_proj, score_s=t_score)
+    return {"cell_map_consistency": float(cell_p.mean()),
+            "cell_map_agreement": float(1 - cell_v.astype(np.float64).mean()),
+            "cell_map_certainty": float(1 - cell_c.astype(np.float64).mean()),
+            "gene_expr_consistency": float(gene_p.mean()),
+            "gene_expr_correctness": float(np.mean(val_gene_scores))}
