@@ -239,6 +239,22 @@ TGB200_API int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
                                 double* pearson_out, float* vote_entropy_out, float* consensus_entropy_out,
                                 int32_t device, void* stream);
 
+/* Annotation transfer from cells onto space (tangram/utils.py:126-153 project_cell_annotations, 205-285
+ * count_cell_annotations, 820-842 cell_type_mapping), in one streaming pass over a DEVICE mapping `map` (rows x cols
+ * row-major f32, leading dimension ld >= cols, on `device`).  `labels_host`: a HOST array of `rows` int32 labels in
+ * [-1, n_labels); a row labelled -1 adds to no sum and gets no argmax.
+ *   sums_out    n_labels x cols doubles (host or device; NULL to skip): sums_out[t, j] = sum of map[i, j] over the rows
+ *               labelled t, in fp64 (the reference's int64 one-hot GEMM runs in float64); 0 for a label without rows
+ *   argmax_out  rows int32 (host or device; NULL to skip): per labelled row the first column holding its maximum, a NaN
+ *               counting as the maximum (np.argmax); -1 for unlabelled rows
+ * No atomics, partials reduced in a fixed order: bit-reproducible.  Scratch is about 8 (rows / 128 + n_labels) cols bytes
+ * for the sums and 8 rows ceil(cols / 1024) bytes for the argmax.  Fails with TGB200_ERR_INVALID (and a message in
+ * tgb200_last_error) for a label outside [-1, n_labels) or ld < cols, and with TGB200_ERR_NO_DEVICE without an sm_90
+ * device (no CPU fallback).  Synchronous on `stream`. */
+TGB200_API int tgb200_annotate(const float* map, int64_t rows, int64_t cols, int64_t ld,
+                               const int32_t* labels_host, int32_t n_labels,
+                               double* sums_out, int32_t* argmax_out, int32_t device, void* stream);
+
 /* Checkpoint / resume (the reference stubs this: `raise NotImplemented`, :151-153).
  * Any pointer may be NULL to skip it.  M, m, v: n_cells x n_voxels f32, host or device. */
 TGB200_API int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream);

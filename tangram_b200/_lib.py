@@ -94,6 +94,8 @@ SIGNATURES = {
     "tgb200_project": (ctypes.c_int, [_P, _P, ctypes.c_int64, _P, _P]),
     "tgb200_agreement": (ctypes.c_int, [ctypes.POINTER(_P), ctypes.c_int32, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                         _P, _P, _P, ctypes.c_int32, _P]),
+    "tgb200_annotate": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int32,
+                                       _P, _P, ctypes.c_int32, _P]),
     "tgb200_get_state":(ctypes.c_int, [_P, _P, _P, _P, _I64, _P]),
     "tgb200_set_state": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int64, _P]),
     "tgb200_kernel_launches": (ctypes.c_int, [_P, _I64]),

@@ -1,6 +1,6 @@
 """Minimal AnnData stand-in used when `anndata` is not installed (it is absent from the
 build image).  Only the surface that map_cells_to_space / project_genes / the reference's
-plot_utils touch: X, obs, var, uns, obsm, obsp, shape, obs_names / var_names,
+plot_utils touch: X, obs, var, uns, obsm, obsp, varm, shape, obs_names / var_names,
 `adata[:, genes]`, `adata[mask]`, copy().  If `anndata` is importable it is used instead."""
 import numpy as np
 import pandas as pd
@@ -11,8 +11,13 @@ except Exception:  # noqa: BLE001
     _RealAnnData = None
 
 
+def _take_rows(v, idx):
+    """Rows `idx` of a per-gene annotation: a DataFrame keeps its index and columns, anything else becomes an array."""
+    return v.iloc[idx] if isinstance(v, (pd.DataFrame, pd.Series)) else np.asarray(v)[idx]
+
+
 class MiniAnnData:
-    def __init__(self, X=None, obs=None, var=None, uns=None, obsm=None, obsp=None):
+    def __init__(self, X=None, obs=None, var=None, uns=None, obsm=None, obsp=None, varm=None):
         n_obs = X.shape[0] if X is not None else (len(obs) if obs is not None else 0)
         n_var = X.shape[1] if X is not None else (len(var) if var is not None else 0)
         self.X = X
@@ -21,6 +26,7 @@ class MiniAnnData:
         self.uns = uns if uns is not None else {}
         self.obsm = obsm if obsm is not None else {}
         self.obsp = obsp if obsp is not None else {}
+        self.varm = varm if varm is not None else {}
         if X is not None and (len(self.obs) != X.shape[0] or len(self.var) != X.shape[1]):
             raise ValueError("obs/var do not match X")
 
@@ -62,8 +68,7 @@ class MiniAnnData:
         if self.X is not None:
             self.X = self.X[:, c] if hasattr(self.X, "tocsr") else np.asarray(self.X)[:, c]
         self.var = self.var.iloc[c].copy()
-        if getattr(self, "varm", None):
-            self.varm = {k: np.asarray(v)[c] for k, v in self.varm.items()}
+        self.varm = {k: _take_rows(v, c) for k, v in self.varm.items()}
 
     def _rows(self, key, index):
         if isinstance(key, slice):
@@ -88,13 +93,14 @@ class MiniAnnData:
             X = X[r][:, c] if hasattr(X, "tocsr") else np.asarray(X)[np.ix_(r, c)]
         obsp = {k: v[r][:, r] for k, v in self.obsp.items()}
         obsm = {k: np.asarray(v)[r] for k, v in self.obsm.items()}
+        varm = {k: _take_rows(v, c) for k, v in self.varm.items()}
         return MiniAnnData(X=X, obs=self.obs.iloc[r].copy(), var=self.var.iloc[c].copy(), uns=self.uns,
-                           obsm=obsm, obsp=obsp)
+                           obsm=obsm, obsp=obsp, varm=varm)
 
     def copy(self):
         X = self.X.copy() if self.X is not None else None
         return MiniAnnData(X=X, obs=self.obs.copy(), var=self.var.copy(), uns=dict(self.uns),
-                           obsm=dict(self.obsm), obsp=dict(self.obsp))
+                           obsm=dict(self.obsm), obsp=dict(self.obsp), varm={k: v.copy() for k, v in self.varm.items()})
 
 
 def make_adata(X=None, obs=None, var=None, uns=None):

@@ -144,14 +144,7 @@ __global__ void __launch_bounds__(kAgrThreads) k_agreement(AgrArgs a) {
     if (kRows) {
       // argmax per run: largest value, first column on ties (np.argmax)
 #pragma unroll
-      for (int r = 0; r < R; ++r) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, acc.best[r], o);
-          const int oi = __shfl_xor_sync(0xffffffffu, acc.bidx[r], o);
-          if (ov > acc.best[r] || (ov == acc.best[r] && oi < acc.bidx[r])) { acc.best[r] = ov; acc.bidx[r] = oi; }
-        }
-      }
+      for (int r = 0; r < R; ++r) warp_argmax(acc.best[r], acc.bidx[r]);
       const double s = warp_sum_d(acc.csum), plogp = warp_sum_d(acc.cplogp);
       if (lane == 0) {
         const double inv_log_cols = 1.0 / log((double)cols);

@@ -23,6 +23,22 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// np.argmax's order on (value, column) pairs: a NaN beats every number, otherwise the larger value wins, and between
+// equal values (or two NaNs) the lower column wins.  -> does (v, i) take the place of (bv, bi)?
+__device__ __forceinline__ bool argmax_prefer(float v, int i, float bv, int bi) {
+  if (v != v) return bv == bv || i < bi;
+  return v > bv || (v == bv && i < bi);
+}
+// Warp-wide (value, column) reduction in that order; every lane ends with the winner.
+__device__ __forceinline__ void warp_argmax(float& best, int& idx) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+    if (argmax_prefer(ov, oi, best, idx)) { best = ov; idx = oi; }
+  }
+}
+
 // Block-wide reductions; `sh` needs >= 32 floats.  Result is broadcast to all threads.
 template <bool kMax>
 __device__ __forceinline__ float block_reduce(float v, float* sh) {

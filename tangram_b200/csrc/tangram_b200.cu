@@ -20,6 +20,7 @@
 #include "adam_rows.cuh"
 #include "legacy_rng.cuh"
 #include "agreement.cuh"
+#include "annotate.cuh"
 #include "mt19937_jump.h"
 #include "nccl_dl.h"
 
@@ -1760,7 +1761,35 @@ extern "C" int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, doub
 }
 
 // ---------------------------------------------------------------------------------------
-// Agreement of R runs (tangram/mapping_parameter_tuning.py:42-82): stateless, no handle.
+// Stateless entry points (no handle): the device checks they share.
+
+// Makes `device` current if it is a visible sm_90 device; *n_sms receives its SM count.
+static int use_sm90_device(int32_t device, int* n_sms) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    return fail(TGB200_ERR_NO_DEVICE, "no CUDA device visible: tangram_b200 has no CPU fallback");
+  }
+  if (device < 0 || device >= ndev) return fail(TGB200_ERR_INVALID, "device %d out of range (%d devices)", device, ndev);
+  int major = 0, minor = 0;                      // attribute queries: cudaGetDeviceProperties costs milliseconds
+  CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
+  CK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+  CK(cudaDeviceGetAttribute(n_sms, cudaDevAttrMultiProcessorCount, device));
+  if (major != 9 || minor != 0)
+    return fail(TGB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+  CK(cudaSetDevice(device));
+  return TGB200_OK;
+}
+
+static int require_device_memory(const void* p, int32_t device, const char* what) {
+  cudaPointerAttributes at;
+  CK(cudaPointerGetAttributes(&at, p));
+  if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != device)
+    return fail(TGB200_ERR_INVALID, "%s is not device memory of device %d", what, device);
+  return TGB200_OK;
+}
+
+// Agreement of R runs (tangram/mapping_parameter_tuning.py:42-82).
 template <int R>
 static void launch_agreement(const AgrArgs& a, int grid, bool rows, cudaStream_t s) {
   if (rows) k_agreement<R, true><<<grid, kAgrThreads, 0, s>>>(a);
@@ -1773,28 +1802,16 @@ extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
   if (R < 1 || R > kAgrMaxRuns) return fail(TGB200_ERR_INVALID, "R=%d runs, supported 1..%d", R, kAgrMaxRuns);
   if (rows <= 0 || cols <= 0 || ld < cols || cols > INT32_MAX)
     return fail(TGB200_ERR_INVALID, "bad shape rows=%lld cols=%lld ld=%lld", (long long)rows, (long long)cols, (long long)ld);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(TGB200_ERR_NO_DEVICE, "no CUDA device visible: tangram_b200 has no CPU fallback");
-  }
-  if (device < 0 || device >= ndev) return fail(TGB200_ERR_INVALID, "device %d out of range (%d devices)", device, ndev);
-  int major = 0, minor = 0, n_sms = 0;           // attribute queries: cudaGetDeviceProperties costs milliseconds
-  CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-  CK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-  CK(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
-  if (major != 9 || minor != 0)
-    return fail(TGB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
-  CK(cudaSetDevice(device));
+  int n_sms = 0;
+  CKS(use_sm90_device(device, &n_sms));
   AgrArgs a{};
   a.rows = rows; a.cols = cols; a.ld = ld;
   a.vec = ld % 4 == 0;
   for (int r = 0; r < R; ++r) {
     if (!arrays[r]) return fail(TGB200_ERR_INVALID, "array %d is null", r);
-    cudaPointerAttributes at;
-    CK(cudaPointerGetAttributes(&at, arrays[r]));
-    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != device)
-      return fail(TGB200_ERR_INVALID, "array %d is not device memory of device %d", r, device);
+    char what[32];
+    snprintf(what, sizeof(what), "array %d", r);
+    CKS(require_device_memory(arrays[r], device, what));
     a.x[r] = arrays[r];
     if (reinterpret_cast<uintptr_t>(arrays[r]) % 16) a.vec = 0;
   }
@@ -1836,6 +1853,92 @@ extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
   }
   if (vote_out) CK(cudaMemcpyAsync(vote_out, vote.p, sizeof(float) * rows, cudaMemcpyDefault, s));
   if (cons_out) CK(cudaMemcpyAsync(cons_out, cons.p, sizeof(float) * rows, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+// Label sums and row argmax of a mapping (tangram/utils.py:126-153, 205-285, 820-842).
+extern "C" int tgb200_annotate(const float* map, int64_t rows, int64_t cols, int64_t ld, const int32_t* labels,
+                               int32_t n_labels, double* sums_out, int32_t* argmax_out, int32_t device, void* stream) {
+  if (!map || !labels) return fail(TGB200_ERR_INVALID, "null argument");
+  if (rows <= 0 || cols <= 0 || ld < cols || rows > INT32_MAX || cols > INT32_MAX)
+    return fail(TGB200_ERR_INVALID, "bad shape rows=%lld cols=%lld ld=%lld", (long long)rows, (long long)cols, (long long)ld);
+  if (n_labels < 1) return fail(TGB200_ERR_INVALID, "n_labels=%d, must be at least 1", n_labels);
+  // stable counting sort of the labelled rows by label; each label's segment cut into items of kAnnChunk rows
+  std::vector<int> seg(n_labels + 1, 0);
+  for (int64_t i = 0; i < rows; ++i) {
+    const int32_t l = labels[i];
+    if (l < -1 || l >= n_labels)
+      return fail(TGB200_ERR_INVALID, "label %d of row %lld is outside [-1, %d)", l, (long long)i, n_labels);
+    if (l >= 0) ++seg[l + 1];
+  }
+  for (int t = 0; t < n_labels; ++t) seg[t + 1] += seg[t];
+  const int n_labelled = seg[n_labels];
+  std::vector<int> perm(std::max(n_labelled, 1)), next(seg.begin(), seg.end() - 1);
+  for (int64_t i = 0; i < rows; ++i)
+    if (labels[i] >= 0) perm[next[labels[i]]++] = (int)i;
+  std::vector<int> item_start, label_items(n_labels + 1);
+  for (int t = 0; t < n_labels; ++t) {
+    label_items[t] = (int)item_start.size();
+    for (int p = seg[t]; p < seg[t + 1]; p += kAnnChunk) item_start.push_back(p);
+  }
+  const int n_items = (int)item_start.size();
+  label_items[n_labels] = n_items;
+  item_start.push_back(n_labelled);
+
+  int n_sms = 0;
+  CKS(use_sm90_device(device, &n_sms));
+  CKS(require_device_memory(map, device, "the mapping"));
+  if (!sums_out && !argmax_out) return TGB200_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  AnnArgs a{};
+  a.map = map; a.cols = cols; a.ld = ld;
+  a.vec = ld % 4 == 0 && reinterpret_cast<uintptr_t>(map) % 16 == 0;
+  a.n_items = n_items;
+  a.n_slabs = (int)ceil_div(cols, kAnnSlab);
+  // scratch: the permutation and item tables, n_items x cols fp64 partials, n_labelled x slabs argmax partials
+  DevBuf<int> d_perm, d_items, d_label_items, d_argmax, amax_idx;
+  DevBuf<double> part, sums;
+  DevBuf<float> amax_val;
+  CKS(d_perm.alloc(perm.size(), false)); CKS(d_items.alloc(item_start.size(), false));
+  CK(cudaMemcpyAsync(d_perm.p, perm.data(), sizeof(int) * perm.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_items.p, item_start.data(), sizeof(int) * item_start.size(), cudaMemcpyHostToDevice, s));
+  a.perm = d_perm.p; a.item_start = d_items.p;
+  if (sums_out) {
+    CKS(d_label_items.alloc(label_items.size(), false));
+    CK(cudaMemcpyAsync(d_label_items.p, label_items.data(), sizeof(int) * label_items.size(), cudaMemcpyHostToDevice, s));
+    CKS(part.alloc(std::max<size_t>((size_t)n_items * cols, 1), false));
+    CKS(sums.alloc((size_t)n_labels * cols, false));
+    a.part = part.p;
+  }
+  if (argmax_out) {
+    CKS(amax_val.alloc(std::max<size_t>((size_t)n_labelled * a.n_slabs, 1), false));
+    CKS(amax_idx.alloc(std::max<size_t>((size_t)n_labelled * a.n_slabs, 1), false));
+    CKS(d_argmax.alloc(rows, false));
+    CK(cudaMemsetAsync(d_argmax.p, 0xff, sizeof(int) * rows, s));            // -1 for the unlabelled rows
+    a.amax_val = amax_val.p; a.amax_idx = amax_idx.p;
+  }
+  if (n_items > 0) {
+    const dim3 grid(a.n_slabs, std::min(n_items, 65535));
+    if (sums_out && argmax_out) k_annotate<true, true><<<grid, kAnnThreads, 0, s>>>(a);
+    else if (sums_out) k_annotate<true, false><<<grid, kAnnThreads, 0, s>>>(a);
+    else k_annotate<false, true><<<grid, kAnnThreads, 0, s>>>(a);
+    CK(cudaGetLastError());
+  }
+  if (sums_out) {
+    const dim3 grid((unsigned)ceil_div(cols, kAnnThreads), std::min(n_labels, 65535));
+    k_annotate_sums<<<grid, kAnnThreads, 0, s>>>(part.p, d_label_items.p, n_labels, cols, sums.p);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(sums_out, sums.p, sizeof(double) * n_labels * cols, cudaMemcpyDefault, s));
+  }
+  if (argmax_out) {
+    if (n_labelled > 0) {
+      const int grid = (int)std::min<int64_t>(ceil_div(n_labelled, kAnnThreads), (int64_t)8 * n_sms);
+      k_annotate_argmax<<<grid, kAnnThreads, 0, s>>>(amax_val.p, amax_idx.p, d_perm.p, n_labelled, a.n_slabs, d_argmax.p);
+      CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(argmax_out, d_argmax.p, sizeof(int32_t) * rows, cudaMemcpyDefault, s));
+  }
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
 }
