@@ -1,6 +1,6 @@
-"""Thin object wrapper over the C-ABI handle (include/tangram_b200.h) for callers that
-manage their own buffers (bench.py, multi-GPU drivers).  `Mapper` is the reference-shaped
-front end; this is the explicit one."""
+"""The one Python owner of a C-ABI handle (include/tangram_b200.h): every call that takes a `tgb200_mapper*` goes through
+`Engine`.  `Mapper` and `MapperConstrained` (the reference-shaped front ends) and the tuner build on it; callers that
+manage their own buffers (bench.py, multi-GPU drivers) use it directly."""
 import ctypes
 
 import numpy as np
@@ -8,9 +8,48 @@ import numpy as np
 from . import _lib
 
 
+def _device_index(device):
+    """Mapper's device: 'cuda' (device 0), 'cuda:1', torch.device -> ordinal.  'cpu' is refused: no CPU fallback."""
+    s = str(device)
+    if s.startswith("cuda"):
+        return int(s.split(":")[1]) if ":" in s else 0
+    raise ValueError(
+        f"tangram_b200.Mapper runs on H100 GPUs only (device={device!r}); "
+        "use the reference implementation for device='cpu'")
+
+
+def _require_device(device):
+    """The tuner's and annotation helpers' device: -> ordinal of a visible CUDA device ('cuda' is torch's current one),
+    or TangramB200Error: there is no CPU fallback."""
+    import torch
+    s = str(device)
+    if not s.startswith("cuda"):
+        raise _lib.TangramB200Error(f"tangram_b200 runs on H100 GPUs only (device={device!r}); no CPU fallback")
+    if not torch.cuda.is_available():
+        raise _lib.TangramB200Error("no CUDA device visible: tangram_b200 has no CPU fallback")
+    return int(s.split(":")[1]) if ":" in s else torch.cuda.current_device()
+
+
+def _csr(mat, n):
+    """n x n spatial operator -- dense ndarray (what the reference passes, mapping_utils.py:319-329), torch tensor or
+    scipy sparse -> CSR triplet (int32 indptr, int32 indices, float32 values) with sorted indices."""
+    import scipy.sparse as sp
+    if hasattr(mat, "detach"):
+        mat = mat.detach().cpu().numpy()
+    csr = mat.tocsr() if sp.issparse(mat) else sp.csr_matrix(np.asarray(mat))
+    if csr.shape != (n, n):
+        raise ValueError(f"spatial operator has shape {csr.shape}, expected {(n, n)}")
+    csr.sort_indices()
+    return (np.ascontiguousarray(csr.indptr, dtype=np.int32),
+            np.ascontiguousarray(csr.indices, dtype=np.int32),
+            np.ascontiguousarray(csr.data, dtype=np.float32))
+
+
 class Engine:
+    """Config fields not given default to 0, except lambda_g1 (1) and lambda_d (1 when there is a density)."""
+
     def __init__(self, n_cells, n_voxels, n_genes, *, n_types=0, n_cells_global=None, device=0,
-                 precision="fp32", density_mode=_lib.DENSITY_CELLS, **lambdas):
+                 precision="fp32", density_mode=_lib.DENSITY_CELLS, constrained=False, **lambdas):
         self._lib = _lib.load()
         cfg = _lib.Config()
         cfg.struct_size = ctypes.sizeof(_lib.Config)
@@ -22,16 +61,18 @@ class Engine:
         cfg.lambda_g1 = lambdas.pop("lambda_g1", 1.0)
         cfg.lambda_d = lambdas.pop("lambda_d", 1.0 if density_mode != _lib.DENSITY_NONE else 0.0)
         for k in ("lambda_g2", "lambda_r", "lambda_l1", "lambda_l2", "lambda_neighborhood_g1",
-                  "lambda_ct_islands", "lambda_getis_ord"):
+                  "lambda_ct_islands", "lambda_getis_ord", "lambda_count", "lambda_f_reg", "target_count"):
             setattr(cfg, k, lambdas.pop(k, 0.0))
         if lambdas:
             raise TypeError(f"unknown arguments {sorted(lambdas)}")
-        cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps = 0.9, 0.999, 1e-8
+        cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps = 0.9, 0.999, 1e-8      # torch.optim.Adam defaults
+        cfg.constrained = int(constrained)
         self.cfg = cfg
         self._h = ctypes.c_void_p()
         _lib.check(self._lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(self._h)))
 
     def close(self):
+        """Free the device state now (M, m, v, operands: ~20 bytes per mapping element) instead of at garbage collection."""
         if self._h:
             self._lib.tgb200_destroy(self._h)
             self._h = None
@@ -55,12 +96,9 @@ class Engine:
     def set_ct_encode(self, E, stream=None):
         _lib.check(self._lib.tgb200_set_ct_encode(self._h, _lib.ptr(E), self._s(stream)))
 
-    def set_graph(self, which, csr, stream=None):
-        csr = csr.tocsr()
-        csr.sort_indices()
-        ip = np.ascontiguousarray(csr.indptr, dtype=np.int32)
-        ix = np.ascontiguousarray(csr.indices, dtype=np.int32)
-        vv = np.ascontiguousarray(csr.data, dtype=np.float32)
+    def set_graph(self, which, mat, stream=None):
+        """`mat`: the n_voxels x n_voxels operator, dense, torch or scipy sparse."""
+        ip, ix, vv = _csr(mat, self.cfg.n_voxels)
         _lib.check(self._lib.tgb200_set_graph(self._h, which, _lib.ptr(ip), _lib.ptr(ix), _lib.ptr(vv), len(vv),
                                               self._s(stream)))
 
@@ -73,11 +111,26 @@ class Engine:
     def init_mapping_legacy(self, state, skip=0, first_row=0, end_normal=None, stream=None):
         """The reference draw np.random.normal(0, 1, ...) from the numpy generator state `state` (get_state() tuple):
         rows [first_row, first_row + n_cells) of a draw that starts `skip` normals into the stream.  Returns (the state
-        after end_normal normals, default the end of these rows; values recomputed on the host)."""
-        from . import legacy_rng
+        after end_normal normals, default the end of these rows, as np.random.set_state takes it; values recomputed on
+        the host)."""
         if end_normal is None:
             end_normal = skip + (first_row + self.cfg.n_cells) * self.cfg.n_voxels
-        return legacy_rng.init_mapping(self._lib, self._h, state, skip, first_row, end_normal, self._s(stream))
+        start, end, n_fixed = _lib.MtState.from_numpy(state), _lib.MtState(), ctypes.c_int64()
+        _lib.check(self._lib.tgb200_init_mapping_legacy(self._h, ctypes.byref(start), int(skip), int(first_row),
+                                                        int(end_normal), ctypes.byref(end), ctypes.byref(n_fixed),
+                                                        self._s(stream)))
+        return end.to_numpy(), n_fixed.value
+
+    def set_filter(self, F0, stream=None):
+        """Constrained mode: initial filter logits (n_cells)."""
+        _lib.check(self._lib.tgb200_set_filter(self._h, _lib.ptr(F0), self._s(stream)))
+
+    def get_filter(self, logits=None, sigmoid=None, stream=None):
+        """Constrained mode: copy the filter logits F and/or sigmoid(F) (n_cells each; None skips) out of the handle."""
+        _lib.check(self._lib.tgb200_get_filter(self._h, _lib.ptr(logits), _lib.ptr(sigmoid), self._s(stream)))
+
+    def reset_adam(self, stream=None):
+        _lib.check(self._lib.tgb200_reset_adam(self._h, self._s(stream)))
 
     def run(self, n_steps, lr=0.1, stream=None):
         _lib.check(self._lib.tgb200_run(self._h, n_steps, lr, self._s(stream)))
@@ -88,20 +141,12 @@ class Engine:
     def step_end(self, lr=0.1, stream=None):
         _lib.check(self._lib.tgb200_step_end(self._h, lr, self._s(stream)))
 
-    def comm_init(self, rank, world, broadcast):
-        """Own NCCL communicator for the cell-sharded tgb200_run: rank 0 creates the 128-byte id (tgb200_comm_unique_id),
-        `broadcast(uint8 ndarray) -> ndarray` carries it to every rank by any means, every rank joins."""
-        uid = np.zeros(128, dtype=np.uint8)
-        if rank == 0:
-            _lib.check(self._lib.tgb200_comm_unique_id(_lib.ptr(uid), uid.nbytes))
-        uid = np.ascontiguousarray(broadcast(uid), dtype=np.uint8)
-        _lib.check(self._lib.tgb200_comm_init_rank(self._h, _lib.ptr(uid), rank, world))
-
     def set_comm(self, comm, rank, world):
         """Lend the handle an existing ncclComm_t (tangram_b200.sharded.nccl_comm_for_group); the caller keeps ownership."""
         _lib.check(self._lib.tgb200_set_comm(self._h, comm, rank, world))
 
     def exchange_tensor(self):
+        """torch view of the device exchange buffer (for torch.distributed.all_reduce)."""
         import torch
         p, n = ctypes.c_void_p(), ctypes.c_int64()
         _lib.check(self._lib.tgb200_exchange_buffer(self._h, ctypes.byref(p), ctypes.byref(n)))
@@ -111,12 +156,24 @@ class Engine:
                                         "version": 3, "strides": None}
         return torch.as_tensor(_Wrap(), device=f"cuda:{self.cfg.device}")
 
-    def history(self):
+    def history_len(self):
         n = ctypes.c_int64()
         _lib.check(self._lib.tgb200_history_len(self._h, ctypes.byref(n)))
-        out = np.empty((n.value, _lib.HIST_COLS), dtype=np.float32)
-        if n.value:
-            _lib.check(self._lib.tgb200_get_history(self._h, 0, n.value, _lib.ptr(out), None))
+        return n.value
+
+    def history(self, first=0, count=None):
+        """Rows [first, first + count) of the loss history (default: to the end), (count, HIST_COLS) float32."""
+        if count is None:
+            count = self.history_len() - first
+        out = np.empty((count, _lib.HIST_COLS), dtype=np.float32)
+        if count:
+            _lib.check(self._lib.tgb200_get_history(self._h, first, count, _lib.ptr(out), None))
+        return out
+
+    def validation_terms(self, stream=None):
+        """(val_total_loss, val_gene_sim, val_sp_sparsity_weighted_sim, val_entropy) of the current mapping, float32."""
+        out = np.zeros(4, dtype=np.float32)
+        _lib.check(self._lib.tgb200_validation_terms(self._h, _lib.ptr(out), self._s(stream)))
         return out
 
     def get_mapping(self, out, stream=None):
@@ -134,6 +191,9 @@ class Engine:
         step = ctypes.c_int64()
         _lib.check(self._lib.tgb200_get_state(self._h, _lib.ptr(M), _lib.ptr(m), _lib.ptr(v), ctypes.byref(step), self._s(stream)))
         return step.value
+
+    def set_state(self, M, m, v, step, stream=None):
+        _lib.check(self._lib.tgb200_set_state(self._h, _lib.ptr(M), _lib.ptr(m), _lib.ptr(v), int(step), self._s(stream)))
 
     def debug(self, name):
         """Internal device buffer by name (tgb200_debug_buffer) as a host array."""

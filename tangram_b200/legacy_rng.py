@@ -51,20 +51,10 @@ def device_draw_supported(n=4000):
     return _PROBE
 
 
-def init_mapping(lib, handle, state, skip, first_row, end_normal, stream=None):
-    """tgb200_init_mapping_legacy from an np.random.get_state() tuple -> (state after end_normal normals as the
-    tuple np.random.set_state takes, number of values recomputed on the host)."""
-    start = _lib.MtState.from_numpy(state)
-    end = _lib.MtState()
-    n_fixed = ctypes.c_int64()
-    _lib.check(lib.tgb200_init_mapping_legacy(handle, ctypes.byref(start), int(skip), int(first_row), int(end_normal),
-                                              ctypes.byref(end), ctypes.byref(n_fixed), stream))
-    return end.to_numpy(), n_fixed.value
-
-
-def draw_global(lib, handle, skip, first_row, end_normal):
-    """The draw from numpy's global generator, which is left where the host draw would leave it."""
-    end, n_fixed = init_mapping(lib, handle, np.random.get_state(), skip, first_row, end_normal)
+def draw_global(engine, skip, first_row, end_normal):
+    """The draw from numpy's global generator into `engine` (Engine.init_mapping_legacy), which leaves the generator
+    where the host draw would leave it."""
+    end, n_fixed = engine.init_mapping_legacy(np.random.get_state(), skip, first_row, end_normal)
     np.random.set_state(end)
     return n_fixed
 

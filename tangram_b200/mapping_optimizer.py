@@ -1,8 +1,8 @@
 """
 Drop-in replacement for the reference optimizer class `Mapper`
 (Tangram's tangram/mapping_optimizer.py:14-408), running on the sm_90a (H100) C-ABI
-library (include/tangram_b200.h).  Same constructor keywords, same `train()` signature,
-same return types and history conventions.  There is no CPU path: `device` must be a
+library (include/tangram_b200.h) through `tangram_b200.engine.Engine`.  Same constructor keywords,
+same `train()` signature, same return types and history conventions.  There is no CPU path: `device` must be a
 CUDA device with compute capability 9.0.
 
 Additions (keyword-only, all optional):
@@ -18,12 +18,12 @@ Additions (keyword-only, all optional):
   train(..., resume=True)  continue with the Adam state of the previous train() call (the reference -- and the default
               here -- builds a fresh optimizer in every train() call, mapping_optimizer.py:373)
   train(..., out=tensor)   write softmax(M) into a CUDA tensor instead of returning a host array
+  validation_terms(), project(X, out=None), state() / load_state(...)
 """
-import ctypes
-
 import numpy as np
 
 from . import _lib, legacy_rng
+from .engine import Engine, _device_index
 from .sharded import shard_rows, sharded_steps
 
 _HIST_KEYS = ["total_loss", "main_loss", "vg_reg", "kl_reg", "entropy_reg"]
@@ -34,32 +34,6 @@ _PRINT_TERMS = [
     (5, "L1 reg"), (6, "L2 reg"), (7, "Spatial weighted score"), (8, "Cell type islands penalty"),
     (9, "Getis-Ord score"),
 ]
-
-
-def _device_index(device):
-    """'cuda', 'cuda:1', torch.device -> ordinal.  'cpu' is refused: no CPU fallback."""
-    s = str(device)
-    if s.startswith("cuda"):
-        return int(s.split(":")[1]) if ":" in s else 0
-    raise ValueError(
-        f"tangram_b200.Mapper runs on H100 GPUs only (device={device!r}); "
-        "use the reference implementation for device='cpu'")
-
-
-def _to_csr(mat, n):
-    """dense ndarray (what the reference passes, mapping_utils.py:319-329) or scipy sparse -> CSR triplet."""
-    import scipy.sparse as sp
-    if mat is None:
-        return None
-    if hasattr(mat, "detach"):
-        mat = mat.detach().cpu().numpy()
-    csr = mat.tocsr() if sp.issparse(mat) else sp.csr_matrix(np.asarray(mat))
-    if csr.shape != (n, n):
-        raise ValueError(f"spatial operator has shape {csr.shape}, expected {(n, n)}")
-    csr.sort_indices()
-    return (np.ascontiguousarray(csr.indptr, dtype=np.int32),
-            np.ascontiguousarray(csr.indices, dtype=np.int32),
-            np.ascontiguousarray(csr.data, dtype=np.float32))
 
 
 class _ResultBuffer:
@@ -113,13 +87,82 @@ def legacy_normal_rows(random_state, n_rows, n_cols, r0, r1, block_rows=4096):
     return out
 
 
-def format_terms(row):
-    """The reference's print line (mapping_optimizer.py:300-307) from one history row."""
-    msg = ["{}: {:.3f}".format(name, row[c]) for c, name in _PRINT_TERMS if not np.isnan(row[c])]
+def format_terms(terms):
+    """The reference's print line (mapping_optimizer.py:300-307, :555-562) from (name, value) pairs; NaN terms are left
+    out."""
+    msg = ["{}: {:.3f}".format(name, value) for name, value in terms if not np.isnan(value)]
     return str(msg).replace("[", "").replace("]", "").replace("'", "")
 
 
-class Mapper:
+class _EngineMapper:
+    """What Mapper and MapperConstrained share: an Engine (`_engine`) of n_cells x n_voxels, the epoch-chunk schedule,
+    the history fetch and the result buffer."""
+
+    def release(self):
+        """Free the device state now (M, m, v, operands: ~20 bytes per mapping element) instead of at garbage collection."""
+        self._engine.close()
+
+    def kernel_launches(self):
+        return self._engine.kernel_launches()
+
+    def project(self, X, out=None):
+        """softmax(M)^T @ X on the device (project_genes' GEMM, tangram/utils.py:368) -> (n_voxels, n_cols) float32
+        ndarray; or, with `out` (a contiguous float32 CUDA tensor of that shape on this mapper's device), written there."""
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        if X.shape[0] != self.n_cells:
+            raise ValueError("X must have one row per cell")
+        if out is None:
+            out = np.empty((self.n_voxels, X.shape[1]), dtype=np.float32)
+        else:
+            self._check_out(out, (self.n_voxels, X.shape[1]))
+        return self._engine.project(X, out)
+
+    def _check_out(self, out, shape):
+        import torch
+        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.device.index == self._cfg.device):
+            raise TypeError(f"out must be a CUDA tensor on cuda:{self._cfg.device}")
+        if out.dtype != torch.float32 or tuple(out.shape) != shape or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous float32 tensor of shape {shape}")
+
+    def _run(self, n_steps, lr):
+        self._engine.run(n_steps, lr)
+
+    def _fit(self, num_epochs, lr, print_each, resume, out=None, val_each=None, val_history=None):
+        """num_epochs updates (a fresh Adam unless `resume`), run in chunks that end where the reference prints or
+        validates (every `val_each` epochs, into the lists of `val_history`).  Sets history_matrix to this call's rows
+        and returns softmax(M), in `out` or a host array."""
+        if not resume:
+            self._engine.reset_adam()
+        first = self._engine.history_len()
+        if out is not None:
+            self._check_out(out, (self.n_cells, self.n_voxels))
+            result = None
+        else:
+            result = _ResultBuffer(_lib.load(), (self.n_cells, self.n_voxels), self._cfg.device)
+        try:
+            t = 0
+            while t < num_epochs:
+                if val_each is not None:
+                    chunk = 1
+                elif print_each:
+                    chunk = min(num_epochs - t, print_each - (t % print_each))
+                else:
+                    chunk = num_epochs - t
+                self._run(chunk, lr)
+                if print_each and t % print_each == 0:
+                    print(format_terms(self._print_terms(self._engine.history(first + t, 1)[0])))
+                if val_each is not None and t % val_each == 0:
+                    for k, x in self.validation_terms().items():
+                        val_history[k].append(x)
+                t += chunk
+            self.history_matrix = self._engine.history(first, num_epochs)
+            return self._engine.get_mapping(out if out is not None else result.ready())
+        finally:
+            if result is not None:
+                result.release()
+
+
+class Mapper(_EngineMapper):
     def __init__(
         self,
         S,
@@ -163,8 +206,6 @@ class Mapper:
         self.device = device
         self.random_state = random_state
         self.precision = precision
-        self._lib = _lib.load()
-        self._h = None
         self._pg = process_group
 
         S = np.asarray(S, dtype=np.float32)
@@ -205,7 +246,7 @@ class Mapper:
             r, w = dist.get_rank(process_group), dist.get_world_size(process_group)
             self._rows = shard_rows(n_cells_global, r, w)
         r0, r1 = self._rows
-        sharded = (r1 - r0) != n_cells_global
+        self._sharded = (r1 - r0) != n_cells_global
         # initial mapping: legacy numpy RNG, float64 draw, f32 cast; seeded only if truthy (:147-157).  A rank of a
         # sharded run draws the same stream and keeps only its rows (pre-sharded callers pass M0 or get a per-rank draw).
         # The draw runs on the device (legacy_rng) unless this numpy's arithmetic differs from the device formula.
@@ -215,34 +256,21 @@ class Mapper:
         elif M0 is not None:
             M0 = M0[r0:r1]
 
-        cfg = _lib.Config()
-        cfg.struct_size = ctypes.sizeof(_lib.Config)
-        cfg.device = _device_index(device)
-        cfg.n_cells, cfg.n_voxels, cfg.n_genes, cfg.n_types = r1 - r0, n_voxels, n_genes, n_types
-        cfg.n_cells_global = n_cells_global
-        cfg.precision = _lib.PREC[precision]
-        cfg.density_mode = density_mode
-        cfg.lambda_g1, cfg.lambda_d, cfg.lambda_g2 = lambda_g1, lambda_d, lambda_g2
-        cfg.lambda_r, cfg.lambda_l1, cfg.lambda_l2 = lambda_r, lambda_l1, lambda_l2
-        cfg.lambda_neighborhood_g1 = lambda_neighborhood_g1
-        cfg.lambda_ct_islands = lambda_ct_islands
-        cfg.lambda_getis_ord = lambda_getis_ord
-        cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps = 0.9, 0.999, 1e-8   # torch.optim.Adam defaults (:373)
-        h = ctypes.c_void_p()
-        _lib.check(self._lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(h)))
-        self._h = h
-        self._cfg = cfg
-        self._sharded = sharded
+        e = self._engine = Engine(
+            r1 - r0, n_voxels, n_genes, n_types=n_types, n_cells_global=n_cells_global, device=_device_index(device),
+            precision=precision, density_mode=density_mode, lambda_g1=lambda_g1, lambda_d=lambda_d,
+            lambda_g2=lambda_g2, lambda_r=lambda_r, lambda_l1=lambda_l1, lambda_l2=lambda_l2,
+            lambda_neighborhood_g1=lambda_neighborhood_g1, lambda_ct_islands=lambda_ct_islands,
+            lambda_getis_ord=lambda_getis_ord)
+        self._cfg = e.cfg
         self.n_cells, self.n_voxels, self.n_genes = r1 - r0, n_voxels, n_genes
 
-        L = self._lib
-        _lib.check(L.tgb200_set_expression(h, _lib.ptr(np.ascontiguousarray(S[r0:r1])), _lib.ptr(G), None))
+        e.set_expression(np.ascontiguousarray(S[r0:r1]), G)
         if self.target_density_enabled:
-            dd = np.ascontiguousarray(np.asarray(d, dtype=np.float32))
             ds = None
             if self.source_density_enabled:
                 ds = np.ascontiguousarray(np.asarray(d_source, dtype=np.float32)[r0:r1])
-            _lib.check(L.tgb200_set_density(h, _lib.ptr(dd), _lib.ptr(ds), None))
+            e.set_density(np.ascontiguousarray(np.asarray(d, dtype=np.float32)), ds)
         graphs = []
         if lambda_neighborhood_g1 > 0:
             graphs.append((_lib.GRAPH_VOXEL_WEIGHTS, voxel_weights, "voxel_weights"))
@@ -253,23 +281,20 @@ class Mapper:
         for which, mat, name in graphs:
             if mat is None:
                 raise ValueError(f"{name} is required by the enabled lambda")
-            indptr, indices, vals = _to_csr(mat, n_voxels)
-            _lib.check(L.tgb200_set_graph(h, which, _lib.ptr(indptr), _lib.ptr(indices), _lib.ptr(vals),
-                                          len(vals), None))
+            e.set_graph(which, mat)
         if lambda_ct_islands > 0:
             if ct_encode is None:
                 raise ValueError("ct_encode is required when lambda_ct_islands > 0")
-            _lib.check(L.tgb200_set_ct_encode(h, _lib.ptr(np.ascontiguousarray(ct_encode[r0:r1])), None))
+            e.set_ct_encode(np.ascontiguousarray(ct_encode[r0:r1]))
         if device_draw:
             if self.random_state:
                 np.random.seed(seed=self.random_state)
-            legacy_rng.draw_global(L, h, 0, r0, r1 * n_voxels)      # the generator ends after row r1, as on the host
+            legacy_rng.draw_global(e, 0, r0, r1 * n_voxels)      # the generator ends after row r1, as on the host
         else:
-            M0 = np.ascontiguousarray(M0, dtype=np.float32)
-            _lib.check(L.tgb200_set_mapping(h, _lib.ptr(M0), None))
+            e.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
             del M0
         self._own_comm = False
-        if sharded and process_group is not None:
+        if self._sharded and process_group is not None:
             self._init_comm(process_group)
 
     def _init_comm(self, pg):
@@ -280,63 +305,28 @@ class Mapper:
         got = nccl_comm_for_group(pg, self._cfg.device)
         if got is None:
             return
-        comm, rank, world = got
-        _lib.check(self._lib.tgb200_set_comm(self._h, comm, rank, world))
+        self._engine.set_comm(*got)
         self._own_comm = True
 
     # ------------------------------------------------------------------------------
-    def release(self):
-        """Free the device state now (M, m, v, operands: ~20 bytes per mapping element) instead of at garbage collection."""
-        if self._h is not None:
-            self._lib.tgb200_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
-
-    def _history_rows(self, first, count):
-        out = np.empty((count, _lib.HIST_COLS), dtype=np.float32)
-        if count:
-            _lib.check(self._lib.tgb200_get_history(self._h, first, count, _lib.ptr(out), None))
-        return out
-
-    def _exchange_tensor(self):
-        """torch view of the device exchange buffer (for torch.distributed.all_reduce)."""
-        import torch
-        p = ctypes.c_void_p()
-        n = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_exchange_buffer(self._h, ctypes.byref(p), ctypes.byref(n)))
-
-        class _Wrap:
-            __cuda_array_interface__ = {
-                "shape": (n.value,), "typestr": "<f4", "data": (p.value, False), "version": 3, "strides": None}
-        return torch.as_tensor(_Wrap(), device=f"cuda:{self._cfg.device}")
-
     def _run(self, n_steps, lr):
-        if n_steps <= 0:
-            return
         if not self._sharded or self._own_comm:
-            _lib.check(self._lib.tgb200_run(self._h, n_steps, lr, None))    # sharded: the NCCL exchange is inside
+            self._engine.run(n_steps, lr)    # sharded: the NCCL exchange is inside
             return
+        from types import SimpleNamespace
+
         import torch
         import torch.distributed as dist
-        mapper, stream = self, ctypes.c_void_p(torch.cuda.current_stream(self._cfg.device).cuda_stream)
-
-        class _Eng:   # the engine protocol of tangram_b200.sharded over the C-ABI handle
-            def exchange_tensor(self):
-                return mapper._exchange_tensor()
-
-            def step_begin(self):
-                _lib.check(mapper._lib.tgb200_step_begin(mapper._h, stream))
-
-            def step_end(self, lr_):
-                _lib.check(mapper._lib.tgb200_step_end(mapper._h, lr_, stream))
-
-        sharded_steps(_Eng(), n_steps, lr,
+        e, stream = self._engine, torch.cuda.current_stream(self._cfg.device).cuda_stream
+        # the engine protocol of tangram_b200.sharded, issued on torch's current stream
+        on_stream = SimpleNamespace(exchange_tensor=e.exchange_tensor, step_begin=lambda: e.step_begin(stream),
+                                    step_end=lambda lr_: e.step_end(lr_, stream))
+        sharded_steps(on_stream, n_steps, lr,
                       lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self._pg))   # the one exchange per step
+
+    @staticmethod
+    def _print_terms(row):
+        return [(name, row[c]) for c, name in _PRINT_TERMS]
 
     def train(self, num_epochs, learning_rate=0.1, print_each=100, val_each=None, *, resume=False, out=None):
         """mapping_optimizer.py:358-408.  Returns (softmax(M) as (N, V) f32 ndarray, history).
@@ -347,99 +337,44 @@ class Mapper:
         import logging
         if print_each:
             logging.info(f"Printing scores every {print_each} epochs.")
-        if not resume:
-            _lib.check(self._lib.tgb200_reset_adam(self._h, None))
-        training_history = {key: [] for key in _HIST_KEYS + _VAL_KEYS}
-        first = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_history_len(self._h, ctypes.byref(first)))
-        first = first.value
-        lr = float(learning_rate)
-        if out is not None:
-            self._check_out(out)
-            return self._train_loop(num_epochs, lr, print_each, val_each, first, training_history, None, out)
-        result = _ResultBuffer(self._lib, (self.n_cells, self.n_voxels), self._cfg.device)
-        try:
-            return self._train_loop(num_epochs, lr, print_each, val_each, first, training_history, result)
-        finally:
-            result.release()
-
-    def _check_out(self, out):
-        import torch
-        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.device.index == self._cfg.device):
-            raise TypeError(f"out must be a CUDA tensor on cuda:{self._cfg.device}")
-        if out.dtype != torch.float32 or tuple(out.shape) != (self.n_cells, self.n_voxels) or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous float32 tensor of shape {(self.n_cells, self.n_voxels)}")
-
-    def _train_loop(self, num_epochs, lr, print_each, val_each, first, training_history, result, out=None):
-        t = 0
-        while t < num_epochs:
-            if val_each is not None:
-                chunk = 1
-            elif print_each:
-                chunk = min(num_epochs - t, print_each - (t % print_each))
-            else:
-                chunk = num_epochs - t
-            self._run(chunk, lr)
-            if print_each and t % print_each == 0:
-                print(format_terms(self._history_rows(first + t, 1)[0]))
-            if val_each is not None and t % val_each == 0:
-                vals = np.zeros(4, dtype=np.float32)
-                _lib.check(self._lib.tgb200_validation_terms(self._h, _lib.ptr(vals), None))
-                for k, x in zip(_VAL_KEYS, vals):
-                    training_history[k].append(float(x))
-            t += chunk
-
-        rows = self._history_rows(first, num_epochs)
-        training_history["total_loss"] = [np.array(x, dtype=np.float32) for x in rows[:, 0]]   # 0-d ndarrays (:390)
+        val_history = {key: [] for key in _VAL_KEYS}
+        output = self._fit(num_epochs, float(learning_rate), print_each, resume, out, val_each, val_history)
+        rows = self.history_matrix
+        training_history = {"total_loss": [np.array(x, dtype=np.float32) for x in rows[:, 0]]}   # 0-d ndarrays (:390)
         for c, key in enumerate(_HIST_KEYS[1:], start=1):
             training_history[key] = [float(x) for x in rows[:, c]]
-        self.history_matrix = rows
-        output = result.ready() if out is None else out
-        _lib.check(self._lib.tgb200_get_mapping(self._h, _lib.ptr(output), None))
+        training_history.update(val_history)
         return output, training_history
 
     # --- extras beyond the reference surface -------------------------------------------
+    def validation_terms(self):
+        """The reference's validation scores (_val_loss_fn, mapping_optimizer.py:311-356) of the current mapping:
+        {val_total_loss, val_gene_sim, val_sp_sparsity_weighted_sim, val_entropy} as floats."""
+        return {k: float(x) for k, x in zip(_VAL_KEYS, self._engine.validation_terms())}
+
     def state(self):
         """(M, m, v, step): checkpoint of the optimizer (the reference stubs resume, :151-153)."""
         M = np.empty((self.n_cells, self.n_voxels), dtype=np.float32)
         m = np.empty_like(M)
         v = np.empty_like(M)
-        step = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_get_state(self._h, _lib.ptr(M), _lib.ptr(m), _lib.ptr(v), ctypes.byref(step), None))
-        return M, m, v, step.value
+        return M, m, v, self._engine.get_state(M, m, v)
 
     def load_state(self, M, m, v, step):
         M, m, v = (np.ascontiguousarray(x, dtype=np.float32) for x in (M, m, v))
-        _lib.check(self._lib.tgb200_set_state(self._h, _lib.ptr(M), _lib.ptr(m), _lib.ptr(v), int(step), None))
-
-    def project(self, X):
-        """softmax(M)^T @ X on the device (project_genes' GEMM, tangram/utils.py:368)."""
-        X = np.ascontiguousarray(X, dtype=np.float32)
-        if X.shape[0] != self.n_cells:
-            raise ValueError("X must have one row per cell")
-        out = np.empty((self.n_voxels, X.shape[1]), dtype=np.float32)
-        _lib.check(self._lib.tgb200_project(self._h, _lib.ptr(X), X.shape[1], _lib.ptr(out), None))
-        return out
+        self._engine.set_state(M, m, v, step)
 
     def _debug(self, name):
         """Diagnostics: internal device buffer by name (see tgb200_debug_buffer)."""
-        n = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_debug_buffer(self._h, name.encode(), None, 0, ctypes.byref(n)))
-        out = np.empty(max(n.value, 4), dtype=np.float32)
-        _lib.check(self._lib.tgb200_debug_buffer(self._h, name.encode(), _lib.ptr(out), out.size, ctypes.byref(n)))
-        return out[:n.value]
-
-    def kernel_launches(self):
-        n = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_kernel_launches(self._h, ctypes.byref(n)))
-        return n.value
+        return self._engine.debug(name)
 
 
-class MapperConstrained:
+class MapperConstrained(_EngineMapper):
     """Drop-in for the reference `MapperConstrained` (mapping_optimizer.py:411-639): same constructor keywords,
     `train()` returns `(mapping, F_out, training_history)` with the reference's history conventions (all values are
     strings, :630).  The per-cell filter rides the same kernels: S_f = sigmoid(F) o S is the operand of all three
     contractions, dL/df_i is the row-dot the backward pass needs anyway, and F gets its own small Adam kernel."""
+    _KEYS = ["total_loss", "main_loss", "vg_reg", "kl_reg", "entropy_reg", "count_reg", "lambda_f_reg"]
+    _PRINT_NAMES = ["Score", "VG reg", "KL reg", "Entropy reg", "Count reg", "Lambda f reg"]          # :555-562
 
     def __init__(self, S, G, d, lambda_d=1, lambda_g1=1, lambda_g2=1, lambda_r=0, lambda_count=1, lambda_f_reg=1,
                  target_count=None, device="cuda:0", adata_map=None, random_state=None, *, precision="bf16x3",
@@ -448,8 +383,6 @@ class MapperConstrained:
             raise NotImplementedError      # the reference raises here too (:476-477)
         if precision not in _lib.PREC:
             raise ValueError(f"precision must be one of {list(_lib.PREC)}")
-        self._lib = _lib.load()
-        self._h = None
         self.random_state = random_state
         S = np.ascontiguousarray(np.asarray(S, dtype=np.float32))
         G = np.ascontiguousarray(np.asarray(G, dtype=np.float32))
@@ -464,112 +397,54 @@ class MapperConstrained:
             np.random.normal(0, 1, (n_cells, n_voxels))
             M0 = np.random.normal(0, 1, (n_cells, n_voxels))
             F0 = np.random.normal(0, 1, n_cells)
-        cfg = _lib.Config()
-        cfg.struct_size = ctypes.sizeof(_lib.Config)
-        cfg.device = _device_index(device)
-        cfg.n_cells, cfg.n_voxels, cfg.n_genes, cfg.n_types = n_cells, n_voxels, n_genes, 0
-        cfg.n_cells_global = n_cells
-        cfg.precision = _lib.PREC[precision]
-        cfg.density_mode = _lib.DENSITY_CELLS if self.target_density_enabled else _lib.DENSITY_NONE
-        cfg.lambda_g1, cfg.lambda_d, cfg.lambda_g2, cfg.lambda_r = lambda_g1, lambda_d, lambda_g2, lambda_r
-        cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps = 0.9, 0.999, 1e-8
-        cfg.constrained = 1
-        cfg.lambda_count, cfg.lambda_f_reg = lambda_count, lambda_f_reg
-        cfg.target_count = float(n_voxels if target_count is None else target_count)      # :480-483
-        self._lam = dict(g1=lambda_g1, d=lambda_d, g2=lambda_g2, r=lambda_r, c=lambda_count, f=lambda_f_reg)
-        h = ctypes.c_void_p()
-        _lib.check(self._lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(h)))
-        self._h, self._cfg = h, cfg
+        e = self._engine = Engine(
+            n_cells, n_voxels, n_genes, device=_device_index(device), precision=precision,
+            density_mode=_lib.DENSITY_CELLS if self.target_density_enabled else _lib.DENSITY_NONE,
+            lambda_g1=lambda_g1, lambda_d=lambda_d, lambda_g2=lambda_g2, lambda_r=lambda_r, constrained=True,
+            lambda_count=lambda_count, lambda_f_reg=lambda_f_reg,
+            target_count=float(n_voxels if target_count is None else target_count))      # :480-483
+        self._cfg = e.cfg
         self.n_cells, self.n_voxels, self.n_genes = n_cells, n_voxels, n_genes
-        L = self._lib
-        _lib.check(L.tgb200_set_expression(h, _lib.ptr(S), _lib.ptr(G), None))
+        e.set_expression(S, G)
         if self.target_density_enabled:
-            dd = np.ascontiguousarray(np.asarray(d, dtype=np.float32))
-            _lib.check(L.tgb200_set_density(h, _lib.ptr(dd), None, None))
+            e.set_density(np.ascontiguousarray(np.asarray(d, dtype=np.float32)))
         if device_draw:
             # the same three draws: the first N x V normals are skipped, the second N x V land in M, F follows on the host
             if self.random_state:
                 np.random.seed(seed=self.random_state)
-            legacy_rng.draw_global(L, h, n_cells * n_voxels, 0, 2 * n_cells * n_voxels)
+            legacy_rng.draw_global(e, n_cells * n_voxels, 0, 2 * n_cells * n_voxels)
             F0 = np.random.normal(0, 1, n_cells)
         else:
-            _lib.check(L.tgb200_set_mapping(h, _lib.ptr(np.ascontiguousarray(M0, dtype=np.float32)), None))
-        _lib.check(L.tgb200_set_filter(h, _lib.ptr(np.ascontiguousarray(F0, dtype=np.float32)), None))
+            e.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
+        e.set_filter(np.ascontiguousarray(F0, dtype=np.float32))
 
-    def __del__(self):
-        try:
-            if self._h is not None:
-                self._lib.tgb200_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
-
-    @staticmethod
-    def _print_line(vals):
-        names = ["Score", "VG reg", "KL reg", "Entropy reg", "Count reg", "Lambda f reg"]          # :555-562
-        msg = ["{}: {:.3f}".format(n, v) for n, v in zip(names, vals) if not np.isnan(v)]
-        return str(msg).replace("[", "").replace("]", "").replace("'", "")
+    def _print_terms(self, row):
+        return zip(self._PRINT_NAMES, self._values_from_row(row))
 
     def train(self, num_epochs, learning_rate=0.1, print_each=100, *, resume=False):
         """mapping_optimizer.py:589-639.  A fresh Adam over [M, F] per call (:607) unless resume=True."""
-        keys = ["total_loss", "main_loss", "vg_reg", "kl_reg", "entropy_reg", "count_reg", "lambda_f_reg"]
-        if not resume:
-            _lib.check(self._lib.tgb200_reset_adam(self._h, None))
-        first = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_history_len(self._h, ctypes.byref(first)))
-        first = first.value
-        result = _ResultBuffer(self._lib, (self.n_cells, self.n_voxels), self._cfg.device)
-        try:
-            return self._train_loop(num_epochs, learning_rate, print_each, first, keys, result)
-        finally:
-            result.release()
-
-    def _train_loop(self, num_epochs, learning_rate, print_each, first, keys, result):
-        t = 0
-        while t < num_epochs:
-            chunk = min(num_epochs - t, print_each - (t % print_each)) if print_each else num_epochs - t
-            _lib.check(self._lib.tgb200_run(self._h, chunk, float(learning_rate), None))
-            if print_each and t % print_each == 0:
-                print(self._print_line(self._row_values(first + t)))
-            t += chunk
-        rows = np.empty((num_epochs, _lib.HIST_COLS), dtype=np.float32)
-        if num_epochs:
-            _lib.check(self._lib.tgb200_get_history(self._h, first, num_epochs, _lib.ptr(rows), None))
-        self.history_matrix = rows
-        hist = {k: [] for k in keys}
-        for r in rows:
-            vals = self._values_from_row(r)
+        output = self._fit(num_epochs, float(learning_rate), print_each, resume)
+        hist = {k: [] for k in self._KEYS}
+        for r in self.history_matrix:
             hist["total_loss"].append("tensor({:.4f}, grad_fn=<AddBackward0>)".format(float(r[0])))     # str(tensor), :630
-            for k, v in zip(keys[1:], vals):
+            for k, v in zip(self._KEYS[1:], self._values_from_row(r)):
                 hist[k].append(str(v))
-        output = result.ready()
-        _lib.check(self._lib.tgb200_get_mapping(self._h, _lib.ptr(output), None))
         F_out = np.empty(self.n_cells, dtype=np.float32)
-        _lib.check(self._lib.tgb200_get_filter(self._h, None, _lib.ptr(F_out), None))
+        self._engine.get_filter(sigmoid=F_out)
         return output, F_out, hist
 
-    def _values_from_row(self, r):
+    @staticmethod
+    def _values_from_row(r):
         """(main_loss, vg_reg, kl_reg, entropy_reg, count_reg, lambda_f_reg) with the reference's sign/NaN conventions."""
         ent = -float(r[4])            # the reference logs +sum(P log P) here (:526, :540)
         return (float(r[1]), float(r[2]), float(r[3]), ent, float(r[10]), float(r[11]))
 
-    def _row_values(self, idx):
-        row = np.empty((1, _lib.HIST_COLS), dtype=np.float32)
-        _lib.check(self._lib.tgb200_get_history(self._h, idx, 1, _lib.ptr(row), None))
-        return self._values_from_row(row[0])
-
     def filter_logits(self):
         F = np.empty(self.n_cells, dtype=np.float32)
-        _lib.check(self._lib.tgb200_get_filter(self._h, _lib.ptr(F), None, None))
+        self._engine.get_filter(logits=F)
         return F
 
     def state(self):
         M = np.empty((self.n_cells, self.n_voxels), dtype=np.float32)
-        step = ctypes.c_int64()
-        _lib.check(self._lib.tgb200_get_state(self._h, _lib.ptr(M), None, None, ctypes.byref(step), None))
-        return M, self.filter_logits(), step.value
-
-
-MapperConstrained.release = Mapper.release
-MapperConstrained.project = Mapper.project
-MapperConstrained.kernel_launches = Mapper.kernel_launches
+        step = self._engine.get_state(M)
+        return M, self.filter_logits(), step

@@ -20,24 +20,13 @@ import ctypes
 import numpy as np
 
 from . import _lib
-from .mapping_optimizer import Mapper, _VAL_KEYS
+from .engine import _require_device
+from .mapping_optimizer import Mapper
 
 _CONFIG_LAMBDAS = ["lambda_d", "lambda_g1", "lambda_g2", "lambda_neighborhood_g1", "lambda_r", "lambda_l1",
                    "lambda_l2", "lambda_ct_islands", "lambda_getis_ord"]     # :97
-_GENE_SIM = _VAL_KEYS.index("val_gene_sim")
 # device bytes per mapping element one Mapper handle holds at most (M, m, v, operands, a projection's P planes)
 _HANDLE_BYTES_PER_ELEMENT = 28
-
-
-def _require_device(device):
-    """-> ordinal of a visible CUDA device, or TangramB200Error: there is no CPU fallback."""
-    import torch
-    s = str(device)
-    if not s.startswith("cuda"):
-        raise _lib.TangramB200Error(f"tangram_b200 runs on H100 GPUs only (device={device!r}); no CPU fallback")
-    if not torch.cuda.is_available():
-        raise _lib.TangramB200Error("no CUDA device visible: tangram_b200 has no CPU fallback")
-    return int(s.split(":")[1]) if ":" in s else torch.cuda.current_device()
 
 
 def _runs_on_device(cube, device):
@@ -107,12 +96,6 @@ def consensus_entropy(pred_probs_cube, *, device=None):
     return agreement(pred_probs_cube, pearson=False, consensus=True, device=device)[2]
 
 
-def _val_gene_sim(mapper):
-    vals = np.zeros(4, dtype=np.float32)
-    _lib.check(mapper._lib.tgb200_validation_terms(mapper._h, _lib.ptr(vals), None))
-    return float(vals[_GENE_SIM])
-
-
 def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details=None):
     """:86-139 -- train the configuration `config` n_runs times (random_state = 0, 1, 2, ...) on `data`, the reference's
     12-entry list [S, G, d_source, d, device, print_each, voxel_weights, ct_encode, neighborhood_filter, spatial_weights,
@@ -168,10 +151,10 @@ def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details
             # the reference validates after every update (val_each=1) and keeps only the last score: one evaluation
             # after the final update is the same number
             mapper.train(num_epochs, learning_rate=learning_rate, print_each=print_each, out=cell_cube[run])
-            val_gene_scores.append(_val_gene_sim(mapper))
+            val_gene_scores.append(mapper.validation_terms()["val_gene_sim"])
             t1 = time.perf_counter()
             # :134 -- S[:, val]^T @ mapping, stored transposed: Pearson over flattened runs does not see the order
-            _lib.check(mapper._lib.tgb200_project(mapper._h, _lib.ptr(S_val), n_val, _lib.ptr(gene_cube[run]), None))
+            mapper.project(S_val, out=gene_cube[run])
             t2 = time.perf_counter()
         finally:
             mapper.release()

@@ -19,7 +19,7 @@ import pandas as pd
 from . import _lib
 from . import mapping_utils as mu
 from .adata import make_adata
-from .mapping_parameter_tuning import _require_device
+from .engine import _require_device
 
 _ANN_CHUNK, _ANN_SLAB = 128, 1024       # rows per work item and columns per slab of tgb200_annotate
 
