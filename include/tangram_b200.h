@@ -272,9 +272,16 @@ TGB200_API int tgb200_profile_step(tgb200_mapper* h, float learning_rate, void* 
 TGB200_API int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, double* flops);
 
 /* Diagnostics: copy an internal device buffer to HOST memory after a step.  name: "Y" (V x Ke),
- * "dY" (V x Ke), "rdot" (n_cells), "Sx" (n_cells x Ke), "shape" (Ke, ld, fwd_splits, r_parts); bf16 mode
- * only: "Pb" (n_cells x ld, the resident unnormalised P the next backward consumes), "dq" (n_cells x ld, the
- * backward's centred dP), "rcenter" (n_cells, the centre dq is stored relative to); bf16 buffers widened to float.
+ * "dY" (V x Ke), "rdot" (n_cells), "Sx" (n_cells x Ke), "shape" (Ke, ld, fwd_splits, r_parts,
+ * cell chunks of the bf16 pipeline),
+ * "M", "m", "v" (n_cells x ld, the Adam state, pad columns included), "stats" (n_cells x 4: RowStat mx, inv_z,
+ * log_z, h); fp32 mode: "Pf" (n_cells x ld, P of the last row pass); bf16x3 mode: "Pb" (n_cells x ld, the three
+ * P planes summed), "dpf" (n_cells x ld, the backward's fp32 dP); bf16 mode only: "Pb" (n_cells x ld, the resident
+ * unnormalised P the next backward consumes), "dq" (n_cells x ld, the backward's centred dP), "rcenter" (n_cells, the
+ * centre dq is stored relative to), "rowc" (n_cells x 4: lse, r', h, 0 of the last update), "zsum", "inv_zt", "lseA"
+ * (the offset Pb was written with: after step_end, the exact log-sum-exp of the rows before that update), "lseT" (after
+ * step_begin, the exact log-sum-exp of the current rows; after step_end, free), and "pxsum", "l1sum", "l2sum" (n_cells,
+ * the update's row sums, when the entropy or L1/L2 terms are on); bf16 buffers (the first moment included) widened to float.
  * "legacy_init": the last tgb200_init_mapping_legacy's ms of jump, count + scan, emit and fix-up (CUDA events), ms of host
  * polynomial work, draw blocks, values recomputed on the host, values that recomputation changed.
  * out_host may be NULL to query the size (*n). */

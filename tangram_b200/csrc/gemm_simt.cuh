@@ -23,11 +23,14 @@ struct AdamScalars {
   float beta1, beta2, one_minus_beta1, one_minus_beta2, step_size, bc2_sqrt, eps, inv_bc2_sqrt;
 };
 
+// torch.optim.Adam(foreach=False) on CUDA element for element, each rounding pinned to the one torch's kernels make:
+// lerp_ is self + w (end - self) contracted to one FMA, addcmul_ is self + value (t1 t2), a division of a tensor by a
+// Python scalar multiplies by fp32(1 / scalar), and addcdiv_ is self + value (t1 / t2) contracted to one FMA.
 __device__ __forceinline__ float adam_update(float x, float g, float& m, float& v, const AdamScalars& a) {
-  m = m + (g - m) * a.one_minus_beta1;               // exp_avg.lerp_(grad, 1-beta1)
-  v = v * a.beta2 + a.one_minus_beta2 * g * g;       // mul_(beta2).addcmul_(g, g, 1-beta2)
-  const float denom = sqrtf(v) / a.bc2_sqrt + a.eps; // (sqrt(v)/sqrt(bc2)).add_(eps)
-  return x - a.step_size * (m / denom);              // addcdiv_(m, denom, -step_size)
+  m = fmaf(g - m, a.one_minus_beta1, m);                                       // exp_avg.lerp_(grad, 1-beta1)
+  v = fmaf(a.one_minus_beta2, __fmul_rn(g, g), __fmul_rn(v, a.beta2));         // mul_(beta2).addcmul_(g, g, 1-beta2)
+  const float denom = __fadd_rn(__fmul_rn(sqrtf(v), a.inv_bc2_sqrt), a.eps);   // (sqrt(v) / sqrt(bc2)).add_(eps)
+  return fmaf(-a.step_size, m / denom, x);                                     // addcdiv_(m, denom, -step_size)
 }
 
 // ---- epilogues --------------------------------------------------------------------

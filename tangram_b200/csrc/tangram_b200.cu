@@ -1142,16 +1142,28 @@ static int loss_stage(tgb200_mapper* h, cudaStream_t s, float* hist_row, bool re
   return TGB200_OK;
 }
 
+// The double a caller wrote when it passed `f` through a float field: the shortest decimal that rounds to `f`
+// (0.999f -> 0.999, not 0.99900001287...).  torch computes Adam's scalars from the Python doubles.
+static double as_written(float f) {
+  char buf[32];
+  for (int digits = 1; digits <= 9; ++digits) {
+    snprintf(buf, sizeof(buf), "%.*g", digits, (double)f);
+    if (strtof(buf, nullptr) == f) return strtod(buf, nullptr);
+  }
+  return (double)f;
+}
+
 static AdamScalars adam_scalars(const tgb200_config& c, int64_t t, float lr) {
-  // torch/optim/adam.py (_single_tensor_adam, non-capturable): python-double scalar math
-  const double b1 = (double)c.adam_beta1, b2 = (double)c.adam_beta2;
+  // torch/optim/adam.py (_single_tensor_adam, non-capturable): python-double scalar math, each scalar cast to fp32 by the
+  // kernel that takes it
+  const double b1 = as_written(c.adam_beta1), b2 = as_written(c.adam_beta2);
   const double bc1 = 1.0 - std::pow(b1, (double)t), bc2 = 1.0 - std::pow(b2, (double)t);
   AdamScalars a;
   a.beta1 = c.adam_beta1; a.beta2 = c.adam_beta2;
   a.one_minus_beta1 = (float)(1.0 - b1); a.one_minus_beta2 = (float)(1.0 - b2);
-  a.step_size = (float)((double)lr / bc1);
-  a.bc2_sqrt = (float)std::sqrt(bc2);
-  a.inv_bc2_sqrt = (float)(1.0 / std::sqrt(bc2));
+  a.step_size = (float)(as_written(lr) / bc1);
+  a.bc2_sqrt = (float)std::pow(bc2, 0.5);                       // bias_correction2 ** 0.5
+  a.inv_bc2_sqrt = (float)(1.0 / std::pow(bc2, 0.5));          // torch divides by a Python scalar as a * fp32(1 / b)
   a.eps = c.adam_eps;
   return a;
 }
@@ -1703,8 +1715,33 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
   const std::string nm(name);
   const float* src = nullptr;
   int64_t cnt = 0;
-  const int64_t vk = (int64_t)h->V * h->Ke;
+  const int64_t vk = (int64_t)h->V * h->Ke, nv = (int64_t)h->N * h->ld;
+  // bf16 buffers (`planes` bf16 planes of n elements, summed) widened to float
+  auto widened = [&](const __nv_bfloat16* p, int64_t count, int planes) -> int {
+    *n = count;
+    if (!out_host) return TGB200_OK;
+    if (cap < count) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)count);
+    return widen_bf16(p, count, planes, out_host);
+  };
   if (nm == "Y") { src = h->Y.p; cnt = vk; }
+  else if (nm == "M") { src = h->M.p; cnt = nv; }
+  else if (nm == "v") { src = h->v.p; cnt = nv; }
+  else if (nm == "m") {
+    if (h->bf16) return widened(h->mb.p, nv, 1);
+    src = h->m.p; cnt = nv;
+  }
+  else if (nm == "Pb" && h->x3) return widened(h->Pb.p, nv, 3);
+  else if (nm == "Pf" && !h->tcm) { src = h->Pf.p; cnt = nv; }
+  else if (nm == "dpf" && h->x3) { src = h->dpf.p; cnt = nv; }
+  else if (nm == "stats") { src = reinterpret_cast<const float*>(h->stats.p); cnt = (int64_t)h->N * 4; }
+  else if (nm == "rowc" && h->bf16) { src = reinterpret_cast<const float*>(h->rowc.p); cnt = (int64_t)h->N * 4; }
+  else if (nm == "zsum" && h->bf16) { src = h->zsum.p; cnt = h->N; }
+  else if (nm == "inv_zt" && h->bf16) { src = h->inv_zt.p; cnt = h->N; }
+  else if (nm == "lseA" && h->bf16) { src = h->lseA; cnt = h->N; }
+  else if (nm == "lseT" && h->bf16) { src = h->lseT; cnt = h->N; }
+  else if (nm == "pxsum" && h->pxsum.p) { src = h->pxsum.p; cnt = h->N; }
+  else if (nm == "l1sum" && h->l1sum.p) { src = h->l1sum.p; cnt = h->N; }
+  else if (nm == "l2sum" && h->l2sum.p) { src = h->l2sum.p; cnt = h->N; }
   else if (nm == "dY") {
     src = h->dY.p; cnt = vk;
     if (h->tcm && out_host) {     // only the bf16 copy (or its three planes) exists on the tensor-core paths
@@ -1714,24 +1751,16 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
       return TGB200_OK;
     }
   }
-  else if ((nm == "dq" || nm == "Pb") && h->bf16) {    // N x ld bf16, widened
-    cnt = (int64_t)h->N * h->ld;
-    *n = cnt;
-    if (out_host) {
-      if (cap < cnt) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)cnt);
-      CKS(widen_bf16(nm == "dq" ? h->dq.p : h->Pb.p, cnt, 1, out_host));
-    }
-    return TGB200_OK;
-  }
+  else if ((nm == "dq" || nm == "Pb") && h->bf16) return widened(nm == "dq" ? h->dq.p : h->Pb.p, nv, 1);
   else if (nm == "rcenter" && h->bf16) { src = h->rcenter.p; cnt = h->N; }
   else if (nm == "rdot") { src = h->rdot.p; cnt = h->N; }
   else if (nm == "Sx") { src = h->Sx.p; cnt = (int64_t)h->N * h->Ke; }
-  else if (nm == "shape") {   // Ke, ld, fwd_splits, r_parts
-    *n = 4;
+  else if (nm == "shape") {   // Ke, ld, fwd_splits, r_parts, cell chunks of the bf16 pipeline
+    *n = 5;
     if (!out_host) return TGB200_OK;
-    if (cap < 4) return fail(TGB200_ERR_INVALID, "cap < 4");
+    if (cap < 5) return fail(TGB200_ERR_INVALID, "cap < 5");
     out_host[0] = (float)h->Ke; out_host[1] = (float)h->ld; out_host[2] = (float)h->fwd_splits; out_host[3] = (float)h->r_parts;
-    *n = 4;
+    out_host[4] = (float)h->nchunks;
     return TGB200_OK;
   } else if (nm == "legacy_init") {
     *n = 8;

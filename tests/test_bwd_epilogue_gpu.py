@@ -12,6 +12,7 @@ CASES = [
     (3000, 2000, 100),   # 192 output tiles, more than there are SMs: CTAs reuse their Pt / dq buffer and barrier phases
     (1000, 257, 130),    # ragged rows and columns, ld = 320
     (9000, 300, 70),     # two cell chunks, one launch each; the last row tile is ragged and its second half empty
+    (33000, 130, 40),    # four cell chunks, one launch each; the last chunk ragged
 ]
 
 
