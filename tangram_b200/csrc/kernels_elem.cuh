@@ -3,6 +3,7 @@
 // Reference: tangram/mapping_optimizer.py:189-309 (_loss_fn).
 #pragma once
 #include "common.cuh"
+#include "gemm_simt.cuh"       // adam_update (k_filter_update)
 #include <curand_kernel.h>
 
 namespace tgb {
@@ -221,23 +222,24 @@ __global__ void k_filter_prepare(const float* __restrict__ F, const float* __res
   v.x *= fi; v.y *= fi; v.z *= fi; v.w *= fi;
   reinterpret_cast<float4*>(Sf)[q] = v;
 }
-// dL/df_i = r_i / f_i (the row-dot of the contractions: Y is linear in f_i) + density/count/regulariser parts;
-// dL/dF_i = dL/df_i f_i (1 - f_i); Adam on F with the same scalars as M (one optimizer over [M, F], :607).
+// dL/df_i = r_i / f_i (the row-dot of the contractions: Y is linear in f_i) + density/count/regulariser parts, and
+// dL/dF_i = dL/df_i f_i (1 - f_i).  Formed without the division,
+//   g_i = r_i (1 - f_i) + (fscal[0] + lam_c fscal[1] + lam_f (1 - 2 f_i)) f_i (1 - f_i),
+// so a saturated cell (f_i exactly 0 or 1, r_i = 0) gets g_i = 0 and keeps its F, as F.grad = grad f (1 - f) does in the
+// reference (:507), instead of 0 / 0.  Every rounding is pinned (no contraction) so a test can form the same g in fp32.
+// Then torch's Adam step with the same scalars as M (one optimizer over [M, F], :607).
 // fscal: [0] lambda_d * sum(d) / sum(f)   [1] sign(sum(f) - target_count)
-struct AdamScalarsF { float one_minus_beta1, beta2, one_minus_beta2, step_size, bc2_sqrt, eps; };
 __global__ void k_filter_update(int n_rows, const float* __restrict__ rdot, const float* __restrict__ f,
-                                const float* __restrict__ fscal, float lam_c, float lam_f, AdamScalarsF a,
+                                const float* __restrict__ fscal, float lam_c, float lam_f, AdamScalars a,
                                 float* __restrict__ F, float* __restrict__ mF, float* __restrict__ vF) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_rows) return;
   const float fi = f[i];
-  const float df = rdot[i] / fi + fscal[0] + lam_c * fscal[1] + lam_f * (1.f - 2.f * fi);
-  const float g = df * fi * (1.f - fi);
+  const float omf = __fsub_rn(1.f, fi);
+  const float c = __fadd_rn(__fadd_rn(fscal[0], __fmul_rn(lam_c, fscal[1])), __fmul_rn(lam_f, __fsub_rn(1.f, __fmul_rn(2.f, fi))));
+  const float g = __fadd_rn(__fmul_rn(rdot[i], omf), __fmul_rn(c, __fmul_rn(fi, omf)));
   float m = mF[i], v = vF[i];
-  m = m + (g - m) * a.one_minus_beta1;
-  v = v * a.beta2 + a.one_minus_beta2 * g * g;
-  const float denom = sqrtf(v) / a.bc2_sqrt + a.eps;
-  F[i] = F[i] - a.step_size * (m / denom);
+  F[i] = adam_update(F[i], g, m, v, a);
   mF[i] = m; vF[i] = v;
 }
 __global__ void k_sigmoid(const float* __restrict__ F, int n, float* __restrict__ out) {

@@ -1169,9 +1169,8 @@ static AdamScalars adam_scalars(const tgb200_config& c, int64_t t, float lr) {
 }
 
 static int filter_update(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a) {
-  const AdamScalarsF af{a.one_minus_beta1, a.beta2, a.one_minus_beta2, a.step_size, a.bc2_sqrt, a.eps};
   k_filter_update<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->N, h->rdot.p, h->fsig.p, h->fscal.p, h->cfg.lambda_count,
-                                                                 h->cfg.lambda_f_reg, af, h->Fl.p, h->mF.p, h->vF.p);
+                                                                 h->cfg.lambda_f_reg, a, h->Fl.p, h->mF.p, h->vF.p);
   LAUNCH_CHECK("filter_update");
   return TGB200_OK;
 }
@@ -1755,6 +1754,13 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
   else if (nm == "rcenter" && h->bf16) { src = h->rcenter.p; cnt = h->N; }
   else if (nm == "rdot") { src = h->rdot.p; cnt = h->N; }
   else if (nm == "Sx") { src = h->Sx.p; cnt = (int64_t)h->N * h->Ke; }
+  else if (nm == "tail") { src = h->Y.p + vk; cnt = kTail; }       // the row-scalar sums after Y_ext (k_row_scalar_reduce)
+  else if (h->constrained && (nm == "F" || nm == "f" || nm == "mF" || nm == "vF")) {
+    src = nm == "F" ? h->Fl.p : nm == "f" ? h->fsig.p : nm == "mF" ? h->mF.p : h->vF.p;
+    cnt = h->N;
+  }
+  else if (nm == "Sf" && h->constrained) { src = h->Sf.p; cnt = (int64_t)h->N * h->Ke; }
+  else if (nm == "fscal" && h->constrained) { src = h->fscal.p; cnt = 2; }
   else if (nm == "shape") {   // Ke, ld, fwd_splits, r_parts, cell chunks of the bf16 pipeline
     *n = 5;
     if (!out_host) return TGB200_OK;
