@@ -167,6 +167,16 @@ TGB200_API int tgb200_mt19937_jump_pow2(const tgb200_mt_state* in, uint32_t log2
  * anew (:373, :607) -- zero moments, bias correction restarts at t = 1.  M, F, the history and its length are kept. */
 TGB200_API int tgb200_reset_adam(tgb200_mapper* h, void* stream);
 
+/* Restrict the loss to a subset of the n_genes training columns (the reference builds the Mapper on S[:, train_genes],
+ * mapping_utils.py:246-275, once per cross-validation fold, utils.py:580-600).  `active`: n_genes bytes (0/1), host;
+ * NULL = all genes (the default; an all-ones mask is the same).  The handle then computes what a handle created on
+ * S[:, active], G[:, active] computes from the same mapping: every cosine term (gene-voxel, voxel-gene, neighbourhood,
+ * Getis-Ord), its history columns and tgb200_validation_terms run over the active genes, and dL/dY is exactly 0 on the
+ * other gene columns.  Density, entropy, L1/L2, cell-type islands and the filter are unaffected.  The mapping, the
+ * filter, the Adam state and the history are kept.  A sharded handle needs the same mask on every rank.
+ * TGB200_ERR_INVALID when no gene is active or a byte is not 0/1; TGB200_ERR_STATE between step_begin and step_end. */
+TGB200_API int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, void* stream);
+
 /* Constrained mode: initial filter logits F0 (n_cells, host or device; the reference draws them at :490).
  * Resets the filter's Adam state. */
 TGB200_API int tgb200_set_filter(tgb200_mapper* h, const float* F0, void* stream);

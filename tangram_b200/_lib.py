@@ -76,6 +76,7 @@ SIGNATURES = {
     "tgb200_mt19937_jump": (ctypes.c_int, [ctypes.POINTER(MtState), ctypes.c_uint64, ctypes.POINTER(MtState)]),
     "tgb200_mt19937_jump_pow2": (ctypes.c_int, [ctypes.POINTER(MtState), ctypes.c_uint32, ctypes.POINTER(MtState)]),
     "tgb200_reset_adam": (ctypes.c_int, [_P, _P]),
+    "tgb200_set_loss_genes": (ctypes.c_int, [_P, _P, _P]),
     "tgb200_set_filter": (ctypes.c_int, [_P, _P, _P]),
     "tgb200_get_filter": (ctypes.c_int, [_P, _P, _P, _P]),
     "tgb200_run": (ctypes.c_int, [_P, ctypes.c_int32, ctypes.c_float, _P]),

@@ -260,6 +260,10 @@ constexpr int kLossCols = 128;  // gene columns per CTA (= threads)
 
 struct LossParams {
   int V, K, Ke, T, ct_off, density_mode;
+  // Training-gene mask (tgb200_set_loss_genes): act[k] = 1 for the Kact genes the loss sees, 0 for the others; null
+  // when every gene is in the loss (Kact == K).  The cosine terms then run over the active genes only, as on S[:, a].
+  const float* act;
+  int Kact;
   long long n_cells_global;
   float lam_g1, lam_d, lam_g2, lam_r, lam_l1, lam_l2, lam_nb, lam_ct, lam_go;
   const float* G;     // V x Ke, zero beyond K
@@ -300,6 +304,9 @@ struct LossParams {
 constexpr int kLossRowsMax = 128;
 constexpr int kLossVec = 4;                       // columns per thread (float4)
 constexpr int kLossColsBlk = kLossCols * kLossVec;  // columns per CTA
+// kMasked: the row statistics skip the genes outside p.act.  A template argument, not a test of p.act: the unmasked
+// instantiation keeps its contracted multiply-adds, so its results do not depend on whether this kernel can mask.
+template <bool kMasked>
 __global__ void __launch_bounds__(kLossCols)
 k_loss_reduce(LossParams p, const float* __restrict__ part, int nsplit, int row_stats, int rows_per_block) {
   __shared__ float shr[4][kLossRowsMax][2];
@@ -328,7 +335,7 @@ k_loss_reduce(LossParams p, const float* __restrict__ part, int nsplit, int row_
       for (int e = 0; e < 4; ++e) {
         if (k + e < p.K) {
           dot[e] += yv[e] * gv[e]; ny2[e] += yv[e] * yv[e]; ys[e] += yv[e];
-          a += yv[e] * gv[e]; b += yv[e] * yv[e];
+          if (!kMasked || p.act[k + e] != 0.f) { a += yv[e] * gv[e]; b += yv[e] * yv[e]; }
         }
       }
     }
@@ -420,13 +427,21 @@ k_ct_islands(LossParams p) {
 // One CTA: finishes every reduction, writes the history row and the dY coefficients.
 // cos(x,y) = <x,y> / (max(|x|,eps) max(|y|,eps))   (torch semantics, :205-206)
 // d mean_k cos / dY_jk = a_k G_jk - b_k Y_jk,  a_k = 1/(K ny ng),  b_k = cos_k/(K ny^2)
+// Under a gene mask the means run over the Kact active genes and an inactive gene's coefficients are 0.
 __global__ void __launch_bounds__(1024)
 k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist_row) {
   __shared__ float sh[32];
   const int tid = threadIdx.x, nt = blockDim.x;
   const float nan = __int_as_float(0x7fc00000);
+  const float Kf = (float)p.Kact;
   float gv = 0.f, nb = 0.f, go = 0.f;
   for (int k = tid; k < p.K; k += nt) {
+    if (p.act != nullptr && p.act[k] == 0.f) {
+      p.coefA[k] = 0.f; p.coefB[k] = 0.f;
+      if (p.lam_nb > 0.f) { p.coefAn[k] = 0.f; p.coefBn[k] = 0.f; }
+      if (p.lam_go > 0.f) { p.coefAg[k] = 0.f; p.coefBg[k] = 0.f; }
+      continue;
+    }
     float dot = 0.f, ny2 = 0.f, ys = 0.f;
     for (int c = 0; c < nchunk; ++c) {
       const float* cp = p.colpart + (size_t)c * 3 * p.Ke;
@@ -435,8 +450,8 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
     const float ny = fmaxf(sqrtf(ny2), kCosEps), ng = p.ngc[k];
     const float cs = dot / (ny * ng);
     gv += cs;
-    p.coefA[k] = p.lam_g1 / ((float)p.K * ny * ng);
-    p.coefB[k] = p.lam_g1 * cs / ((float)p.K * ny * ny);
+    p.coefA[k] = p.lam_g1 / (Kf * ny * ng);
+    p.coefB[k] = p.lam_g1 * cs / (Kf * ny * ny);
     if (p.lam_nb > 0.f) {
       float d2 = 0.f, n2 = 0.f;
       for (int c = 0; c < nchunk; ++c) {
@@ -446,8 +461,8 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
       const float nz = fmaxf(sqrtf(n2), kCosEps), nr = p.nwg[k];
       const float c2 = d2 / (nz * nr);
       nb += c2;
-      p.coefAn[k] = p.lam_nb / ((float)p.K * nz * nr);
-      p.coefBn[k] = p.lam_nb * c2 / ((float)p.K * nz * nz);
+      p.coefAn[k] = p.lam_nb / (Kf * nz * nr);
+      p.coefBn[k] = p.lam_nb * c2 / (Kf * nz * nz);
     }
     if (p.lam_go > 0.f) {
       // cos(G*(G), G*(Y)) with G*(X) = (A+I) X / colsum(X)  (:171): the per-gene scale
@@ -461,13 +476,13 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
       const float nz = fmaxf(sqrtf(n2), kCosEps), nr = p.nag[k];
       const float c2 = d2 / (nz * nr);
       go += sgn * c2;
-      p.coefAg[k] = sgn * p.lam_go / ((float)p.K * nz * nr);
-      p.coefBg[k] = sgn * p.lam_go * c2 / ((float)p.K * nz * nz);
+      p.coefAg[k] = sgn * p.lam_go / (Kf * nz * nr);
+      p.coefBg[k] = sgn * p.lam_go * c2 / (Kf * nz * nz);
     }
   }
-  gv = block_reduce<false>(gv, sh) / (float)p.K;
-  nb = block_reduce<false>(nb, sh) / (float)p.K;
-  go = block_reduce<false>(go, sh) / (float)p.K;
+  gv = block_reduce<false>(gv, sh) / Kf;
+  nb = block_reduce<false>(nb, sh) / Kf;
+  go = block_reduce<false>(go, sh) / Kf;
 
   float vg = 0.f;
   if (p.lam_g2 != 0.f) {
@@ -565,6 +580,7 @@ k_dy_assemble(LossParams p, float* __restrict__ dY, __nv_bfloat16* __restrict__ 
     const int k = k0 + e;
     float dy = 0.f;
     if (k < p.K) {
+      if (p.act != nullptr && p.act[k] == 0.f) { out[e] = 0.f; continue; }   // a gene outside the loss: exactly 0
       const float y = yv[e], g = gv[e];
       dy = -(p.coefA[k] * g - p.coefB[k] * y);
       if (p.lam_g2 != 0.f) dy -= p.coefAr[j] * g - p.coefBr[j] * y;
@@ -625,12 +641,16 @@ __global__ void k_col_norms(int V, int K, int Ke, const float* __restrict__ X, f
   nrm[k] = fmaxf(sqrtf(s2), kCosEps);
   if (sgn) sgn[k] = s > 0.f ? 1.f : -1.f;
 }
-// per-row clamped norm over the K gene columns (warp per row)
-__global__ void k_row_norms(int V, int K, int Ke, const float* __restrict__ X, float* __restrict__ nrm) {
+// per-row clamped norm over the K gene columns, or over the active ones of a gene mask `act` (warp per row)
+__global__ void k_row_norms(int V, int K, int Ke, const float* __restrict__ X, const float* __restrict__ act,
+                            float* __restrict__ nrm) {
   const int j = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (j >= V) return;
   float s2 = 0.f;
-  for (int k = threadIdx.x & 31; k < K; k += 32) { const float x = X[(size_t)j * Ke + k]; s2 += x * x; }
+  for (int k = threadIdx.x & 31; k < K; k += 32) {
+    if (act != nullptr && act[k] == 0.f) continue;
+    const float x = X[(size_t)j * Ke + k]; s2 += x * x;
+  }
   s2 = warp_sum(s2);
   if ((threadIdx.x & 31) == 0) nrm[j] = fmaxf(sqrtf(s2), kCosEps);
 }

@@ -132,6 +132,12 @@ struct tgb200_mapper {
   CsrDev W, WT, F, FT, A, AT;
   int nchunk = 0, ncolchunk = 0, nredchunk = 0, n_ct_blocks = 0, loss_rows = 16;
   DevBuf<float> colfin;         // finalised per-gene sums: [3 | 2 | 2][Ke]
+  // training-gene mask of the loss (tgb200_set_loss_genes): gene_act[k] in {0, 1} (Ke floats, device and host) when
+  // `masked`; n_active of the K genes are in the loss
+  bool masked = false;
+  int n_active = 0;
+  DevBuf<float> gene_act;
+  std::vector<float> gene_act_host;
   // history
   DevBuf<float> hist;
   int64_t hist_len = 0, hist_cap = 0;
@@ -293,6 +299,7 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (h->cfg.adam_beta2 == 0.f) h->cfg.adam_beta2 = 0.999f;
   if (h->cfg.adam_eps == 0.f) h->cfg.adam_eps = 1e-8f;
   h->N = cfg->n_cells; h->V = cfg->n_voxels; h->K = cfg->n_genes; h->T = cfg->n_types;
+  h->n_active = h->K;
   h->constrained = cfg->constrained != 0;
   h->bf16 = cfg->precision == TGB200_PREC_BF16;
   h->x3 = cfg->precision == TGB200_PREC_BF16X3;
@@ -474,7 +481,7 @@ extern "C" int tgb200_set_expression(tgb200_mapper* h, const float* S, const flo
   CKS(upload_padded(h, G, h->V, h->K, h->G.p, h->Ke, 0, s));
   k_col_norms<<<(unsigned)ceil_div(h->K, 128), 128, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->ngc.p, nullptr);
   LAUNCH_CHECK("col_norms");
-  k_row_norms<<<(unsigned)ceil_div(h->V, 8), 256, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->ngr.p);
+  k_row_norms<<<(unsigned)ceil_div(h->V, 8), 256, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->masked ? h->gene_act.p : nullptr, h->ngr.p);
   LAUNCH_CHECK("row_norms");
   h->have_expr = true;
   h->have_ct = false;
@@ -587,6 +594,41 @@ extern "C" int tgb200_reset_adam(tgb200_mapper* h, void* stream) {
     CK(cudaMemsetAsync(h->vF.p, 0, h->vF.n * sizeof(float), s));
   }
   h->step = 0;
+  return TGB200_OK;
+}
+
+// The loss over a subset of the training genes (one cross-validation fold): the handle then computes what a handle created
+// on S[:, active], G[:, active] computes.  The per-voxel norms of G (lambda_g2) follow the mask; M, F, the Adam state and
+// the history are kept.  An all-ones mask is no mask.
+extern "C" int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, void* stream) {
+  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
+  if (h->in_step) return fail(TGB200_ERR_STATE, "set_loss_genes inside a step");
+  int n = h->K;
+  std::vector<float> flags;
+  if (active) {
+    flags.assign(h->Ke, 0.f);
+    n = 0;
+    for (int k = 0; k < h->K; ++k) {
+      if (active[k] > 1) return fail(TGB200_ERR_INVALID, "active[%d] = %d, expected 0 or 1", k, (int)active[k]);
+      flags[k] = (float)active[k];
+      n += active[k];
+    }
+    if (n == 0) return fail(TGB200_ERR_INVALID, "no gene is active");
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(h->cfg.device));
+  h->masked = n < h->K;
+  h->n_active = n;
+  if (h->masked) {
+    if (!h->gene_act.p) CKS(h->gene_act.alloc(h->Ke, false));
+    h->gene_act_host.swap(flags);
+    CK(cudaMemcpyAsync(h->gene_act.p, h->gene_act_host.data(), sizeof(float) * h->Ke, cudaMemcpyHostToDevice, s));
+  }
+  if (h->have_expr) {
+    k_row_norms<<<(unsigned)ceil_div(h->V, 8), 256, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->masked ? h->gene_act.p : nullptr, h->ngr.p);
+    LAUNCH_CHECK("row_norms");
+  }
+  CK(cudaStreamSynchronize(s));
   return TGB200_OK;
 }
 
@@ -915,6 +957,7 @@ static LossParams make_loss_params(tgb200_mapper* h) {
   memset(&p, 0, sizeof(p));
   const tgb200_config& c = h->cfg;
   p.V = h->V; p.K = h->K; p.Ke = h->Ke; p.T = h->T; p.ct_off = h->ct_off; p.density_mode = c.density_mode;
+  p.act = h->masked ? h->gene_act.p : nullptr; p.Kact = h->n_active;
   p.n_cells_global = c.n_cells_global;
   p.lam_g1 = c.lambda_g1; p.lam_d = c.lambda_d; p.lam_g2 = c.lambda_g2; p.lam_r = c.lambda_r;
   p.lam_l1 = c.lambda_l1; p.lam_l2 = c.lambda_l2; p.lam_nb = c.lambda_neighborhood_g1;
@@ -1099,7 +1142,8 @@ static int ensure_history(tgb200_mapper* h, int64_t need, cudaStream_t s) {
 static int reduce_columns(tgb200_mapper* h, cudaStream_t s, LossParams& p, bool from_partials, int with_g2) {
   const bool planes = from_partials && h->fwd_splits > 1;
   dim3 vgrid(h->nredchunk, h->nchunk);          // four columns per thread
-  k_loss_reduce<<<vgrid, kLossCols, 0, s>>>(p, planes ? h->Ypart.p : h->Y.p, planes ? h->fwd_splits : 1, with_g2, h->loss_rows);
+  auto reduce = p.act ? k_loss_reduce<true> : k_loss_reduce<false>;
+  reduce<<<vgrid, kLossCols, 0, s>>>(p, planes ? h->Ypart.p : h->Y.p, planes ? h->fwd_splits : 1, with_g2, h->loss_rows);
   LAUNCH_CHECK("loss_reduce");
   k_col_finalize<<<dim3((unsigned)ceil_div(h->Ke, 128), 3), 128, 0, s>>>(h->colpart.p, h->nchunk, 3, h->Ke, h->colfin.p);
   LAUNCH_CHECK("col_finalize");
@@ -1618,14 +1662,16 @@ extern "C" int tgb200_validation_terms(tgb200_mapper* h, float* out4, void* stre
   std::vector<float> ngc(h->K);
   CK(cudaMemcpyAsync(ngc.data(), h->ngc.p, sizeof(float) * h->K, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  // cos_k = coefB_k * K * ny^2 with ny = 1/(coefA_k * K * ng)  (lam_g1 = 1 here)
+  // cos_k = coefB_k * K' * ny^2 with ny = 1/(coefA_k * K' * ng)  (lam_g1 = 1 here; the K' genes of the loss)
   double wsum = 0.0, acc = 0.0;
+  const double Kd = h->n_active;
   for (int k = 0; k < h->K; ++k) {
+    if (h->masked && h->gene_act_host[k] == 0.f) continue;
     long nz = 0;
     for (int j = 0; j < h->V; ++j) nz += Gh[(size_t)j * h->Ke + k] != 0.f;
     const double w = (double)nz / h->V;       // 1 - gene_sparsity (:330)
-    const double ny = 1.0 / ((double)cA[k] * h->K * ngc[k]);
-    const double cosk = (double)cB[k] * h->K * ny * ny;
+    const double ny = 1.0 / ((double)cA[k] * Kd * ngc[k]);
+    const double cosk = (double)cB[k] * Kd * ny * ny;
     wsum += w; acc += cosk * w;
   }
   const float gv = hrow[1], vg = hrow[2];

@@ -129,6 +129,18 @@ class Engine:
         """Constrained mode: copy the filter logits F and/or sigmoid(F) (n_cells each; None skips) out of the handle."""
         _lib.check(self._lib.tgb200_get_filter(self._h, _lib.ptr(logits), _lib.ptr(sigmoid), self._s(stream)))
 
+    def set_loss_genes(self, active=None, stream=None):
+        """Restrict the loss to the genes flagged in `active` (n_genes booleans or 0/1 values; None = every gene).  The
+        handle then computes what a handle created on S[:, active], G[:, active] computes from the same mapping; the
+        mapping, the Adam state and the history are kept (tgb200_set_loss_genes)."""
+        a = None
+        if active is not None:
+            a = np.asarray(active)
+            if a.shape != (self.cfg.n_genes,):
+                raise ValueError(f"active has shape {a.shape}, expected ({self.cfg.n_genes},)")
+            a = np.ascontiguousarray(a, dtype=np.uint8)
+        _lib.check(self._lib.tgb200_set_loss_genes(self._h, _lib.ptr(a), self._s(stream)))
+
     def reset_adam(self, stream=None):
         _lib.check(self._lib.tgb200_reset_adam(self._h, self._s(stream)))
 

@@ -127,17 +127,23 @@ class _EngineMapper:
     def _run(self, n_steps, lr):
         self._engine.run(n_steps, lr)
 
-    def _fit(self, num_epochs, lr, print_each, resume, out=None, val_each=None, val_history=None):
+    def _set_loss_genes(self, active):
+        """Cross-validation fold: the loss sees only the genes flagged in `active` (n_genes booleans; None = all), as a
+        mapper built on S[:, active], G[:, active] would (Engine.set_loss_genes)."""
+        self._engine.set_loss_genes(active)
+
+    def _fit(self, num_epochs, lr, print_each, resume, out=None, val_each=None, val_history=None, fetch=True):
         """num_epochs updates (a fresh Adam unless `resume`), run in chunks that end where the reference prints or
         validates (every `val_each` epochs, into the lists of `val_history`).  Sets history_matrix to this call's rows
-        and returns softmax(M), in `out` or a host array."""
+        and returns softmax(M), in `out` or a host array; with fetch=False (cross-validation scores genes with project()
+        and needs no mapping on the host) it returns None."""
         if not resume:
             self._engine.reset_adam()
         first = self._engine.history_len()
+        result = None
         if out is not None:
             self._check_out(out, (self.n_cells, self.n_voxels))
-            result = None
-        else:
+        elif fetch:
             result = _ResultBuffer(_lib.load(), (self.n_cells, self.n_voxels), self._cfg.device)
         try:
             t = 0
@@ -156,6 +162,8 @@ class _EngineMapper:
                         val_history[k].append(x)
                 t += chunk
             self.history_matrix = self._engine.history(first, num_epochs)
+            if out is None and result is None:
+                return None
             return self._engine.get_mapping(out if out is not None else result.ready())
         finally:
             if result is not None:
@@ -247,13 +255,8 @@ class Mapper(_EngineMapper):
             self._rows = shard_rows(n_cells_global, r, w)
         r0, r1 = self._rows
         self._sharded = (r1 - r0) != n_cells_global
-        # initial mapping: legacy numpy RNG, float64 draw, f32 cast; seeded only if truthy (:147-157).  A rank of a
-        # sharded run draws the same stream and keeps only its rows (pre-sharded callers pass M0 or get a per-rank draw).
-        # The draw runs on the device (legacy_rng) unless this numpy's arithmetic differs from the device formula.
-        device_draw = M0 is None and not presharded and legacy_rng.device_draw_supported()
-        if M0 is None and not device_draw:
-            M0 = legacy_normal_rows(self.random_state, n_rows_given, n_voxels, r0, r1)
-        elif M0 is not None:
+        self._presharded = presharded
+        if M0 is not None:
             M0 = M0[r0:r1]
 
         e = self._engine = Engine(
@@ -286,16 +289,29 @@ class Mapper(_EngineMapper):
             if ct_encode is None:
                 raise ValueError("ct_encode is required when lambda_ct_islands > 0")
             e.set_ct_encode(np.ascontiguousarray(ct_encode[r0:r1]))
-        if device_draw:
-            if self.random_state:
-                np.random.seed(seed=self.random_state)
-            legacy_rng.draw_global(e, 0, r0, r1 * n_voxels)      # the generator ends after row r1, as on the host
+        if M0 is None:
+            self._draw_initial_mapping()
         else:
             e.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
             del M0
         self._own_comm = False
         if self._sharded and process_group is not None:
             self._init_comm(process_group)
+
+    def _draw_initial_mapping(self):
+        """The reference's initial mapping (:147-157): np.random.normal(0, 1, (N, V)) from numpy's legacy global generator,
+        seeded first only if random_state is truthy, cast to float32.  A rank of a sharded run draws the same stream and
+        keeps only its rows (pre-sharded callers get a per-rank draw).  The draw runs on the device (legacy_rng) unless
+        this numpy's arithmetic differs from the device formula; either way the generator ends where the host draw leaves
+        it.  Resets the Adam state and the history."""
+        r0, r1 = self._rows
+        if not self._presharded and legacy_rng.device_draw_supported():
+            if self.random_state:
+                np.random.seed(seed=self.random_state)
+            legacy_rng.draw_global(self._engine, 0, r0, r1 * self.n_voxels)   # the generator ends after row r1
+        else:
+            M0 = legacy_normal_rows(self.random_state, r1, self.n_voxels, r0, r1)
+            self._engine.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
 
     def _init_comm(self, pg):
         """NCCL group: lend the handle the process-level communicator of this group (tangram_b200.sharded.nccl_comm_for_group,
@@ -388,15 +404,6 @@ class MapperConstrained(_EngineMapper):
         G = np.ascontiguousarray(np.asarray(G, dtype=np.float32))
         n_cells, n_voxels, n_genes = S.shape[0], G.shape[0], S.shape[1]
         self.target_density_enabled = d is not None
-        draw = M0 is None or F0 is None
-        device_draw = draw and legacy_rng.device_draw_supported()
-        if draw and not device_draw:
-            # :472-493 -- M is drawn twice (the second draw is used), F after it, legacy numpy RNG
-            if self.random_state:
-                np.random.seed(seed=self.random_state)
-            np.random.normal(0, 1, (n_cells, n_voxels))
-            M0 = np.random.normal(0, 1, (n_cells, n_voxels))
-            F0 = np.random.normal(0, 1, n_cells)
         e = self._engine = Engine(
             n_cells, n_voxels, n_genes, device=_device_index(device), precision=precision,
             density_mode=_lib.DENSITY_CELLS if self.target_density_enabled else _lib.DENSITY_NONE,
@@ -408,15 +415,26 @@ class MapperConstrained(_EngineMapper):
         e.set_expression(S, G)
         if self.target_density_enabled:
             e.set_density(np.ascontiguousarray(np.asarray(d, dtype=np.float32)))
-        if device_draw:
-            # the same three draws: the first N x V normals are skipped, the second N x V land in M, F follows on the host
-            if self.random_state:
-                np.random.seed(seed=self.random_state)
-            legacy_rng.draw_global(e, n_cells * n_voxels, 0, 2 * n_cells * n_voxels)
-            F0 = np.random.normal(0, 1, n_cells)
+        if M0 is None or F0 is None:
+            self._draw_initial_mapping()
         else:
             e.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
-        e.set_filter(np.ascontiguousarray(F0, dtype=np.float32))
+            e.set_filter(np.ascontiguousarray(F0, dtype=np.float32))
+
+    def _draw_initial_mapping(self):
+        """The reference's initial M and F (:472-493) from numpy's legacy global generator, seeded first only if
+        random_state is truthy: M is drawn twice (the second draw is used), F after it.  M is drawn on the device when
+        this numpy's arithmetic matches the device formula (the first N x V normals are skipped), F on the host.  Resets
+        the Adam state (of M and F) and the history."""
+        n_cells, n_voxels = self.n_cells, self.n_voxels
+        if self.random_state:
+            np.random.seed(seed=self.random_state)
+        if legacy_rng.device_draw_supported():
+            legacy_rng.draw_global(self._engine, n_cells * n_voxels, 0, 2 * n_cells * n_voxels)
+        else:
+            np.random.normal(0, 1, (n_cells, n_voxels))
+            self._engine.set_mapping(np.ascontiguousarray(np.random.normal(0, 1, (n_cells, n_voxels)), dtype=np.float32))
+        self._engine.set_filter(np.ascontiguousarray(np.random.normal(0, 1, n_cells), dtype=np.float32))
 
     def _print_terms(self, row):
         return zip(self._PRINT_NAMES, self._values_from_row(row))

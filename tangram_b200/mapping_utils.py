@@ -114,27 +114,13 @@ def _validate_mapping_args(mode, cluster_label, lambda_g1, lambda_d, density_pri
     return lambda_d
 
 
-def map_cells_to_space(
-    adata_sc, adata_sp, cv_train_genes=None, cluster_label=None, mode="cells", device="cuda:0",
-    learning_rate=0.1, num_epochs=1000, scale=True,
-    lambda_d=0, lambda_g1=1, lambda_g2=0, lambda_r=0, lambda_l1=0, lambda_l2=0,
-    lambda_count=1, lambda_f_reg=1, target_count=None,
-    lambda_neighborhood_g1=0, lambda_ct_islands=0, lambda_getis_ord=0, lambda_moran=0, lambda_geary=0,
-    random_state=None, verbose=True, density_prior="rna_count_based", precision="bf16x3",
-    process_group=None, gather=False, keep_on_device=False,
-):
-    """Same contract as the reference (mapping_utils.py:141-428); `device` must be CUDA.  Added keywords:
-    precision       "bf16x3" parity-grade on tensor cores (default) | "fp32" FFMA | "bf16" throughput
-    process_group   torch.distributed group, one process per GPU (mode='cells' only): every rank passes the SAME adata_sc /
-                    adata_sp; the cells are sharded in contiguous blocks (tangram_b200.shard_rows), each rank draws only its
-                    rows of the reference's M0 stream and trains them, one NCCL exchange per epoch.  Each rank returns the
-                    AnnData of ITS cells (obs = that block of adata_sc.obs; `uns['shard_rows']` = (first, last)); the
-                    per-gene scores, the history and `uns` are global and identical on every rank.  gather=True: rank 0
-                    additionally receives the full mapping (all cells) and the other ranks return None.
-    keep_on_device  keep the trained mapper (device state ~20 B per mapping element) attached to the result so that
-                    project_genes contracts on the GPU; default: release it (`adata_map.X` is all project_genes needs)."""
-    if process_group is not None and mode != "cells":
-        raise ValueError("process_group shards the cells axis: only mode='cells' can be sharded (clusters mode has too few rows).")
+def _prepare_mapping(adata_sc, adata_sp, cv_train_genes, cluster_label, mode, scale, density_prior, lambda_d, lambda_g1,
+                     lambda_g2, lambda_r, lambda_l1, lambda_l2, lambda_count, lambda_f_reg, target_count,
+                     lambda_neighborhood_g1, lambda_ct_islands, lambda_getis_ord, lambda_moran, lambda_geary,
+                     process_group=None):
+    """map_cells_to_space's preparation (mapping_utils.py:206-375): argument checks, cluster aggregation, the training
+    genes, S, G, the density prior and the spatial operators.  Returns (adata_sc -- aggregated in clusters mode --,
+    training_genes, S, G, the keywords of the mode's mapper class apart from device / random_state / precision)."""
     lambda_d = _validate_mapping_args(mode, cluster_label, lambda_g1, lambda_d, density_prior, target_count,
                                       lambda_f_reg, lambda_count)
 
@@ -187,8 +173,7 @@ def map_cells_to_space(
             d = density_prior
         if lambda_d is None or lambda_d == 0:
             lambda_d = 1
-
-    print_each = 100 if verbose else None
+    d = None if d is None else np.asarray(d, dtype=np.float32)
 
     voxel_weights, neighborhood_filter, ct_encode, spatial_weights = None, None, None, None   # :317-329
     if mode == "constrained":
@@ -205,25 +190,62 @@ def map_cells_to_space(
     if lambda_getis_ord > 0:
         spatial_weights = sw.spatial_weights(adata_sp, standardized=False, self_inclusion=True)
 
-    hyperparameters = {
-        "lambda_d": lambda_d, "lambda_g1": lambda_g1, "lambda_g2": lambda_g2, "lambda_r": lambda_r,
-        "lambda_l1": lambda_l1, "lambda_l2": lambda_l2, "d_source": d_source,
-        "lambda_neighborhood_g1": lambda_neighborhood_g1, "voxel_weights": voxel_weights,
-        "lambda_ct_islands": lambda_ct_islands, "neighborhood_filter": neighborhood_filter,
-        "ct_encode": ct_encode, "lambda_getis_ord": lambda_getis_ord, "spatial_weights": spatial_weights,
-    }
+    if mode == "constrained":                                                     # :366-375
+        mapper_kw = dict(S=S, G=G, d=d, lambda_d=lambda_d, lambda_g1=lambda_g1, lambda_g2=lambda_g2, lambda_r=lambda_r,
+                         lambda_count=lambda_count, lambda_f_reg=lambda_f_reg, target_count=target_count)
+    else:
+        mapper_kw = dict(
+            S=S, G=G, d=d, lambda_d=lambda_d, lambda_g1=lambda_g1, lambda_g2=lambda_g2, lambda_r=lambda_r,
+            lambda_l1=lambda_l1, lambda_l2=lambda_l2, d_source=d_source,
+            lambda_neighborhood_g1=lambda_neighborhood_g1, voxel_weights=voxel_weights,
+            lambda_ct_islands=lambda_ct_islands, neighborhood_filter=neighborhood_filter,
+            ct_encode=ct_encode, lambda_getis_ord=lambda_getis_ord, spatial_weights=spatial_weights)
     logging.info("Begin training with {} genes and {} density_prior in {} mode...".format(len(training_genes), d_str, mode))
+    return adata_sc, training_genes, S, G, mapper_kw
+
+
+def _make_mapper(mode, mapper_kw, **kw):
+    """The mode's mapper class, looked up on the module `mo` at call time (a test can stand another class in there)."""
+    if mode == "constrained":
+        return mo.MapperConstrained(**mapper_kw, **kw)
+    return mo.Mapper(**mapper_kw, **kw)
+
+
+def map_cells_to_space(
+    adata_sc, adata_sp, cv_train_genes=None, cluster_label=None, mode="cells", device="cuda:0",
+    learning_rate=0.1, num_epochs=1000, scale=True,
+    lambda_d=0, lambda_g1=1, lambda_g2=0, lambda_r=0, lambda_l1=0, lambda_l2=0,
+    lambda_count=1, lambda_f_reg=1, target_count=None,
+    lambda_neighborhood_g1=0, lambda_ct_islands=0, lambda_getis_ord=0, lambda_moran=0, lambda_geary=0,
+    random_state=None, verbose=True, density_prior="rna_count_based", precision="bf16x3",
+    process_group=None, gather=False, keep_on_device=False,
+):
+    """Same contract as the reference (mapping_utils.py:141-428); `device` must be CUDA.  Added keywords:
+    precision       "bf16x3" parity-grade on tensor cores (default) | "fp32" FFMA | "bf16" throughput
+    process_group   torch.distributed group, one process per GPU (mode='cells' only): every rank passes the SAME adata_sc /
+                    adata_sp; the cells are sharded in contiguous blocks (tangram_b200.shard_rows), each rank draws only its
+                    rows of the reference's M0 stream and trains them, one NCCL exchange per epoch.  Each rank returns the
+                    AnnData of ITS cells (obs = that block of adata_sc.obs; `uns['shard_rows']` = (first, last)); the
+                    per-gene scores, the history and `uns` are global and identical on every rank.  gather=True: rank 0
+                    additionally receives the full mapping (all cells) and the other ranks return None.
+    keep_on_device  keep the trained mapper (device state ~20 B per mapping element) attached to the result so that
+                    project_genes contracts on the GPU; default: release it (`adata_map.X` is all project_genes needs)."""
+    if process_group is not None and mode != "cells":
+        raise ValueError("process_group shards the cells axis: only mode='cells' can be sharded (clusters mode has too few rows).")
+    adata_sc, training_genes, S, G, mapper_kw = _prepare_mapping(
+        adata_sc, adata_sp, cv_train_genes, cluster_label, mode, scale, density_prior, lambda_d, lambda_g1, lambda_g2,
+        lambda_r, lambda_l1, lambda_l2, lambda_count, lambda_f_reg, target_count, lambda_neighborhood_g1,
+        lambda_ct_islands, lambda_getis_ord, lambda_moran, lambda_geary, process_group)
+    print_each = 100 if verbose else None
+
     F_out = None
     if mode == "constrained":                                                     # :366-389
-        mapper = mo.MapperConstrained(
-            S=S, G=G, d=None if d is None else np.asarray(d, dtype=np.float32), device=device, random_state=random_state,
-            precision=precision, lambda_d=lambda_d, lambda_g1=lambda_g1, lambda_g2=lambda_g2, lambda_r=lambda_r,
-            lambda_count=lambda_count, lambda_f_reg=lambda_f_reg, target_count=target_count)
+        mapper = _make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision)
         mapping_matrix, F_out, training_history = mapper.train(
             learning_rate=learning_rate, num_epochs=num_epochs, print_each=print_each)
     else:
-        mapper = mo.Mapper(S=S, G=G, d=None if d is None else np.asarray(d, dtype=np.float32), device=device,
-                           random_state=random_state, precision=precision, process_group=process_group, **hyperparameters)
+        mapper = _make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision,
+                              process_group=process_group)
         mapping_matrix, training_history = mapper.train(
             learning_rate=learning_rate, num_epochs=num_epochs, print_each=print_each)
 

@@ -12,6 +12,7 @@ instead of the reference's float64 upcast GEMM, and the row argmax instead of np
 no CPU path.
 """
 import ctypes
+import logging
 
 import numpy as np
 import pandas as pd
@@ -242,3 +243,203 @@ def deconvolve_cell_annotations(adata_sp, filter_cell_annotation=None):
     adata_segment.obsm["spatial"] = cells[["y", "x"]].to_numpy()
     adata_segment.uns = adata_sp.uns
     return adata_segment
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Gene cross-validation (tangram/utils.py:377-758)
+
+def compare_spatial_geneexp(adata_ge, adata_sp, adata_sc=None, genes=None):
+    """:377-463 -- per gene the cosine between the projected expression (adata_ge, as project_genes returns it) and the
+    measured one (adata_sp): a frame indexed by gene with 'score', 'is_training' (where adata_ge.var or adata_sp.var has
+    it), 'sparsity_sp' and, with adata_sc, 'sparsity_sc' and 'sparsity_diff', sorted by score (highest first).
+    `genes` (default adata_ge.uns["overlap_genes"]) picks the genes.  As in the reference, the sparsity columns are
+    written into adata_sp.var (and adata_sc.var), and the root logger is disabled."""
+    logging.getLogger().disabled = True
+    if not set(["training_genes", "overlap_genes"]).issubset(set(adata_sp.uns.keys())):
+        raise ValueError("Missing tangram parameters. Run `pp_adatas()`.")
+    if not set(["training_genes", "overlap_genes"]).issubset(set(adata_ge.uns.keys())):
+        raise ValueError("Missing tangram parameters. Use `project_genes()` to get adata_ge.")
+    assert list(adata_sp.uns["overlap_genes"]) == list(adata_ge.uns["overlap_genes"])
+    overlap_genes = adata_ge.uns["overlap_genes"] if genes is None else genes
+    mu.annotate_gene_sparsity(adata_sp)
+    X_1 = _mapping_of(adata_ge[:, overlap_genes])
+    X_2 = _mapping_of(adata_sp[:, overlap_genes])
+    cos_sims = [(v1 @ v2) / (np.linalg.norm(v1) * np.linalg.norm(v2)) for v1, v2 in zip(X_1.T, X_2.T)]
+    df_g = pd.DataFrame(cos_sims, overlap_genes, columns=["score"])
+    for adata in (adata_ge, adata_sp):
+        if "is_training" in adata.var.keys():
+            df_g["is_training"] = adata.var.is_training
+    df_g["sparsity_sp"] = adata_sp[:, overlap_genes].var.sparsity
+    if adata_sc is not None:
+        if not set(["training_genes", "overlap_genes"]).issubset(set(adata_sc.uns.keys())):
+            raise ValueError("Missing tangram parameters. Run `pp_adatas()`.")
+        assert list(adata_sc.uns["overlap_genes"]) == list(adata_sp.uns["overlap_genes"])
+        mu.annotate_gene_sparsity(adata_sc)
+        df_g = df_g.merge(pd.DataFrame(adata_sc[:, overlap_genes].var["sparsity"]), left_index=True, right_index=True)
+        df_g.rename({"sparsity": "sparsity_sc"}, inplace=True, axis="columns")
+        df_g["sparsity_diff"] = df_g["sparsity_sp"] - df_g["sparsity_sc"]
+    if genes is not None:
+        df_g = df_g.loc[genes]
+    return df_g.sort_values(by="score", ascending=False)
+
+
+def _cv_splits(n, cv_mode):
+    """(train positions, test positions) of sklearn's LeaveOneOut ('loo') or unshuffled KFold(n_splits=10) ('10fold')
+    over n items: KFold's first n % 10 folds hold one item more than the others."""
+    if cv_mode == "loo":
+        if n < 2:
+            raise ValueError(f"Cannot perform LeaveOneOut with n_samples={n}.")
+        sizes = [1] * n
+    elif cv_mode == "10fold":
+        if n < 10:
+            raise ValueError(f"Cannot have number of splits n_splits=10 greater than the number of samples: n_samples={n}.")
+        sizes = [n // 10 + (1 if f < n % 10 else 0) for f in range(10)]
+    else:
+        raise ValueError(f'cv_mode must be "loo" or "10fold", got {cv_mode!r}')
+    idx, start = np.arange(n), 0
+    for size in sizes:
+        test = idx[start:start + size]
+        yield np.concatenate([idx[:start], idx[start + size:]]), test
+        start += size
+
+
+def cv_data_gen(adata_sc, adata_sp, cv_mode="loo"):
+    """:466-500 -- yields (train_genes, test_genes) lists over the training genes of pp_adatas: leave-one-out
+    (cv_mode="loo") or ten contiguous folds ("10fold"), as sklearn's LeaveOneOut / KFold(10) split them.  An unknown
+    cv_mode raises ValueError (the reference fails there with UnboundLocalError)."""
+    if "training_genes" not in adata_sc.uns.keys():
+        raise ValueError("Missing tangram parameters. Run `pp_adatas()`.")
+    if "training_genes" not in adata_sp.uns.keys():
+        raise ValueError("Missing tangram parameters. Run `pp_adatas()`.")
+    if not list(adata_sp.uns["training_genes"]) == list(adata_sc.uns["training_genes"]):
+        raise ValueError("Unmatched training_genes field in two Anndatas. Run `pp_adatas()`.")
+    genes_array = np.array(adata_sp.uns["training_genes"])
+    for train_idx, test_idx in _cv_splits(len(genes_array), cv_mode):
+        yield list(genes_array[train_idx]), list(genes_array[test_idx])
+
+
+def cross_val(adata_sc, adata_sp, cluster_label=None, mode="clusters", scale=True, lambda_d=0, lambda_g1=1, lambda_g2=0,
+              lambda_r=0, lambda_count=1, lambda_f_reg=1, target_count=None, num_epochs=1000, device="cuda:0",
+              learning_rate=0.1, cv_mode="loo", return_gene_pred=False, density_prior=None, random_state=None,
+              verbose=False, *, precision="bf16x3"):
+    """:503-668 -- gene cross-validation: for each fold of cv_data_gen, a mapping trained on the fold's training genes
+    (as map_cells_to_space(cv_train_genes=...) trains it) scores the held-out genes with compare_spatial_geneexp.
+    Returns cv_dict {"avg_test_score", "avg_train_score"} (nanmean over the folds; a fold's train score is the last
+    main_loss of its history), and with cv_mode="loo" and return_gene_pred=True also adata_ge_cv (spots x test genes:
+    each gene's projection from the fold that held it out; var "test_score") and test_gene_df (the test genes' rows of
+    compare_spatial_geneexp).  verbose prints each fold's scores.
+
+    All folds train on one device handle built once over all training genes: each fold restricts the loss to its
+    training genes (a handle masked to S[:, train] computes what a handle built on those columns computes), redraws
+    the initial mapping from numpy's global generator exactly as a fresh mapper would (reseeded when random_state is
+    truthy), trains num_epochs with a fresh Adam, and projects only the test genes on the device.  `precision` as in
+    map_cells_to_space."""
+    logging.getLogger().disabled = True
+    logging.getLogger("anndata").disabled = True
+    folds = list(cv_data_gen(adata_sc, adata_sp, cv_mode))
+    adata_ref, genes, S, _, mapper_kw = mu._prepare_mapping(
+        adata_sc, adata_sp, None, cluster_label, mode, scale, density_prior, lambda_d, lambda_g1, lambda_g2, lambda_r,
+        0, 0, lambda_count, lambda_f_reg, target_count, 0, 0, 0, 0, 0)
+    if mode != "clusters":
+        adata_ref = adata_sc
+    column = {g: k for k, g in enumerate(genes)}
+    test_genes_list, test_pred_list, test_score_list, train_score_list, test_df_list = [], [], [], [], []
+    mapper = mu._make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision)
+    try:
+        for fold, (train_genes, test_genes) in enumerate(folds):
+            if fold > 0:                      # the constructor made the first fold's draw
+                mapper._draw_initial_mapping()
+            active = np.zeros(len(genes), dtype=bool)
+            active[[column[g] for g in train_genes]] = True
+            mapper._set_loss_genes(active)
+            mapper._fit(num_epochs, float(learning_rate), None, False, fetch=False)
+            train_score = float(mapper.history_matrix[-1, 1])                    # main_loss (:622)
+            pred = mapper.project(S[:, [column[g] for g in test_genes]])          # (spots, test genes)
+            var = pd.DataFrame({"is_training": np.zeros(len(test_genes), dtype=bool)}, index=test_genes)
+            adata_ge = make_adata(X=pred, obs=adata_sp.obs.copy(), var=var, uns=adata_ref.uns)
+            df_g = compare_spatial_geneexp(adata_ge, adata_sp, adata_ref, test_genes)
+            test_score = df_g.loc[test_genes]["score"].mean()
+            if cv_mode == "loo" and return_gene_pred:
+                test_pred_list.append(pred.T)
+            test_genes_list.append(test_genes)
+            test_score_list.append(test_score)
+            train_score_list.append(train_score)
+            test_df_list.append(df_g)
+            if verbose:
+                print("cv set: {}----train score: {:.3f}----test score: {:.3f}".format(fold + 1, train_score, test_score))
+    finally:
+        mapper.release()
+
+    avg_test_score = np.nanmean(test_score_list)
+    avg_train_score = np.nanmean(train_score_list)
+    cv_dict = {"avg_test_score": avg_test_score, "avg_train_score": avg_train_score}
+    print("cv avg test score {:.3f}".format(avg_test_score))
+    print("cv avg train score {:.3f}".format(avg_train_score))
+    if cv_mode == "loo" and return_gene_pred:
+        test_gene_df = pd.concat(test_df_list, axis=0)
+        adata_ge_cv = make_adata(
+            X=np.squeeze(test_pred_list).T, obs=adata_sp.obs.copy(),
+            var=pd.DataFrame(test_score_list, columns=["test_score"], index=np.squeeze(test_genes_list)))
+        return cv_dict, adata_ge_cv, test_gene_df
+    return cv_dict
+
+
+def _auc(x, y):
+    """sklearn.metrics.auc: the trapezoidal area under (x, y), x monotonic in either direction."""
+    x, y = np.asarray(x).reshape(-1), np.asarray(y).reshape(-1)
+    if x.shape[0] != y.shape[0]:
+        raise ValueError(f"Found input variables with inconsistent numbers of samples: [{x.shape[0]}, {y.shape[0]}]")
+    if x.shape[0] < 2:
+        raise ValueError(f"At least 2 points are needed to compute area under curve, but x.shape = {x.shape[0]}")
+    direction = 1
+    dx = np.diff(x)
+    if np.any(dx < 0):
+        if np.all(dx <= 0):
+            direction = -1
+        else:
+            raise ValueError("x is neither increasing nor decreasing : {}.".format(x))
+    trapezoid = getattr(np, "trapezoid", None) or np.trapz
+    return direction * trapezoid(y, x)
+
+
+def eval_metric(df_all_genes, test_genes=None):
+    """:671-758 -- metrics of a compare_spatial_geneexp frame over `test_genes` (default: the genes whose is_training is
+    False): ({"avg_test_score", "avg_train_score", "sp_sparsity_score", "auc_score"}, ((fitted xs, ys), (raw test scores,
+    raw sparsity_sp))).  auc_score is the area under the quadratic fit of sparsity against score, restricted to the unit
+    square, exactly as the reference computes it."""
+    if test_genes is not None:
+        if not set(test_genes).issubset(set(df_all_genes.index.values)):
+            raise ValueError("the input of test_genes should be subset of genes of input dataframe")
+        test_genes = np.unique(test_genes)
+    else:
+        test_genes = list(set(df_all_genes[df_all_genes["is_training"] == False].index.values))  # noqa: E712
+    test_gene_scores = df_all_genes.loc[test_genes]["score"]
+    test_gene_sparsity_sp = df_all_genes.loc[test_genes]["sparsity_sp"]
+    test_score_avg = test_gene_scores.mean()
+    train_score_avg = df_all_genes[df_all_genes["is_training"] == True]["score"].mean()  # noqa: E712
+    test_score_sps_sp_g2 = np.sum((test_gene_scores * (1 - test_gene_sparsity_sp)) / (1 - test_gene_sparsity_sp).sum())
+
+    xs = list(test_gene_scores)
+    ys = list(test_gene_sparsity_sp)
+    pol = np.poly1d(np.polyfit(xs, ys, 2))
+    pol_xs = np.linspace(0, 1, 10)
+    pol_ys = [pol(x) for x in pol_xs]
+    if pol_ys[0] > 1:
+        pol_ys[0] = 1
+    root = None                                   # the first real root in [0, 1] adds the point (root, 0)
+    for r in pol.r:
+        if np.isreal(r) and r <= 1 and r >= 0:
+            root = r
+            break
+    if root is not None:
+        pol_xs = np.append(pol_xs, root)
+        pol_ys = np.append(pol_ys, 0)
+    # the reference's np.append(pol_xs, 1) / np.append(pol_ys, pol(1)) discard their results: no point (1, pol(1))
+    del_idx = [i for i in range(len(pol_xs)) if pol_xs[i] < 0 or pol_ys[i] < 0 or pol_xs[i] > 1 or pol_ys[i] > 1]
+    # points are dropped by the position of their value's FIRST occurrence, as the reference's list.index does
+    pol_xs = [x for x in pol_xs if list(pol_xs).index(x) not in del_idx]
+    pol_ys = [y for y in pol_ys if list(pol_ys).index(y) not in del_idx]
+    auc_test_score = np.real(_auc(pol_xs, pol_ys))
+    metric_dict = {"avg_test_score": test_score_avg, "avg_train_score": train_score_avg,
+                   "sp_sparsity_score": test_score_sps_sp_g2, "auc_score": auc_test_score}
+    return metric_dict, ((pol_xs, pol_ys), (xs, ys))
