@@ -265,6 +265,28 @@ TGB200_API int tgb200_annotate(const float* map, int64_t rows, int64_t cols, int
                                const int32_t* labels_host, int32_t n_labels,
                                double* sums_out, int32_t* argmax_out, int32_t device, void* stream);
 
+/* project_genes' GEMM from any mapping (tangram/utils.py:366-368: `adata_map.X.T @ adata_sc.X` on the host, after densifying
+ * a sparse adata_sc.X), with no handle: out[j, k] = sum_i map[i, j] X[i, k].
+ *   map      rows x cols probabilities, row-major f32, leading dimension ld >= cols (host or device)
+ *   X        dense rows x n_genes, row-major f32, leading dimension x_ld >= n_genes (host or device), or NULL for CSR:
+ *   indptr   rows + 1 int64 offsets from 0 to nnz, non-decreasing (host or device)
+ *   indices  nnz int32 columns in [0, n_genes), strictly increasing within a row (host or device)
+ *   data     nnz f32 values (host or device)
+ *   out      cols x n_genes f32 (host or device)
+ *   block_rows  cells staged per block, a multiple of 2048; 0 = about an eighth of the cells, less if free memory needs it
+ * Arithmetic as tgb200_project: three bf16 planes per operand, six partial products on the tensor cores; accumulation
+ * chains of 512 cells (tgb200_project: at most 2048), added in cell order in fp32 (round-to-nearest); no atomics.  The result does not depend on how
+ * the data is staged: dense or CSR X, host or device pointers and any block size give identical bits.
+ * Cell blocks of the mapping and X are double-buffered (the copies of block b + 1 run on a second stream while block b
+ * contracts); device memory is out plus two blocks of staging, whatever `rows` is.  A CSR block is turned into the bf16
+ * planes directly, one warp per row.  TGB200_ERR_INVALID for bad shapes, a malformed indptr, a column index outside
+ * [0, n_genes) or out of order (such entries are skipped, never written), or when free device memory cannot hold out and
+ * one block of 2048 cells (the message gives the sizes); TGB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).
+ * Synchronous on `stream`. */
+TGB200_API int tgb200_project_map(const float* map, int64_t rows, int64_t cols, int64_t ld, const float* X, int64_t x_ld,
+                                  const int64_t* indptr, const int32_t* indices, const float* data, int64_t nnz,
+                                  int64_t n_genes, float* out, int64_t block_rows, int32_t device, void* stream);
+
 /* Checkpoint / resume (the reference stubs this: `raise NotImplemented`, :151-153).
  * Any pointer may be NULL to skip it.  M, m, v: n_cells x n_voxels f32, host or device. */
 TGB200_API int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream);

@@ -3,6 +3,7 @@
     import tangram_b200 as tg
     tg.pp_adatas(ad_sc, ad_sp); ad_map = tg.map_cells_to_space(ad_sc, ad_sp, device="cuda:0")
     ad_ge = tg.project_genes(ad_map, ad_sc)
+    X_space = tg.project(ad_map.X, ad_sc.X)          # mapping^T X on the GPU from any mapping; sparse X stays sparse
     tg.project_cell_annotations(ad_map, ad_sp, annotation="cell_type")   # ad_sp.obsm["tangram_ct_pred"]
     cv_dict = tg.cross_val(ad_sc, ad_sp, cluster_label="cell_type", cv_mode="10fold")   # gene cross-validation
     metrics = tg.train_multiple_Mapper(config, data)     # the tuner's trial: five run-to-run agreement metrics
@@ -12,7 +13,7 @@ from .sharded import shard_rows  # noqa: F401
 from .mapping_utils import (  # noqa: F401
     adata_to_cluster_expression, map_cells_to_space, pp_adatas, annotate_gene_sparsity, one_hot_encoding)
 from .utils import (  # noqa: F401
-    project_genes, annotate, project_cell_annotations, cell_type_mapping, count_cell_annotations, create_segment_cell_df,
+    project_genes, project, annotate, project_cell_annotations, cell_type_mapping, count_cell_annotations, create_segment_cell_df,
     deconvolve_cell_annotations, df_to_cell_types, cross_val, cv_data_gen, compare_spatial_geneexp, eval_metric)
 from . import mapping_parameter_tuning  # noqa: F401
 from .mapping_parameter_tuning import train_multiple_Mapper  # noqa: F401

@@ -97,6 +97,8 @@ SIGNATURES = {
                                         _P, _P, _P, ctypes.c_int32, _P]),
     "tgb200_annotate": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int32,
                                        _P, _P, ctypes.c_int32, _P]),
+    "tgb200_project_map": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int64,
+                                          _P, _P, _P, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int64, ctypes.c_int32, _P]),
     "tgb200_get_state":(ctypes.c_int, [_P, _P, _P, _P, _I64, _P]),
     "tgb200_set_state": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int64, _P]),
     "tgb200_kernel_launches": (ctypes.c_int, [_P, _I64]),

@@ -648,14 +648,15 @@ static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs
   return tc_check_launch("tc_gemm_fwd", err, n);
 }
 // cells [row0, row1) only (row0 a multiple of 64): `out` = or += this chunk's partial sum -- the host pipelines cell chunks
-// behind the streaming Adam kernel; the chunks run one after the other on one stream, so the summation order is fixed
-static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, float* out, int accumulate, int row0, int row1, int V, int Ke,
-                                         cudaStream_t s, char* err, size_t n) {
+// behind the streaming Adam kernel (and tgb200_project_map adds its 512-cell chains); the chunks run one after the other
+// on one stream, so the summation order is fixed
+static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int accumulate, int row0, int row1,
+                                         int V, int Ke, cudaStream_t s, char* err, size_t n) {
   auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
   if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, accumulate};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
-  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, 1, row1, (int)round_up(row1 - row0, TC_BK), tm, tn,
+  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, row1, (int)round_up(row1 - row0, TC_BK), tm, tn,
                                                                     1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
   return tc_check_launch("tc_gemm_fwd", err, n);
 }

@@ -21,6 +21,7 @@
 #include "legacy_rng.cuh"
 #include "agreement.cuh"
 #include "annotate.cuh"
+#include "project.cuh"
 #include "mt19937_jump.h"
 #include "nccl_dl.h"
 
@@ -1027,7 +1028,7 @@ static int forward_chunk(tgb200_mapper* h, cudaStream_t s, int c, int fresh, con
   LAUNCH_CHECK("scale_rows");
   if (h->nchunks > 1) {
     // chunk 0 overwrites the exchange buffer, the others add to it (same stream, fixed order): no partial planes to sum
-    CKS(tc_forward_launch_rows(h->tc, h->plan_fwd, h->Y.p, c > 0 ? 1 : 0, r0, r1, h->V, h->Ke, s, g_err, sizeof(g_err)));
+    CKS(tc_forward_launch_rows(h->tc, h->plan_fwd, 1, h->Y.p, c > 0 ? 1 : 0, r0, r1, h->V, h->Ke, s, g_err, sizeof(g_err)));
     mark(h, s, "tc_gemm_fwd");
   }
   return TGB200_OK;
@@ -2020,6 +2021,175 @@ extern "C" int tgb200_annotate(const float* map, int64_t rows, int64_t cols, int
     }
     CK(cudaMemcpyAsync(argmax_out, d_argmax.p, sizeof(int32_t) * rows, cudaMemcpyDefault, s));
   }
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+// Projection of X through any mapping (tangram/utils.py:366-368), streamed over cell blocks.
+namespace {
+constexpr int64_t kProjUnit = 2048;      // blocks are multiples of 2048 cells
+// cells per accumulation chain: a truncating tensor-core chain of c same-sign terms drifts by up to c / 8 u (DESIGN 2);
+// 512 keeps all-positive data (probabilities times expression) well inside 3e-6 rel-Frobenius.  It divides kProjUnit,
+// so the chains, and the order they are added in, do not depend on the block size.
+constexpr int64_t kProjChain = 512;
+constexpr int64_t kProjBlocks = 8;       // default: about this many blocks, so the copies of one hide under the others
+struct CopyStream {                      // the second stream and its events, released on every return path
+  cudaStream_t s = nullptr;
+  cudaEvent_t start = nullptr, copied[2] = {}, freed[2] = {};
+  ~CopyStream() {
+    for (cudaEvent_t e : {start, copied[0], copied[1], freed[0], freed[1]}) if (e) cudaEventDestroy(e);
+    if (s) cudaStreamDestroy(s);
+  }
+};
+}  // namespace
+
+extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, int64_t ld, const float* X, int64_t x_ld,
+                                  const int64_t* indptr, const int32_t* indices, const float* data, int64_t nnz,
+                                  int64_t n_genes, float* out, int64_t block_rows, int32_t device, void* stream) {
+  if (!map || !out) return fail(TGB200_ERR_INVALID, "null argument");
+  const bool csr = X == nullptr;
+  if (csr == (indptr == nullptr)) return fail(TGB200_ERR_INVALID, "give exactly one of X (dense) and indptr (CSR)");
+  if (rows <= 0 || cols <= 0 || ld < cols || n_genes <= 0 || rows > INT32_MAX || cols > INT32_MAX || n_genes > INT32_MAX - 64 ||
+      (!csr && x_ld < n_genes))
+    return fail(TGB200_ERR_INVALID, "bad shape rows=%lld cols=%lld ld=%lld n_genes=%lld x_ld=%lld", (long long)rows,
+                (long long)cols, (long long)ld, (long long)n_genes, (long long)x_ld);
+  if (csr && (nnz < 0 || (nnz > 0 && (!indices || !data))))
+    return fail(TGB200_ERR_INVALID, "CSR with nnz=%lld needs indices and data", (long long)nnz);
+  if (block_rows < 0 || block_rows % kProjUnit)
+    return fail(TGB200_ERR_INVALID, "block_rows=%lld is not a multiple of %lld", (long long)block_rows, (long long)kProjUnit);
+  int n_sms = 0;
+  CKS(use_sm90_device(device, &n_sms));
+  cudaStream_t s = (cudaStream_t)stream;
+  // the row pointers are read on the host: every block's entry range is then known to lie inside [0, nnz)
+  std::vector<int64_t> ip;
+  if (csr) {
+    ip.resize(rows + 1);
+    CK(cudaMemcpyAsync(ip.data(), indptr, sizeof(int64_t) * (rows + 1), cudaMemcpyDefault, s));
+    CK(cudaStreamSynchronize(s));
+    if (ip[0] != 0 || ip[rows] != nnz)
+      return fail(TGB200_ERR_INVALID, "CSR indptr runs from %lld to %lld, expected 0 to nnz=%lld", (long long)ip[0],
+                  (long long)ip[rows], (long long)nnz);
+    for (int64_t r = 0; r < rows; ++r)
+      if (ip[r + 1] < ip[r]) return fail(TGB200_ERR_INVALID, "CSR indptr decreases at row %lld", (long long)r);
+  }
+  const int64_t ldm = round_up(cols, 64), ldx = round_up(n_genes, 64), cap = round_up(rows, kProjUnit);
+  auto max_nnz = [&](int64_t B) {
+    int64_t m = 0;
+    for (int64_t r0 = 0; csr && r0 < rows; r0 += B) m = std::max(m, ip[std::min(rows, r0 + B)] - ip[r0]);
+    return m;
+  };
+  // out, then per block: the mapping twice in fp32 (copy target, double-buffered) and once in three bf16 planes, X in three
+  // planes and, double-buffered, in fp32 (dense) or as the block's CSR entries
+  auto need = [&](int64_t B) {
+    double b = 4.0 * cols * ldx + 2 * 4.0 * B * ldm + 6.0 * B * ldm + 6.0 * B * ldx;
+    return b + (csr ? 2 * (8.0 * max_nnz(B) + 8.0 * (B + 1)) : 2 * 4.0 * B * ldx);
+  };
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const double avail = (double)free_b - 256.0 * (1 << 20);    // headroom for the launches' own allocations
+  int64_t B = block_rows > 0 ? std::min(block_rows, cap)
+                             : std::min(cap, std::max(kProjUnit, round_up(ceil_div(rows, kProjBlocks), kProjUnit)));
+  while (block_rows == 0 && B > kProjUnit && need(B) > avail) B -= kProjUnit;
+  if (need(B) > avail)
+    return fail(TGB200_ERR_INVALID, "projecting a %lld x %lld mapping onto %lld genes needs %.2f GiB on device %d in blocks of "
+                "%lld cells (%.2f GiB of it for the result); %.2f GiB are free", (long long)rows, (long long)cols,
+                (long long)n_genes, need(B) / 1073741824.0, device, (long long)B, 4.0 * cols * ldx / 1073741824.0,
+                free_b / 1073741824.0);
+
+  DevBuf<float> O, Mf[2], Xf[2], D[2];
+  DevBuf<__nv_bfloat16> Mp, Xp;
+  DevBuf<int64_t> P[2];
+  DevBuf<int> I[2], bad;
+  CKS(O.alloc((size_t)cols * ldx, false));
+  CKS(Mp.alloc((size_t)3 * B * ldm, false)); CKS(Xp.alloc((size_t)3 * B * ldx, false));
+  CKS(bad.alloc(1, false));
+  const int64_t block_nnz = max_nnz(B);
+  for (int k = 0; k < 2; ++k) {
+    CKS(Mf[k].alloc((size_t)B * ldm, false));
+    if (csr) {
+      CKS(P[k].alloc(B + 1, false)); CKS(I[k].alloc(std::max<int64_t>(block_nnz, 1), false));
+      CKS(D[k].alloc(std::max<int64_t>(block_nnz, 1), false));
+    } else {
+      CKS(Xf[k].alloc((size_t)B * ldx, false));
+    }
+  }
+  // zeroed on `stream` before cp.start is recorded, so the copy stream's first writes come after them whatever kind of
+  // stream the caller passed: the flag starts at 0 and the staging's pad columns stay finite
+  CK(cudaMemsetAsync(bad.p, 0, sizeof(int), s));
+  for (int k = 0; k < 2; ++k) {
+    CK(cudaMemsetAsync(Mf[k].p, 0, sizeof(float) * Mf[k].n, s));
+    if (!csr) CK(cudaMemsetAsync(Xf[k].p, 0, sizeof(float) * Xf[k].n, s));
+  }
+  TcContext tc;
+  if (tc_init(tc, g_err, sizeof(g_err))) return TGB200_ERR_CUDA;
+  TcPlan pl;                                                   // the planes never move within the call
+  if (tc_forward_plan(tc, pl, Mp.p, (size_t)B * ldm, Xp.p, (size_t)B * ldx, 3, (int)B, (int)cols, (int)ldx, (int)ldm, g_err,
+                      sizeof(g_err)))
+    return TGB200_ERR_CUDA;
+  CopyStream cp;
+  CK(cudaStreamCreateWithFlags(&cp.s, cudaStreamNonBlocking));
+  for (cudaEvent_t* e : {&cp.start, &cp.copied[0], &cp.copied[1], &cp.freed[0], &cp.freed[1]})
+    CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  CK(cudaEventRecord(cp.start, s));                            // inputs written on `stream` before the call
+  CK(cudaStreamWaitEvent(cp.s, cp.start, 0));
+
+  const int64_t n_blocks = ceil_div(rows, B);
+  // block b's inputs into slot b % 2 on the copy stream, once the contraction stream has consumed block b - 2 from it
+  auto stage = [&](int64_t b) -> int {
+    const int k = (int)(b & 1);
+    const int64_t r0 = b * B, nb = std::min(B, rows - r0), nb64 = round_up(nb, 64);
+    if (b >= 2) CK(cudaStreamWaitEvent(cp.s, cp.freed[k], 0));
+    if (nb < nb64) {                                           // the last k-block reads up to nb64 rows: zero the tail
+      CK(cudaMemsetAsync(Mf[k].p + nb * ldm, 0, sizeof(float) * (nb64 - nb) * ldm, cp.s));
+      if (!csr) CK(cudaMemsetAsync(Xf[k].p + nb * ldx, 0, sizeof(float) * (nb64 - nb) * ldx, cp.s));
+    }
+    CK(cudaMemcpy2DAsync(Mf[k].p, sizeof(float) * ldm, map + r0 * ld, sizeof(float) * ld, sizeof(float) * cols, nb,
+                         cudaMemcpyDefault, cp.s));
+    if (csr) {
+      const int64_t e0 = ip[r0], ne = ip[r0 + nb] - e0;
+      CK(cudaMemcpyAsync(P[k].p, ip.data() + r0, sizeof(int64_t) * (nb + 1), cudaMemcpyHostToDevice, cp.s));
+      if (ne > 0) {
+        CK(cudaMemcpyAsync(I[k].p, indices + e0, sizeof(int32_t) * ne, cudaMemcpyDefault, cp.s));
+        CK(cudaMemcpyAsync(D[k].p, data + e0, sizeof(float) * ne, cudaMemcpyDefault, cp.s));
+      }
+    } else {
+      CK(cudaMemcpy2DAsync(Xf[k].p, sizeof(float) * ldx, X + r0 * x_ld, sizeof(float) * x_ld, sizeof(float) * n_genes, nb,
+                           cudaMemcpyDefault, cp.s));
+    }
+    CK(cudaEventRecord(cp.copied[k], cp.s));
+    return TGB200_OK;
+  };
+  CKS(stage(0));
+  for (int64_t b = 0; b < n_blocks; ++b) {
+    const int k = (int)(b & 1);
+    const int64_t r0 = b * B, nb = std::min(B, rows - r0), nb64 = round_up(nb, 64);
+    CK(cudaStreamWaitEvent(s, cp.copied[k], 0));
+    const long long m4 = nb64 * ldm / 4;
+    k_split3<<<(unsigned)ceil_div(m4, 256), 256, 0, s>>>(Mf[k].p, Split3{Mp.p, (size_t)B * ldm}, m4);
+    CK(cudaGetLastError());
+    if (csr) {
+      const CsrSplitArgs a{P[k].p, I[k].p, D[k].p, (int)nb, (int)nb64, (int)n_genes, (int)ldx, Split3{Xp.p, (size_t)B * ldx}, bad.p};
+      k_csr_split3<<<(unsigned)ceil_div(nb64 * kWarp, kProjThreads), kProjThreads, 0, s>>>(a);
+    } else {
+      const long long x4 = nb64 * ldx / 4;
+      k_split3<<<(unsigned)ceil_div(x4, 256), 256, 0, s>>>(Xf[k].p, Split3{Xp.p, (size_t)B * ldx}, x4);
+    }
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(cp.freed[k], s));
+    // chains of 512 cells, added into out in cell order by the accumulating epilogue (fp32, round-to-nearest)
+    for (int64_t c0 = 0; c0 < nb; c0 += kProjChain)
+      CKS(tc_forward_launch_rows(tc, pl, 6, O.p, b > 0 || c0 > 0, (int)c0, (int)std::min(nb, c0 + kProjChain), (int)cols,
+                                 (int)ldx, s, g_err, sizeof(g_err)));
+    if (b + 1 < n_blocks) CKS(stage(b + 1));                   // after block b's launches: its copies run under them
+  }
+  int bad_host = 0;
+  CK(cudaMemcpyAsync(&bad_host, bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad_host)
+    return fail(TGB200_ERR_INVALID, "a CSR column index is outside [0, %lld) or not strictly increasing within its row",
+                (long long)n_genes);
+  CK(cudaMemcpy2DAsync(out, sizeof(float) * n_genes, O.p, sizeof(float) * ldx, sizeof(float) * n_genes, cols,
+                       cudaMemcpyDefault, s));
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
 }

@@ -25,7 +25,24 @@ from .engine import _require_device
 _ANN_CHUNK, _ANN_SLAB = 128, 1024       # rows per work item and columns per slab of tgb200_annotate
 
 
+def _dense(X):
+    return X.toarray() if hasattr(X, "toarray") else np.asarray(X)
+
+
+def _sm90_device(mapping):
+    """The device project_genes contracts on: the CUDA device of a tensor `mapping`, else torch's current one, when it is
+    an sm_90 device; None otherwise (then the host GEMM is the only path)."""
+    import torch
+    if not torch.cuda.is_available():
+        return None
+    dev = mapping.device.index if isinstance(mapping, torch.Tensor) and mapping.is_cuda else torch.cuda.current_device()
+    return dev if torch.cuda.get_device_capability(dev) == (9, 0) else None
+
+
 def project_genes(adata_map, adata_sc, cluster_label=None, scale=True):
+    """:338-374 -- adata_map.X^T adata_sc.X over every gene kept, as a (spots x genes) AnnData.  With the mapper kept on
+    the device (map_cells_to_space(keep_on_device=True)) it projects through that handle; otherwise, on an sm_90 device,
+    through `project` (a sparse adata_sc.X is streamed as CSR, never densified on the host); without one, on the host."""
     adata_sc.var.index = [g.lower() for g in adata_sc.var.index]                 # :353
     adata_sc.var_names_make_unique()                                              # :356
     keep = np.asarray((adata_sc.X != 0).sum(axis=0)).reshape(-1) >= 1             # :359
@@ -35,12 +52,13 @@ def project_genes(adata_map, adata_sc, cluster_label=None, scale=True):
         adata_sc = mu.adata_to_cluster_expression(adata_sc, cluster_label, scale=scale)
     if not adata_map.obs.index.equals(adata_sc.obs.index):
         raise ValueError("The two AnnDatas need to have same `obs` index.")
-    X = adata_sc.X.toarray() if hasattr(adata_sc.X, "toarray") else np.asarray(adata_sc.X)
     mapper = getattr(adata_map, "_tgb200_mapper", None)
-    if mapper is not None and mapper.n_cells == X.shape[0]:
-        X_space = mapper.project(X)               # softmax(M)^T X on the device (:368 is a host GEMM)
+    if mapper is not None and mapper.n_cells == adata_sc.X.shape[0]:
+        X_space = mapper.project(_dense(adata_sc.X))   # softmax(M)^T X on the device (:368 is a host GEMM)
+    elif (dev := _sm90_device(adata_map.X)) is not None:
+        X_space = project(adata_map.X, adata_sc.X, device=f"cuda:{dev}")
     else:
-        X_space = np.asarray(adata_map.X).T @ X
+        X_space = np.asarray(adata_map.X).T @ _dense(adata_sc.X)
     adata_ge = make_adata(X=X_space, obs=adata_map.var, var=adata_sc.var, uns=adata_sc.uns)
     training_genes = adata_map.uns["train_genes_df"].index.values
     adata_ge.var["is_training"] = adata_ge.var.index.isin(training_genes)
@@ -101,6 +119,99 @@ def annotate(mapping, labels, n_labels, *, sums=True, argmax=False, device=None)
     _lib.check(lib.tgb200_annotate(_lib._P(X.data_ptr()), N, V, X.stride(0), _lib.ptr(lab), n_labels, _lib.ptr(out_s),
                                    _lib.ptr(out_a), dev, stream))
     return out_s, out_a
+
+
+def _canonical_csr(X, n_rows):
+    """A scipy sparse X -> (int64 indptr, int32 indices, float32 data, n_genes) of canonical CSR: columns strictly
+    increasing within each row, duplicates summed (in X's dtype, as toarray() sums them), explicit zeros kept.  The
+    structure is checked before scipy touches it; X itself is never modified (a non-canonical input is fixed on a copy)."""
+    import scipy.sparse as sp
+    csr = X.tocsr()
+    if csr.shape[0] != n_rows:
+        raise ValueError(f"X has {csr.shape[0]} rows for a mapping of {n_rows} rows")
+    n_genes = int(csr.shape[1])
+    indptr, indices = np.asarray(csr.indptr), np.asarray(csr.indices)
+    nnz = indices.shape[0]
+    if indptr.shape != (n_rows + 1,) or csr.data.shape[0] != nnz:
+        raise ValueError(f"malformed CSR: indptr of length {indptr.shape[0]} for {n_rows} rows, "
+                         f"{nnz} indices and {csr.data.shape[0]} values")
+    if indptr[0] != 0 or indptr[-1] != nnz or (np.diff(indptr) < 0).any():
+        raise ValueError(f"malformed CSR: indptr must rise from 0 to nnz={nnz}")
+    if nnz and (indices.min() < 0 or indices.max() >= n_genes):
+        raise ValueError(f"CSR column index outside [0, {n_genes})")
+    if n_genes > np.iinfo(np.int32).max - 64:
+        raise ValueError(f"{n_genes} genes: more than int32 column indices address")
+    row_start = np.zeros(nnz, dtype=bool)
+    row_start[indptr[:-1][np.diff(indptr) > 0]] = True
+    if not (row_start[1:] | (indices[1:] > indices[:-1])).all():
+        if csr is X:
+            csr = csr.copy()
+        csr = sp.csr_matrix((csr.data, csr.indices, csr.indptr), shape=csr.shape)
+        csr.sum_duplicates()                                 # sorts the columns and sums repeats, in X's dtype
+    return (np.ascontiguousarray(csr.indptr, dtype=np.int64), np.ascontiguousarray(csr.indices, dtype=np.int32),
+            np.ascontiguousarray(csr.data, dtype=np.float32), n_genes)
+
+
+def project(mapping, X, *, device=None, _block_rows=0):
+    """mapping^T X on the device (tgb200_project_map): the (V, n_genes) float32 projection of X through an (N, V) mapping,
+    fp32-grade (split-bf16 operands on the tensor cores, chains of 512 cells added in order), identical bits whether X
+    comes dense or sparse, from the host or the device.
+
+    `mapping`: a numpy array, or a CUDA tensor (a float32 one with unit column stride is read in place, row stride
+    included).  `X`: (N, n_genes) dense numpy array, CUDA tensor, or any scipy sparse matrix -- passed as canonical CSR
+    (float32 data, int32 indices, int64 indptr), never densified.  The work runs on the device of a CUDA tensor argument,
+    else on `device` (default: torch's current CUDA device), streamed over cell blocks, so neither the mapping nor X has
+    to fit in device memory; the result must.  Malformed input raises ValueError before any device work."""
+    import scipy.sparse as sp
+    import torch
+    cuda_map = isinstance(mapping, torch.Tensor) and mapping.is_cuda
+    cuda_x = isinstance(X, torch.Tensor) and X.is_cuda
+    M = mapping if cuda_map else np.asarray(mapping)
+    if M.ndim != 2:
+        raise ValueError(f"expected an (N, V) mapping, got shape {tuple(M.shape)}")
+    N, V = (int(n) for n in M.shape)
+    if sp.issparse(X):
+        csr = _canonical_csr(X, N)
+        n_genes = csr[3]
+    else:
+        if not cuda_x:
+            X = np.asarray(X)
+        if X.ndim != 2 or X.shape[0] != N:
+            raise ValueError(f"X has shape {tuple(X.shape)} for a mapping of {N} rows")
+        csr, n_genes = None, int(X.shape[1])
+    if N == 0 or V == 0 or n_genes == 0:
+        return np.zeros((V, n_genes), dtype=np.float32)
+    if cuda_map:
+        dev = M.device.index
+    elif cuda_x:
+        dev = X.device.index
+    else:
+        dev = _require_device("cuda" if device is None else device)
+    if cuda_map:
+        if M.dtype != torch.float32 or M.stride(1) != 1 or M.stride(0) < V:
+            M = M.float().contiguous()
+        m_ld = M.stride(0)
+    else:
+        M = np.ascontiguousarray(M, dtype=np.float32)
+        m_ld = V
+    if csr is not None:
+        indptr, indices, data, _ = csr
+        x_args = (None, 0, _lib.ptr(indptr), _lib.ptr(indices), _lib.ptr(data), indices.shape[0])
+    else:
+        if cuda_x:
+            if X.dtype != torch.float32 or X.stride(1) != 1 or X.stride(0) < n_genes:
+                X = X.float().contiguous()
+            x_ld = X.stride(0)
+        else:
+            X = np.ascontiguousarray(X, dtype=np.float32)
+            x_ld = n_genes
+        x_args = (_lib.ptr(X), x_ld, None, None, None, 0)
+    out = np.empty((V, n_genes), dtype=np.float32)
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    lib = _lib.load()
+    _lib.check(lib.tgb200_project_map(_lib.ptr(M), N, V, m_ld, *x_args, n_genes, _lib.ptr(out), int(_block_rows), dev,
+                                      stream))
+    return out
 
 
 def _label_columns(series):
