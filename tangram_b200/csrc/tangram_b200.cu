@@ -538,6 +538,9 @@ extern "C" int tgb200_set_graph(tgb200_mapper* h, int which, const int32_t* indp
   if (which < 0 || which > 2) return fail(TGB200_ERR_INVALID, "unknown graph id %d", which);
   const int V = h->V;
   if (indptr[0] != 0 || indptr[V] != nnz) return fail(TGB200_ERR_INVALID, "CSR indptr does not match nnz=%lld", (long long)nnz);
+  // non-decreasing from 0 to nnz: every row range lies in [0, nnz), so the transpose below counts each entry once
+  for (int j = 0; j < V; ++j)
+    if (indptr[j + 1] < indptr[j]) return fail(TGB200_ERR_INVALID, "CSR indptr decreases at row %d (%d -> %d)", j, indptr[j], indptr[j + 1]);
   for (int64_t e = 0; e < nnz; ++e)
     if (indices[e] < 0 || indices[e] >= V) return fail(TGB200_ERR_INVALID, "CSR column index %d out of range", indices[e]);
   cudaStream_t s = (cudaStream_t)stream;
