@@ -78,6 +78,12 @@ enum {
   TGB200_HIST_GETIS_ORD = 9,    /* getis_ord_sim       :257  */
   TGB200_HIST_COUNT = 10,       /* count_reg     (MapperConstrained :543) */
   TGB200_HIST_F_REG = 11,       /* lambda_f_reg  (MapperConstrained :544) */
+  /* _val_loss_fn (:311-356) of the mapping AFTER that epoch's update, on the rows tgb200_set_validation selects; NaN on the
+   * other rows while validation is on, 0 on every row while it is off */
+  TGB200_HIST_VAL_TOTAL = 12,      /* val_total_loss               :328 */
+  TGB200_HIST_VAL_GENE_SIM = 13,   /* val_gene_sim                 :326 */
+  TGB200_HIST_VAL_SPARSITY = 14,   /* val_sp_sparsity_weighted_sim :329-331 */
+  TGB200_HIST_VAL_ENTROPY = 15,    /* val_entropy                  :333 */
   TGB200_HIST_COLS = 16
 };
 
@@ -177,6 +183,20 @@ TGB200_API int tgb200_reset_adam(tgb200_mapper* h, void* stream);
  * TGB200_ERR_INVALID when no gene is active or a byte is not 0/1; TGB200_ERR_STATE between step_begin and step_end. */
 TGB200_API int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, void* stream);
 
+/* Mapper.train(val_each=every) (:398-403) without leaving the device: while `every` > 0, tgb200_run and step_begin /
+ * step_end validate epoch e -- counted from this call, from 0 -- when e % every == 0, and write _val_loss_fn's four values
+ * (:311-356: on the training matrices, over the genes of the loss mask) into history columns TGB200_HIST_VAL_* of that
+ * epoch's row.  Values are those of tgb200_validation_terms after the epoch's update: bit for bit, except the sparsity-weighted
+ * score, which is summed from the per-gene cosines in fp32 (tgb200_validation_terms recovers them from the loss
+ * coefficients on the host).  fp32 / bf16x3: the next iteration of the same tgb200_run call computes the validation from its
+ * own forward (identical: same row pass, same contraction); the last iteration of a call and constrained mode run one
+ * separate forward.  bf16 mode: one exact row pass and forward per validated epoch, which -- as after
+ * tgb200_validation_terms -- the next iteration then starts from.  No allocation and no host sync in the loop.
+ * every = 0 (the default) turns validation off.  TGB200_ERR_STATE between step_begin and step_end; every > 0 on a sharded
+ * handle is TGB200_ERR_UNSUPPORTED.  Allocates the validation's scratch (about 8 (Ke + V) bytes, more when lambda_g2 == 0) on first use;
+ * queues no work on `stream`. */
+TGB200_API int tgb200_set_validation(tgb200_mapper* h, int32_t every, void* stream);
+
 /* Constrained mode: initial filter logits F0 (n_cells, host or device; the reference draws them at :490).
  * Resets the filter's Adam state. */
 TGB200_API int tgb200_set_filter(tgb200_mapper* h, const float* F0, void* stream);
@@ -185,8 +205,8 @@ TGB200_API int tgb200_get_filter(tgb200_mapper* h, float* F_out, float* f_out, v
 
 /* ---- the hot loop ------------------------------------------------------------------ */
 
-/* Mapper.train's loop body x n_steps (:382-396): loss, backward, Adam.  No host syncs;
- * per-epoch scalars go to a device-side history buffer. */
+/* Mapper.train's loop body x n_steps (:382-396): loss, backward, Adam, and the validation of the epochs
+ * tgb200_set_validation selects (:398-403).  No host syncs; per-epoch scalars go to a device-side history buffer. */
 TGB200_API int tgb200_run(tgb200_mapper* h, int32_t n_steps, float learning_rate, void* stream);
 
 /* Cell-sharded operation (one handle per rank): step_begin computes this rank's partial
@@ -227,7 +247,8 @@ TGB200_API int tgb200_history_len(tgb200_mapper* h, int64_t* n);
 TGB200_API int tgb200_get_history(tgb200_mapper* h, int64_t first, int64_t count, float* out_host, void* stream);
 /* softmax(M, dim=1) as n_cells x n_voxels f32 (host or device).  Replaces :406-408. */
 TGB200_API int tgb200_get_mapping(tgb200_mapper* h, float* out, void* stream);
-/* _val_loss_fn (:311-356): out[4] = expression_sim, gv_sim, sp_sparsity_weighted_gv_sim, entropy (HOST). */
+/* _val_loss_fn (:311-356) of the current mapping: out[4] = expression_sim, gv_sim, sp_sparsity_weighted_gv_sim, entropy
+ * (HOST).  Synchronous, with scratch allocated per call; tgb200_set_validation computes the same inside the loop. */
 TGB200_API int tgb200_validation_terms(tgb200_mapper* h, float* out4_host, void* stream);
 /* project_genes' GEMM (tangram/utils.py:368): out (n_voxels x n_cols) = softmax(M)^T X,
  * X (n_cells x n_cols) row-major f32, host or device; fp32 accumulate. */

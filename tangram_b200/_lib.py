@@ -8,6 +8,8 @@ import numpy as np
 from . import _build
 
 HIST_COLS = 16
+# history columns of the per-epoch validation (tgb200_set_validation): total, gene_sim, sparsity-weighted, entropy
+HIST_VAL_TOTAL, HIST_VAL_GENE_SIM, HIST_VAL_SPARSITY, HIST_VAL_ENTROPY = 12, 13, 14, 15
 PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 DENSITY_NONE, DENSITY_CELLS, DENSITY_SOURCE = 0, 1, 2
 GRAPH_VOXEL_WEIGHTS, GRAPH_NEIGHBORHOOD_FILTER, GRAPH_SPATIAL_WEIGHTS = 0, 1, 2
@@ -77,6 +79,7 @@ SIGNATURES = {
     "tgb200_mt19937_jump_pow2": (ctypes.c_int, [ctypes.POINTER(MtState), ctypes.c_uint32, ctypes.POINTER(MtState)]),
     "tgb200_reset_adam": (ctypes.c_int, [_P, _P]),
     "tgb200_set_loss_genes": (ctypes.c_int, [_P, _P, _P]),
+    "tgb200_set_validation": (ctypes.c_int, [_P, ctypes.c_int32, _P]),
     "tgb200_set_filter": (ctypes.c_int, [_P, _P, _P]),
     "tgb200_get_filter": (ctypes.c_int, [_P, _P, _P, _P]),
     "tgb200_run": (ctypes.c_int, [_P, ctypes.c_int32, ctypes.c_float, _P]),

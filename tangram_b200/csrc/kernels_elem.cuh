@@ -295,6 +295,13 @@ struct LossParams {
   int constrained;
   float lam_c, lam_f, target_count;
   float* fscal;                   // [2] coefficients for k_filter_update
+  // history columns 12-15: 0 with validation off, NaN on the rows a validation does not fill (tgb200_set_validation)
+  float hist_fill;
+  // validation (_val_loss_fn, mapping_optimizer.py:311-356): k_loss_scalars<true> also writes
+  // val_out[0..3] = (gv + vg, gv, sum_k cos_k w_k / sum_k w_k, -(sum_i h_i / log V) / n_cells)
+  const float* gw;                // Ke   w_k: fraction of voxels where G[:, k] != 0 (0 outside the mask)
+  float* val_out;
+  float val_log_v, val_n;         // logf(V) as the host computes it, n_cells
 };
 
 // Y = sum over split partials; per-gene <Y,G>, |Y|^2, colsum(Y) for this row chunk;
@@ -428,13 +435,16 @@ k_ct_islands(LossParams p) {
 // cos(x,y) = <x,y> / (max(|x|,eps) max(|y|,eps))   (torch semantics, :205-206)
 // d mean_k cos / dY_jk = a_k G_jk - b_k Y_jk,  a_k = 1/(K ny ng),  b_k = cos_k/(K ny^2)
 // Under a gene mask the means run over the Kact active genes and an inactive gene's coefficients are 0.
+// kVal: the validation's instantiation (p.gw, p.val_out).  A template argument, not a test of p.gw: the training
+// instantiation compiles without the validation's arithmetic, so its results do not depend on it.
+template <bool kVal>
 __global__ void __launch_bounds__(1024)
 k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist_row) {
   __shared__ float sh[32];
   const int tid = threadIdx.x, nt = blockDim.x;
   const float nan = __int_as_float(0x7fc00000);
   const float Kf = (float)p.Kact;
-  float gv = 0.f, nb = 0.f, go = 0.f;
+  float gv = 0.f, nb = 0.f, go = 0.f, sw = 0.f, ws = 0.f;
   for (int k = tid; k < p.K; k += nt) {
     if (p.act != nullptr && p.act[k] == 0.f) {
       p.coefA[k] = 0.f; p.coefB[k] = 0.f;
@@ -450,6 +460,7 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
     const float ny = fmaxf(sqrtf(ny2), kCosEps), ng = p.ngc[k];
     const float cs = dot / (ny * ng);
     gv += cs;
+    if constexpr (kVal) { sw += cs * p.gw[k]; ws += p.gw[k]; }
     p.coefA[k] = p.lam_g1 / (Kf * ny * ng);
     p.coefB[k] = p.lam_g1 * cs / (Kf * ny * ny);
     if (p.lam_nb > 0.f) {
@@ -483,6 +494,10 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
   gv = block_reduce<false>(gv, sh) / Kf;
   nb = block_reduce<false>(nb, sh) / Kf;
   go = block_reduce<false>(go, sh) / Kf;
+  if constexpr (kVal) {
+    sw = block_reduce<false>(sw, sh);
+    ws = block_reduce<false>(ws, sh);
+  }
 
   float vg = 0.f;
   if (p.lam_g2 != 0.f) {
@@ -558,7 +573,13 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
     hist_row[9] = (p.lam_go > 0.f) ? go : nan;
     hist_row[10] = (p.constrained && p.lam_c != 0.f) ? count_abs : nan;
     hist_row[11] = (p.constrained && p.lam_f != 0.f) ? freg : nan;
-    for (int i = 12; i < 16; ++i) hist_row[i] = 0.f;
+    for (int i = 12; i < 16; ++i) hist_row[i] = p.hist_fill;
+    if constexpr (kVal) {
+      p.val_out[0] = gv + vg;                            // expression_sim (:328)
+      p.val_out[1] = gv;                                 // gv_sim (:326)
+      p.val_out[2] = sw / ws;                            // sp_sparsity_weighted_gv_sim (:329-331)
+      p.val_out[3] = -(tail[0] / p.val_log_v) / p.val_n;  // entropy (:333)
+    }
   }
 }
 
@@ -640,6 +661,17 @@ __global__ void k_col_norms(int V, int K, int Ke, const float* __restrict__ X, f
   for (int j = 0; j < V; ++j) { const float x = X[(size_t)j * Ke + k]; s2 += x * x; s += x; }
   nrm[k] = fmaxf(sqrtf(s2), kCosEps);
   if (sgn) sgn[k] = s > 0.f ? 1.f : -1.f;
+}
+// Sparsity weight of each gene (_val_loss_fn, mapping_optimizer.py:329-331): w_k = 1 - gene_sparsity_k = (voxels where
+// G[:, k] != 0) / V, from an integer count (thread per column); 0 for a gene outside the mask `act` and on pad columns.
+__global__ void k_gene_weights(int V, int K, int Ke, const float* __restrict__ G, const float* __restrict__ act,
+                               float* __restrict__ w) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= Ke) return;
+  int nz = 0;
+  if (k < K && (act == nullptr || act[k] != 0.f))
+    for (int j = 0; j < V; ++j) nz += G[(size_t)j * Ke + k] != 0.f;
+  w[k] = (float)nz / (float)V;
 }
 // per-row clamped norm over the K gene columns, or over the active ones of a gene mask `act` (warp per row)
 __global__ void k_row_norms(int V, int K, int Ke, const float* __restrict__ X, const float* __restrict__ act,

@@ -139,6 +139,14 @@ struct tgb200_mapper {
   int n_active = 0;
   DevBuf<float> gene_act;
   std::vector<float> gene_act_host;
+  DevBuf<float> gw;             // Ke: sparsity weight of each gene in the loss (k_gene_weights), for the validation
+  // per-epoch validation in the loop (tgb200_set_validation): epoch e (counted from that call) is validated when
+  // e % val_every == 0, into history columns 12-15 of its row
+  int val_every = 0;
+  int64_t val_epoch = 0;
+  int64_t val_row = -1;         // fp32 / bf16x3: the row whose validation this iteration's forward computes (see loss_stage)
+  bool val_fuse = false;        // tgb200_run, not its last iteration: a validation may wait for the next iteration's forward
+  DevBuf<float> val_coef, val_rowpart, val_hist;   // what the validation's k_loss_scalars writes beside its four values
   // history
   DevBuf<float> hist;
   int64_t hist_len = 0, hist_cap = 0;
@@ -390,6 +398,7 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   h->nredchunk = (int)ceil_div(h->Ke, kLossColsBlk);
   A(h->colpart.alloc((size_t)h->nchunk * 3 * h->Ke));
   A(h->coefA.alloc(h->Ke)); A(h->coefB.alloc(h->Ke));
+  A(h->gw.alloc(h->Ke));
   A(h->densg.alloc(h->V));
   if (cfg->lambda_g2 != 0.f) { A(h->rowpart.alloc((size_t)h->ncolchunk * h->V * 2)); A(h->coefAr.alloc(h->V)); A(h->coefBr.alloc(h->V)); }
   if (cfg->lambda_neighborhood_g1 > 0.f) {
@@ -452,6 +461,12 @@ static int fill_density_cols(tgb200_mapper* h, cudaStream_t s) {
   return refresh_bf16_operands(h, s);
 }
 
+static int gene_weights(tgb200_mapper* h, cudaStream_t s) {
+  k_gene_weights<<<(unsigned)ceil_div(h->Ke, 128), 128, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->masked ? h->gene_act.p : nullptr, h->gw.p);
+  LAUNCH_CHECK("gene_weights");
+  return TGB200_OK;
+}
+
 static int precompute_graph_constants(tgb200_mapper* h, cudaStream_t s) {
   if (!h->have_expr) return TGB200_OK;
   dim3 grid(h->V, (unsigned)ceil_div(h->Ke, 128));      // voxels on x: gridDim.y is limited to 65535
@@ -484,6 +499,7 @@ extern "C" int tgb200_set_expression(tgb200_mapper* h, const float* S, const flo
   LAUNCH_CHECK("col_norms");
   k_row_norms<<<(unsigned)ceil_div(h->V, 8), 256, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->masked ? h->gene_act.p : nullptr, h->ngr.p);
   LAUNCH_CHECK("row_norms");
+  CKS(gene_weights(h, s));
   h->have_expr = true;
   h->have_ct = false;
   CKS(fill_density_cols(h, s));
@@ -631,8 +647,29 @@ extern "C" int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, vo
   if (h->have_expr) {
     k_row_norms<<<(unsigned)ceil_div(h->V, 8), 256, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->masked ? h->gene_act.p : nullptr, h->ngr.p);
     LAUNCH_CHECK("row_norms");
+    CKS(gene_weights(h, s));
   }
   CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+// Per-epoch validation inside tgb200_run / step_end (Mapper.train(val_each=), mapping_optimizer.py:398-403).  The scratch
+// of the validation's loss scalars is allocated here, on first use, never in the loop.
+extern "C" int tgb200_set_validation(tgb200_mapper* h, int32_t every, void* stream) {
+  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
+  if (every < 0) return fail(TGB200_ERR_INVALID, "every = %d < 0", every);
+  if (h->in_step) return fail(TGB200_ERR_STATE, "set_validation inside a step");
+  if (every > 0 && h->cfg.n_cells_global != h->N) return fail(TGB200_ERR_UNSUPPORTED, "validation on a sharded handle");
+  CK(cudaSetDevice(h->cfg.device));
+  if (every > 0) {
+    if (!h->val_coef.p) CKS(h->val_coef.alloc(2 * (size_t)h->Ke + 2 * (size_t)h->V));
+    if (!h->val_hist.p) CKS(h->val_hist.alloc(TGB200_HIST_COLS));
+    if (!h->rowpart.p && !h->val_rowpart.p) CKS(h->val_rowpart.alloc((size_t)h->ncolchunk * h->V * 2));
+  }
+  (void)stream;                                      // nothing is queued: the switch takes effect at the next step
+  h->val_every = every;
+  h->val_epoch = 0;
+  h->val_row = -1;
   return TGB200_OK;
 }
 
@@ -1101,9 +1138,11 @@ extern "C" int tgb200_step_begin(tgb200_mapper* h, void* stream) {
     LAUNCH_CHECK("filter_prepare");
     CKS(refresh_bf16_operands(h, s));
   }
-  CKS(forward_pass(h, s, h->cfg.lambda_r != 0.f ? 1 : 0));
+  // a pending validation (fp32 / bf16x3) needs the row entropies of this forward; P is the same bits either way
+  const bool val = h->val_row >= 0;
+  CKS(forward_pass(h, s, h->cfg.lambda_r != 0.f || val ? 1 : 0));
   const size_t vk = (size_t)h->V * h->Ke;
-  if (needs_rowscalars(h->cfg) || h->constrained) {
+  if (needs_rowscalars(h->cfg) || h->constrained || val) {
     k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, needs_rowaux(h->cfg) ? h->rowaux.p : nullptr,
                                            h->constrained ? h->fsig.p : nullptr, h->N, h->Y.p + vk);
     LAUNCH_CHECK("row_scalar_reduce");
@@ -1155,12 +1194,39 @@ static int reduce_columns(tgb200_mapper* h, cudaStream_t s, LossParams& p, bool 
   return TGB200_OK;
 }
 
-// everything on V x Ke: reductions, scalars + history row, dY_ext
+// per-voxel partials of the row cosine: the training's own when lambda_g2 != 0, the validation's otherwise
+static float* any_rowpart(tgb200_mapper* h) { return h->rowpart.p ? h->rowpart.p : h->val_rowpart.p; }
+
+// _val_loss_fn's parameters (:311-356, as tgb200_validation_terms sets them): gene-voxel and voxel-gene cosines with weight 1,
+// no other term; the four values go to `out` (device), everything else k_loss_scalars writes goes to the validation's own
+// scratch, so the training's coefficients, dY and filter scalars are left alone
+static LossParams val_loss_params(tgb200_mapper* h, float* out) {
+  LossParams p = make_loss_params(h);
+  p.rowpart = any_rowpart(h);
+  p.coefA = h->val_coef.p; p.coefB = h->val_coef.p + h->Ke;
+  p.coefAr = h->val_coef.p + 2 * (size_t)h->Ke; p.coefBr = p.coefAr + h->V;
+  p.lam_g2 = 1.f; p.lam_g1 = 1.f; p.lam_nb = 0.f; p.lam_go = 0.f; p.lam_ct = 0.f; p.density_mode = 0;
+  p.constrained = 0;
+  p.gw = h->gw.p; p.val_out = out;
+  p.val_log_v = logf((float)h->V); p.val_n = (float)h->N;
+  return p;
+}
+
+static float* val_out_of(tgb200_mapper* h, int64_t row) {
+  return h->hist.p + (size_t)row * TGB200_HIST_COLS + TGB200_HIST_VAL_TOTAL;
+}
+
+// everything on V x Ke: reductions, scalars + history row, dY_ext.  With a validation pending (h->val_row, fp32 / bf16x3),
+// this iteration's forward is the validation's forward: the same row pass (entropies requested) and the same contraction
+// of the same mapping, so the validation only adds the row statistics and one k_loss_scalars.
 static int loss_stage(tgb200_mapper* h, cudaStream_t s, float* hist_row, bool reduce_partials_first) {
   LossParams p = make_loss_params(h);
   const tgb200_config& c = h->cfg;
+  const bool val = h->val_row >= 0;
+  if (h->val_every > 0) p.hist_fill = NAN;
+  if (val) p.rowpart = any_rowpart(h);
   dim3 rgrid(h->ncolchunk, h->nchunk);          // spatial kernels: one column per thread
-  CKS(reduce_columns(h, s, p, reduce_partials_first, c.lambda_g2 != 0.f ? 1 : 0));
+  CKS(reduce_columns(h, s, p, reduce_partials_first, c.lambda_g2 != 0.f || val ? 1 : 0));
   const dim3 fgrid2((unsigned)ceil_div(h->Ke, 128), 2);
   if (c.lambda_neighborhood_g1 > 0.f) {
     k_spatial_colstats<<<rgrid, kLossCols, 0, s>>>(h->V, h->K, h->Ke, h->W.view(), h->Y.p, h->WG.p, h->Z.p, h->colpart_nb.p, h->loss_rows);
@@ -1180,8 +1246,15 @@ static int loss_stage(tgb200_mapper* h, cudaStream_t s, float* hist_row, bool re
     k_ct_islands<<<h->n_ct_blocks, 256, 0, s>>>(p);
     LAUNCH_CHECK("ct_islands");
   }
-  k_loss_scalars<<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist_row);
+  k_loss_scalars<false><<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist_row);
   LAUNCH_CHECK("loss_scalars");
+  if (val) {
+    LossParams pv = val_loss_params(h, val_out_of(h, h->val_row));
+    pv.colpart = p.colpart;                             // the column sums reduce_columns finalised
+    k_loss_scalars<true><<<1, 1024, 0, s>>>(pv, 1, h->nredchunk, h->val_hist.p);
+    LAUNCH_CHECK("loss_scalars");
+    h->val_row = -1;
+  }
   dim3 dgrid(h->V, h->nredchunk);                       // voxels on x: gridDim.y is limited to 65535
   // fp32 dY_ext in fp32 mode (dY is not allocated otherwise), its bf16 copy or three bf16 planes on tensor cores
   k_dy_assemble<<<dgrid, kLossCols, 0, s>>>(p, h->dY.p, h->bf16 ? h->dYb.p : nullptr,
@@ -1312,6 +1385,23 @@ static int backward_fp32(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
   return TGB200_OK;
 }
 
+// The separate validation forward: what tgb200_validation_terms runs on the device, into out[0..3] (device), on `s`.
+// bf16 mode re-runs the exact row pass, so the per-row entropy exists whatever lambda_r is; P is then fresh and the next
+// iteration starts from it, exactly as after tgb200_validation_terms.
+static int validation_forward(tgb200_mapper* h, cudaStream_t s, float* out) {
+  if (h->bf16) { h->p_state = PState::stale; h->fwd_ahead = false; }
+  CKS(forward_pass(h, s, 1));
+  LossParams p = val_loss_params(h, out);
+  CKS(reduce_columns(h, s, p, true, 1));
+  k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, nullptr, nullptr, h->N, h->Y.p + (size_t)h->V * h->Ke);
+  LAUNCH_CHECK("row_scalar_reduce");
+  k_loss_scalars<true><<<1, 1024, 0, s>>>(p, 1, h->nredchunk, h->val_hist.p);
+  LAUNCH_CHECK("loss_scalars");
+  return TGB200_OK;
+}
+
+static bool val_due(const tgb200_mapper* h) { return h->val_every > 0 && h->val_epoch % h->val_every == 0; }
+
 extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
   if (!h) return fail(TGB200_ERR_INVALID, "null handle");
   cudaStream_t caller = (cudaStream_t)stream;
@@ -1327,9 +1417,25 @@ extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
   if (h->pipelined && !h->serial) CK(cudaEventRecord(h->ev_loss, s));
 
   const AdamScalars a = adam_scalars(h->cfg, h->step + 1, lr);
-  if (h->bf16) CKS(backward_bf16(h, s, update_stream(h, caller), a));
+  cudaStream_t su = update_stream(h, caller);
+  if (h->bf16) CKS(backward_bf16(h, s, su, a));
   else if (h->x3) CKS(backward_bf16x3(h, s, a));
   else CKS(backward_fp32(h, s, a));
+  // the validation of this epoch, on the mapping its update produced (mapping_optimizer.py:398-403)
+  if (val_due(h)) {
+    // fp32 / bf16x3 inside tgb200_run: the next iteration's forward serves it.  Constrained mode keeps the separate forward,
+    // which (as tgb200_validation_terms) still sees the filter of this epoch; the next forward sees the updated one.
+    if (h->val_fuse && !h->bf16 && !h->constrained) {
+      h->val_row = h->hist_len;
+    } else {
+      if (su != s) {                           // the row pass reads every row the update stream wrote
+        CK(cudaEventRecord(h->ev_join_lo, su));
+        CK(cudaStreamWaitEvent(s, h->ev_join_lo, 0));
+      }
+      CKS(validation_forward(h, s, val_out_of(h, h->hist_len)));
+    }
+  }
+  if (h->val_every > 0) h->val_epoch++;
   CKS(join_streams(h, caller));
   h->step++;
   h->hist_len++;
@@ -1445,13 +1551,17 @@ extern "C" int tgb200_run(tgb200_mapper* h, int32_t n_steps, float lr, void* str
   h->defer_join = true;                      // iterations chain through the handle's own streams and events
   int st = TGB200_OK;
   for (int i = 0; i < n_steps && st == TGB200_OK; ++i) {
-    h->prefetch_next = i + 1 < n_steps;
+    // a validated bf16 epoch runs its own row pass after the update: no next forward issued ahead of it
+    h->prefetch_next = i + 1 < n_steps && !val_due(h);
+    h->val_fuse = i + 1 < n_steps;
     st = tgb200_step_begin(h, stream);
     if (st == TGB200_OK && sharded) st = exchange_partials(h, work_stream(h, (cudaStream_t)stream));
     if (st == TGB200_OK) st = tgb200_step_end(h, lr, stream);
   }
   h->defer_join = false;
   h->prefetch_next = false;
+  h->val_fuse = false;
+  h->val_row = -1;                           // set only when an iteration follows, unless that iteration failed
   CKS(join_streams(h, (cudaStream_t)stream));
   return st;
 }
@@ -1654,7 +1764,7 @@ extern "C" int tgb200_validation_terms(tgb200_mapper* h, float* out4, void* stre
   CKS(reduce_columns(h, s, p, true, 1));
   k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, nullptr, nullptr, h->N, h->Y.p + (size_t)h->V * h->Ke);
   LAUNCH_CHECK("row_scalar_reduce");
-  k_loss_scalars<<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist.p);
+  k_loss_scalars<false><<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist.p);
   LAUNCH_CHECK("loss_scalars");
   // sparsity-weighted gene score needs per-gene cosines: recover them from coefA/coefB on the host
   std::vector<float> hrow(TGB200_HIST_COLS), cA(h->K), cB(h->K), Gh((size_t)h->V * h->Ke), tail(4);

@@ -141,6 +141,11 @@ class Engine:
             a = np.ascontiguousarray(a, dtype=np.uint8)
         _lib.check(self._lib.tgb200_set_loss_genes(self._h, _lib.ptr(a), self._s(stream)))
 
+    def set_validation(self, every, stream=None):
+        """Validate every `every`-th epoch (counted from this call; 0 = off) inside run() / step_end(): _val_loss_fn's four
+        values of the updated mapping go to history columns HIST_VAL_* of the epoch's row (tgb200_set_validation)."""
+        _lib.check(self._lib.tgb200_set_validation(self._h, int(every), self._s(stream)))
+
     def reset_adam(self, stream=None):
         _lib.check(self._lib.tgb200_reset_adam(self._h, self._s(stream)))
 

@@ -87,6 +87,20 @@ def legacy_normal_rows(random_state, n_rows, n_cols, r0, r1, block_rows=4096):
     return out
 
 
+def _validation_period(val_each):
+    """train(val_each=) -> the period of Engine.set_validation (0: no validation).  The reference validates the epochs t with
+    t % val_each == 0 (mapping_optimizer.py:398), which for a negative integer are those of -val_each; 0 fails there as
+    here."""
+    if val_each is None:
+        return 0
+    every = int(val_each)
+    if every != val_each:
+        raise ValueError(f"val_each must be an integer, got {val_each!r}")
+    if every == 0:
+        raise ZeroDivisionError("val_each = 0: integer modulo by zero")
+    return abs(every)
+
+
 def format_terms(terms):
     """The reference's print line (mapping_optimizer.py:300-307, :555-562) from (name, value) pairs; NaN terms are left
     out."""
@@ -133,10 +147,12 @@ class _EngineMapper:
         self._engine.set_loss_genes(active)
 
     def _fit(self, num_epochs, lr, print_each, resume, out=None, val_each=None, val_history=None, fetch=True):
-        """num_epochs updates (a fresh Adam unless `resume`), run in chunks that end where the reference prints or
-        validates (every `val_each` epochs, into the lists of `val_history`).  Sets history_matrix to this call's rows
-        and returns softmax(M), in `out` or a host array; with fetch=False (cross-validation scores genes with project()
-        and needs no mapping on the host) it returns None."""
+        """num_epochs updates (a fresh Adam unless `resume`), run in chunks that end where the reference prints.  With
+        `val_each`, the epochs t with t % val_each == 0 are validated on the device inside those chunks
+        (Engine.set_validation) and their four values are appended to the lists of `val_history`.  Sets history_matrix to
+        this call's rows and returns softmax(M), in `out` or a host array; with fetch=False (cross-validation scores genes
+        with project() and needs no mapping on the host) it returns None."""
+        every = _validation_period(val_each)
         if not resume:
             self._engine.reset_adam()
         first = self._engine.history_len()
@@ -145,27 +161,31 @@ class _EngineMapper:
             self._check_out(out, (self.n_cells, self.n_voxels))
         elif fetch:
             result = _ResultBuffer(_lib.load(), (self.n_cells, self.n_voxels), self._cfg.device)
+        validating = False
         try:
+            if every:
+                self._engine.set_validation(every)
+                validating = True
             t = 0
             while t < num_epochs:
-                if val_each is not None:
-                    chunk = 1
-                elif print_each:
+                if print_each:
                     chunk = min(num_epochs - t, print_each - (t % print_each))
                 else:
                     chunk = num_epochs - t
                 self._run(chunk, lr)
                 if print_each and t % print_each == 0:
                     print(format_terms(self._print_terms(self._engine.history(first + t, 1)[0])))
-                if val_each is not None and t % val_each == 0:
-                    for k, x in self.validation_terms().items():
-                        val_history[k].append(x)
                 t += chunk
             self.history_matrix = self._engine.history(first, num_epochs)
+            if every:
+                for c, key in enumerate(_VAL_KEYS, start=_lib.HIST_VAL_TOTAL):
+                    val_history[key].extend(float(x) for x in self.history_matrix[::every, c])
             if out is None and result is None:
                 return None
             return self._engine.get_mapping(out if out is not None else result.ready())
         finally:
+            if validating:
+                self._engine.set_validation(0)
             if result is not None:
                 result.release()
 
