@@ -212,7 +212,18 @@ TGB200_API int tgb200_run(tgb200_mapper* h, int32_t n_steps, float learning_rate
 /* Cell-sharded operation (one handle per rank): step_begin computes this rank's partial
  * sums; the caller all-reduces (sum) the exchange buffer across ranks (NCCL); step_end
  * finishes the iteration.  tgb200_run == step_begin + step_end when not sharded, and step_begin + NCCL all-reduce +
- * step_end on a sharded handle that has a communicator (below). */
+ * step_end on a sharded handle that has a communicator (below).
+ * A handle is sharded when n_cells_global != n_cells, in plain and in constrained mode alike (a sharded constrained handle
+ * needs target_count > 0).  The exchange buffer holds n_voxels x Ke floats of Y_ext = P^T S_ext over this rank's cells
+ * (gene columns, two density columns, cell-type columns; Ke = n_genes + 2 + n_types rounded up to 64), then an 8-float
+ * tail of row sums: [0] the per-row entropy terms (when lambda_r != 0), [1] sum |M| and [2] sum M^2 (the L1 / L2 terms),
+ * [3] sum f and [4] sum (f - f^2) (constrained mode), [5..7] zero.  In constrained mode the operand is f o S_ext
+ * (f = sigmoid(F) of this rank's cells), so the density columns already hold the f-weighted column sums, and after the sum
+ * [3] / [4] are the filter's global count and regulariser; every scalar of the filter update (lambda_d sum d / sum f,
+ * sign(sum f - target_count)) is derived from the summed buffer, so each rank updates its own F entries with global
+ * coefficients.  A constrained handle runs each iteration on one stream, so the filter update of iteration t is ordered
+ * before the filter refresh (sigmoid(F), f o S_ext) and the exchange of iteration t + 1, in tgb200_run as in a
+ * caller-driven loop. */
 TGB200_API int tgb200_step_begin(tgb200_mapper* h, void* stream);
 TGB200_API int tgb200_exchange_buffer(tgb200_mapper* h, float** device_ptr, int64_t* n_floats);
 TGB200_API int tgb200_step_end(tgb200_mapper* h, float learning_rate, void* stream);

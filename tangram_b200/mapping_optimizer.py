@@ -13,8 +13,9 @@ Additions (keyword-only, all optional):
               (legacy_rng), leaving numpy's global generator where the host draw leaves it
   process_group / shard  cell-sharded multi-GPU operation (one process per GPU): every rank passes the
               full S (/ M0) and keeps rows shard_rows(N, rank, world); with a NCCL process group the handle gets its own
-              NCCL communicator (tgb200_comm_init_rank) and the per-iteration exchange runs inside tgb200_run
-  n_cells_global         pre-sharded variant: S, M0, d_source, ct_encode already hold only this rank's rows
+              NCCL communicator (tgb200_comm_init_rank) and the per-iteration exchange runs inside tgb200_run;
+              MapperConstrained takes both with the same meaning (full S, M0 and F0 on every rank)
+  n_cells_global         pre-sharded variant (Mapper only): S, M0, d_source, ct_encode already hold only this rank's rows
   train(..., resume=True)  continue with the Adam state of the previous train() call (the reference -- and the default
               here -- builds a fresh optimizer in every train() call, mapping_optimizer.py:373)
   train(..., out=tensor)   write softmax(M) into a CUDA tensor instead of returning a host array
@@ -87,6 +88,14 @@ def legacy_normal_rows(random_state, n_rows, n_cols, r0, r1, block_rows=4096):
     return out
 
 
+def discard_normal_rows(n_rows, n_cols, block_rows=4096):
+    """Advance numpy's legacy global generator past `np.random.normal(0, 1, (n_rows, n_cols))` block by block, without
+    holding the draw: the legacy normals are consumed one at a time (the cached second value of a pair included), so the
+    generator ends in the same state as after the full draw."""
+    for b0 in range(0, n_rows, block_rows):
+        np.random.normal(0, 1, (min(block_rows, n_rows - b0), n_cols))
+
+
 def _validation_period(val_each):
     """train(val_each=) -> the period of Engine.set_validation (0: no validation).  The reference validates the epochs t with
     t % val_each == 0 (mapping_optimizer.py:398), which for a negative integer are those of -val_each; 0 fails there as
@@ -109,8 +118,40 @@ def format_terms(terms):
 
 
 class _EngineMapper:
-    """What Mapper and MapperConstrained share: an Engine (`_engine`) of n_cells x n_voxels, the epoch-chunk schedule,
-    the history fetch and the result buffer."""
+    """What Mapper and MapperConstrained share: an Engine (`_engine`) of n_cells x n_voxels, the cell-sharded setup and
+    loop, the epoch-chunk schedule, the history fetch and the result buffer."""
+
+    def _select_rows(self, n_rows_given, n_cells_global, shard, process_group, presharded=False):
+        """Cell-sharded operation: the block [r0, r1) of the n_cells_global cells this rank keeps -- all given rows for a
+        pre-sharded caller, else `shard`, else this rank's block of `process_group` (shard_rows), else every cell.  Sets
+        _rows, _pg, _sharded and returns (r0, r1)."""
+        self._pg = process_group
+        self._rows = (0, n_rows_given)
+        if presharded:
+            pass
+        elif shard is not None:
+            self._rows = (int(shard[0]), int(shard[1]))
+            if not 0 <= self._rows[0] < self._rows[1] <= n_cells_global:
+                raise ValueError(f"shard {tuple(shard)} is not a non-empty block of rows of [0, {n_cells_global})")
+        elif process_group is not None:
+            import torch.distributed as dist
+            r, w = dist.get_rank(process_group), dist.get_world_size(process_group)
+            self._rows = shard_rows(n_cells_global, r, w)
+        r0, r1 = self._rows
+        self._sharded = (r1 - r0) != n_cells_global
+        self._own_comm = False
+        return r0, r1
+
+    def _init_comm(self, pg):
+        """NCCL group: lend the handle the process-level communicator of this group (tangram_b200.sharded.nccl_comm_for_group,
+        created once) so that tgb200_run issues the per-iteration exchange itself.  Non-NCCL groups (gloo in the CPU tests)
+        keep the host-driven exchange of tangram_b200.sharded."""
+        from .sharded import nccl_comm_for_group
+        got = nccl_comm_for_group(pg, self._cfg.device)
+        if got is None:
+            return
+        self._engine.set_comm(*got)
+        self._own_comm = True
 
     def release(self):
         """Free the device state now (M, m, v, operands: ~20 bytes per mapping element) instead of at garbage collection."""
@@ -139,7 +180,19 @@ class _EngineMapper:
             raise ValueError(f"out must be a contiguous float32 tensor of shape {shape}")
 
     def _run(self, n_steps, lr):
-        self._engine.run(n_steps, lr)
+        if not self._sharded or self._own_comm:
+            self._engine.run(n_steps, lr)    # sharded: the NCCL exchange is inside
+            return
+        from types import SimpleNamespace
+
+        import torch
+        import torch.distributed as dist
+        e, stream = self._engine, torch.cuda.current_stream(self._cfg.device).cuda_stream
+        # the engine protocol of tangram_b200.sharded, issued on torch's current stream
+        on_stream = SimpleNamespace(exchange_tensor=e.exchange_tensor, step_begin=lambda: e.step_begin(stream),
+                                    step_end=lambda lr_: e.step_end(lr_, stream))
+        sharded_steps(on_stream, n_steps, lr,
+                      lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self._pg))   # the one exchange per step
 
     def _set_loss_genes(self, active):
         """Cross-validation fold: the loss sees only the genes flagged in `active` (n_genes booleans; None = all), as a
@@ -234,7 +287,6 @@ class Mapper(_EngineMapper):
         self.device = device
         self.random_state = random_state
         self.precision = precision
-        self._pg = process_group
 
         S = np.asarray(S, dtype=np.float32)
         G = np.asarray(G, dtype=np.float32)
@@ -264,17 +316,7 @@ class Mapper(_EngineMapper):
                 raise ValueError("M0 has the wrong shape")
 
         # cell-sharded operation: this rank keeps rows [r0, r1)
-        self._rows = (0, n_rows_given)
-        if presharded:
-            pass
-        elif shard is not None:
-            self._rows = (int(shard[0]), int(shard[1]))
-        elif process_group is not None:
-            import torch.distributed as dist
-            r, w = dist.get_rank(process_group), dist.get_world_size(process_group)
-            self._rows = shard_rows(n_cells_global, r, w)
-        r0, r1 = self._rows
-        self._sharded = (r1 - r0) != n_cells_global
+        r0, r1 = self._select_rows(n_rows_given, n_cells_global, shard, process_group, presharded)
         self._presharded = presharded
         if M0 is not None:
             M0 = M0[r0:r1]
@@ -314,7 +356,6 @@ class Mapper(_EngineMapper):
         else:
             e.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
             del M0
-        self._own_comm = False
         if self._sharded and process_group is not None:
             self._init_comm(process_group)
 
@@ -333,33 +374,7 @@ class Mapper(_EngineMapper):
             M0 = legacy_normal_rows(self.random_state, r1, self.n_voxels, r0, r1)
             self._engine.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
 
-    def _init_comm(self, pg):
-        """NCCL group: lend the handle the process-level communicator of this group (tangram_b200.sharded.nccl_comm_for_group,
-        created once) so that tgb200_run issues the per-iteration exchange itself.  Non-NCCL groups (gloo in the CPU tests)
-        keep the host-driven exchange of tangram_b200.sharded."""
-        from .sharded import nccl_comm_for_group
-        got = nccl_comm_for_group(pg, self._cfg.device)
-        if got is None:
-            return
-        self._engine.set_comm(*got)
-        self._own_comm = True
-
     # ------------------------------------------------------------------------------
-    def _run(self, n_steps, lr):
-        if not self._sharded or self._own_comm:
-            self._engine.run(n_steps, lr)    # sharded: the NCCL exchange is inside
-            return
-        from types import SimpleNamespace
-
-        import torch
-        import torch.distributed as dist
-        e, stream = self._engine, torch.cuda.current_stream(self._cfg.device).cuda_stream
-        # the engine protocol of tangram_b200.sharded, issued on torch's current stream
-        on_stream = SimpleNamespace(exchange_tensor=e.exchange_tensor, step_begin=lambda: e.step_begin(stream),
-                                    step_end=lambda lr_: e.step_end(lr_, stream))
-        sharded_steps(on_stream, n_steps, lr,
-                      lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self._pg))   # the one exchange per step
-
     @staticmethod
     def _print_terms(row):
         return [(name, row[c]) for c, name in _PRINT_TERMS]
@@ -408,13 +423,18 @@ class MapperConstrained(_EngineMapper):
     """Drop-in for the reference `MapperConstrained` (mapping_optimizer.py:411-639): same constructor keywords,
     `train()` returns `(mapping, F_out, training_history)` with the reference's history conventions (all values are
     strings, :630).  The per-cell filter rides the same kernels: S_f = sigmoid(F) o S is the operand of all three
-    contractions, dL/df_i is the row-dot the backward pass needs anyway, and F gets its own small Adam kernel."""
+    contractions, dL/df_i is the row-dot the backward pass needs anyway, and F gets its own small Adam kernel.
+
+    Cell-sharded like Mapper (`process_group=` / `shard=`): every rank passes the full S (and M0, F0) and keeps a block of
+    cells -- its rows of M and S, its entries of F and the Adam state of both.  The filter's global sums (sum f and the
+    f-regulariser) travel in the tail of the one exchange per epoch, so every rank sees the global loss; `train()` returns
+    this rank's mapping rows and F_out entries, with the global history."""
     _KEYS = ["total_loss", "main_loss", "vg_reg", "kl_reg", "entropy_reg", "count_reg", "lambda_f_reg"]
     _PRINT_NAMES = ["Score", "VG reg", "KL reg", "Entropy reg", "Count reg", "Lambda f reg"]          # :555-562
 
     def __init__(self, S, G, d, lambda_d=1, lambda_g1=1, lambda_g2=1, lambda_r=0, lambda_count=1, lambda_f_reg=1,
                  target_count=None, device="cuda:0", adata_map=None, random_state=None, *, precision="bf16x3",
-                 M0=None, F0=None):
+                 M0=None, F0=None, process_group=None, shard=None):
         if adata_map is not None:
             raise NotImplementedError      # the reference raises here too (:476-477)
         if precision not in _lib.PREC:
@@ -423,38 +443,52 @@ class MapperConstrained(_EngineMapper):
         S = np.ascontiguousarray(np.asarray(S, dtype=np.float32))
         G = np.ascontiguousarray(np.asarray(G, dtype=np.float32))
         n_cells, n_voxels, n_genes = S.shape[0], G.shape[0], S.shape[1]
+        if M0 is not None and F0 is not None:
+            M0, F0 = np.asarray(M0), np.asarray(F0)
+            if M0.shape != (n_cells, n_voxels) or F0.shape != (n_cells,):
+                raise ValueError("M0 / F0 have the wrong shape")
+        # cell-sharded operation: this rank keeps cells [r0, r1)
+        r0, r1 = self._select_rows(n_cells, n_cells, shard, process_group)
         self.target_density_enabled = d is not None
         e = self._engine = Engine(
-            n_cells, n_voxels, n_genes, device=_device_index(device), precision=precision,
+            r1 - r0, n_voxels, n_genes, n_cells_global=n_cells, device=_device_index(device), precision=precision,
             density_mode=_lib.DENSITY_CELLS if self.target_density_enabled else _lib.DENSITY_NONE,
             lambda_g1=lambda_g1, lambda_d=lambda_d, lambda_g2=lambda_g2, lambda_r=lambda_r, constrained=True,
             lambda_count=lambda_count, lambda_f_reg=lambda_f_reg,
             target_count=float(n_voxels if target_count is None else target_count))      # :480-483
         self._cfg = e.cfg
-        self.n_cells, self.n_voxels, self.n_genes = n_cells, n_voxels, n_genes
-        e.set_expression(S, G)
+        self.n_cells, self.n_voxels, self.n_genes = r1 - r0, n_voxels, n_genes
+        self._n_cells_global = n_cells
+        e.set_expression(np.ascontiguousarray(S[r0:r1]), G)
         if self.target_density_enabled:
             e.set_density(np.ascontiguousarray(np.asarray(d, dtype=np.float32)))
         if M0 is None or F0 is None:
             self._draw_initial_mapping()
         else:
-            e.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
-            e.set_filter(np.ascontiguousarray(F0, dtype=np.float32))
+            e.set_mapping(np.ascontiguousarray(M0[r0:r1], dtype=np.float32))
+            e.set_filter(np.ascontiguousarray(F0[r0:r1], dtype=np.float32))
+        if self._sharded and process_group is not None:
+            self._init_comm(process_group)
 
     def _draw_initial_mapping(self):
         """The reference's initial M and F (:472-493) from numpy's legacy global generator, seeded first only if
         random_state is truthy: M is drawn twice (the second draw is used), F after it.  M is drawn on the device when
-        this numpy's arithmetic matches the device formula (the first N x V normals are skipped), F on the host.  Resets
-        the Adam state (of M and F) and the history."""
-        n_cells, n_voxels = self.n_cells, self.n_voxels
+        this numpy's arithmetic matches the device formula (the first N x V normals are skipped), F on the host.  A rank
+        of a sharded run keeps rows [r0, r1) of the second draw and F[r0:r1]; on every rank the generator ends where the
+        unsharded draw leaves it.  Resets the Adam state (of M and F) and the history."""
+        n_cells, n_voxels = self._n_cells_global, self.n_voxels
+        r0, r1 = self._rows
         if self.random_state:
             np.random.seed(seed=self.random_state)
         if legacy_rng.device_draw_supported():
-            legacy_rng.draw_global(self._engine, n_cells * n_voxels, 0, 2 * n_cells * n_voxels)
+            legacy_rng.draw_global(self._engine, n_cells * n_voxels, r0, 2 * n_cells * n_voxels)
         else:
-            np.random.normal(0, 1, (n_cells, n_voxels))
-            self._engine.set_mapping(np.ascontiguousarray(np.random.normal(0, 1, (n_cells, n_voxels)), dtype=np.float32))
-        self._engine.set_filter(np.ascontiguousarray(np.random.normal(0, 1, n_cells), dtype=np.float32))
+            discard_normal_rows(n_cells, n_voxels)                       # the first draw, discarded (:475)
+            M0 = legacy_normal_rows(None, n_cells, n_voxels, r0, r1)     # rows [r0, r1) of the second (:485)
+            discard_normal_rows(n_cells - r1, n_voxels)
+            self._engine.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
+        F0 = np.random.normal(0, 1, n_cells)                                # :490
+        self._engine.set_filter(np.ascontiguousarray(F0[r0:r1], dtype=np.float32))
 
     def _print_terms(self, row):
         return zip(self._PRINT_NAMES, self._values_from_row(row))

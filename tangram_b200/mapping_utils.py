@@ -222,16 +222,19 @@ def map_cells_to_space(
 ):
     """Same contract as the reference (mapping_utils.py:141-428); `device` must be CUDA.  Added keywords:
     precision       "bf16x3" parity-grade on tensor cores (default) | "fp32" FFMA | "bf16" throughput
-    process_group   torch.distributed group, one process per GPU (mode='cells' only): every rank passes the SAME adata_sc /
-                    adata_sp; the cells are sharded in contiguous blocks (tangram_b200.shard_rows), each rank draws only its
-                    rows of the reference's M0 stream and trains them, one NCCL exchange per epoch.  Each rank returns the
-                    AnnData of ITS cells (obs = that block of adata_sc.obs; `uns['shard_rows']` = (first, last)); the
-                    per-gene scores, the history and `uns` are global and identical on every rank.  gather=True: rank 0
-                    additionally receives the full mapping (all cells) and the other ranks return None.
+    process_group   torch.distributed group, one process per GPU (mode='cells' or 'constrained'): every rank passes the SAME
+                    adata_sc / adata_sp; the cells are sharded in contiguous blocks (tangram_b200.shard_rows), each rank
+                    draws only its rows of the reference's M0 stream (and, in constrained mode, its entries of F0) and
+                    trains them, one NCCL exchange per epoch.  Each rank returns the AnnData of ITS cells (obs = that block
+                    of adata_sc.obs, with `obs['F_out']` of those cells in constrained mode; `uns['shard_rows']` =
+                    (first, last)); the per-gene scores, the history and `uns` are global and identical on every rank.
+                    gather=True: rank 0 additionally receives the full mapping (all cells, and the full F_out) and the
+                    other ranks return None.
     keep_on_device  keep the trained mapper (device state ~20 B per mapping element) attached to the result so that
                     project_genes contracts on the GPU; default: release it (`adata_map.X` is all project_genes needs)."""
-    if process_group is not None and mode != "cells":
-        raise ValueError("process_group shards the cells axis: only mode='cells' can be sharded (clusters mode has too few rows).")
+    if process_group is not None and mode == "clusters":
+        raise ValueError("process_group shards the cells axis: only mode='cells' can be sharded, and mode='constrained' "
+                         "(clusters mode has too few rows).")
     adata_sc, training_genes, S, G, mapper_kw = _prepare_mapping(
         adata_sc, adata_sp, cv_train_genes, cluster_label, mode, scale, density_prior, lambda_d, lambda_g1, lambda_g2,
         lambda_r, lambda_l1, lambda_l2, lambda_count, lambda_f_reg, target_count, lambda_neighborhood_g1,
@@ -239,13 +242,12 @@ def map_cells_to_space(
     print_each = 100 if verbose else None
 
     F_out = None
+    mapper = _make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision,
+                          process_group=process_group)
     if mode == "constrained":                                                     # :366-389
-        mapper = _make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision)
         mapping_matrix, F_out, training_history = mapper.train(
             learning_rate=learning_rate, num_epochs=num_epochs, print_each=print_each)
     else:
-        mapper = _make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision,
-                              process_group=process_group)
         mapping_matrix, training_history = mapper.train(
             learning_rate=learning_rate, num_epochs=num_epochs, print_each=print_each)
 
@@ -297,14 +299,19 @@ def map_cells_to_space(
 
 def _gather_mapping(adata_map, obs_all, pg, device):
     """Rank 0 of the group receives every rank's block of rows (gather_object of the host arrays: result packaging, once
-    per mapping) and returns the AnnData over all cells; the other ranks return None."""
+    per mapping) and returns the AnnData over all cells, with the full `obs['F_out']` in constrained mode; the other ranks
+    return None."""
     import torch.distributed as dist
     rank, world = dist.get_rank(pg), dist.get_world_size(pg)
     parts = [None] * world if rank == 0 else None
-    dist.gather_object((adata_map.uns["shard_rows"], np.asarray(adata_map.X)), parts, dst=dist.get_global_rank(pg, 0), group=pg)
+    F_out = np.asarray(adata_map.obs["F_out"]) if "F_out" in adata_map.obs.keys() else None
+    dist.gather_object((adata_map.uns["shard_rows"], np.asarray(adata_map.X), F_out), parts,
+                       dst=dist.get_global_rank(pg, 0), group=pg)
     if rank != 0:
         return None
     parts.sort(key=lambda p: p[0][0])
     full = make_adata(X=np.concatenate([p[1] for p in parts], axis=0), obs=obs_all, var=adata_map.var)
+    if F_out is not None:
+        full.obs["F_out"] = np.concatenate([p[2] for p in parts])
     full.uns.update({k: v for k, v in adata_map.uns.items() if k != "shard_rows"})
     return full
