@@ -95,7 +95,7 @@ typedef struct tgb200_config {
   int32_t n_voxels;        /* G.shape[0]                                                      */
   int32_t n_genes;         /* training genes (S.shape[1] == G.shape[1])                       */
   int32_t n_types;         /* ct_encode.shape[1], 0 if unused (:134-136)                      */
-  int64_t n_cells_global;  /* total cells over all ranks (== n_cells when not sharded)        */
+  int64_t n_cells_global;  /* total cells over all ranks (== n_cells when not sharded; <= 0: n_cells; below n_cells: invalid) */
   int32_t precision;       /* tgb200_precision                                                */
   int32_t density_mode;    /* tgb200_density_mode                                             */
   float lambda_g1;         /* :27  */

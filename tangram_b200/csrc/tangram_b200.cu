@@ -283,6 +283,9 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
     return fail(TGB200_ERR_INVALID, "unknown precision %d", cfg->precision);
   if (cfg->density_mode < 0 || cfg->density_mode > 2) return fail(TGB200_ERR_INVALID, "unknown density_mode %d", cfg->density_mode);
   if (cfg->lambda_ct_islands > 0.f && cfg->n_types <= 0) return fail(TGB200_ERR_INVALID, "lambda_ct_islands > 0 needs n_types > 0");
+  // a shard holds a block of the n_cells_global cells: fewer would count the handle as sharded and scale the density wrong
+  if (cfg->n_cells_global > 0 && cfg->n_cells_global < cfg->n_cells)
+    return fail(TGB200_ERR_INVALID, "n_cells_global=%lld < n_cells=%d", (long long)cfg->n_cells_global, cfg->n_cells);
   if (cfg->constrained) {
     if (cfg->density_mode == TGB200_DENSITY_SOURCE) return fail(TGB200_ERR_INVALID, "constrained mode has no d_source (mapping_optimizer.py:417-432)");
     if (cfg->lambda_neighborhood_g1 > 0.f || cfg->lambda_ct_islands > 0.f || cfg->lambda_getis_ord > 0.f || cfg->lambda_l1 != 0.f || cfg->lambda_l2 != 0.f)

@@ -300,6 +300,8 @@ class Mapper(_EngineMapper):
         n_rows_given, n_voxels, n_genes = S.shape[0], G.shape[0], S.shape[1]
         presharded = n_cells_global is not None
         n_cells_global = int(n_cells_global) if presharded else n_rows_given
+        if n_cells_global < n_rows_given:
+            raise ValueError(f"n_cells_global={n_cells_global} is smaller than the {n_rows_given} rows of S given")
 
         self.target_density_enabled = d is not None
         self.source_density_enabled = d_source is not None

@@ -84,7 +84,24 @@ def test_bad_config_is_rejected_before_touching_the_device():
     cfg.lambda_g1 = 0.0
     assert lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(h)) == -1
     assert b"lambda_g1 cannot be 0" in lib.tgb200_last_error()
+    # a shard of fewer global cells than its own rows would count itself sharded and divide the density by the wrong N
+    cfg.lambda_g1 = 1.0
+    for n_global in (1, 3):
+        cfg.n_cells_global = n_global
+        assert lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(h)) == -1
+        assert f"n_cells_global={n_global} < n_cells=4".encode() in lib.tgb200_last_error()
+        assert not h.value
     assert lib.tgb200_destroy(None) == 0
+
+
+def test_mapper_refuses_fewer_global_cells_than_rows_given():
+    """Mapper(n_cells_global=) below the rows of S is refused before any device work (so also without a GPU)."""
+    import numpy as np
+    from tangram_b200 import Mapper
+    S = np.ones((6, 3), dtype=np.float32)
+    G = np.ones((5, 3), dtype=np.float32)
+    with pytest.raises(ValueError, match="n_cells_global=5 is smaller than the 6 rows"):
+        Mapper(S, G, device="cuda:0", M0=np.zeros((6, 5), dtype=np.float32), n_cells_global=5)
 
 
 @pytest.mark.gpu

@@ -54,18 +54,22 @@ def _g(x):
 
 
 class Run:
-    """An Engine plus the float64 copies of its inputs."""
+    """An Engine plus the float64 copies of its inputs.  rows=(r0, r1): a cell shard holding rows [r0, r1) of the N cells'
+    inputs and initial mapping (n_cells_global = N); self.N is then the shard's row count."""
 
-    def __init__(self, precision, N, V, K, seed=0, T=0, clusters=False, lam=None):
+    def __init__(self, precision, N, V, K, seed=0, T=0, clusters=False, lam=None, rows=None):
         from tangram_b200 import _lib
         from tangram_b200.engine import Engine
         lam = dict(lam or {})
-        self.precision, self.N, self.V, self.K, self.T, self.clusters, self.lam = precision, N, V, K, T, clusters, lam
+        r0, r1 = rows or (0, N)
+        rs = slice(r0, r1)
+        self.precision, self.N, self.V, self.K, self.T, self.clusters, self.lam = precision, r1 - r0, V, K, T, clusters, lam
         inp = synthetic_inputs(N, V, K, seed=seed, n_types=T, clusters=clusters)
-        self.e = Engine(N, V, K, n_types=T, precision=precision, lambda_d=1.0,
+        self.e = Engine(r1 - r0, V, K, n_types=T, n_cells_global=N, precision=precision, lambda_d=1.0,
                         density_mode=_lib.DENSITY_SOURCE if clusters else _lib.DENSITY_CELLS, **lam)
-        self.e.set_expression(inp["S"], inp["G"])
-        self.e.set_density(inp["d"], inp.get("d_source"))
+        self.e.set_expression(np.ascontiguousarray(inp["S"][rs]), inp["G"])
+        d_source = inp.get("d_source")
+        self.e.set_density(inp["d"], None if d_source is None else np.ascontiguousarray(d_source[rs]))
         self.graphs = {}
         if lam.get("lambda_neighborhood_g1") or lam.get("lambda_ct_islands") or lam.get("lambda_getis_ord"):
             conn, dist = grid_graph(V)
@@ -74,11 +78,11 @@ class Run:
                            _lib.GRAPH_SPATIAL_WEIGHTS: spatial_weights_from_graph(conn, dist, False, True)}
             for which, mat in self.graphs.items():
                 self.e.set_graph(which, mat)
-            self.e.set_ct_encode(inp["ct_encode"])
-        self.e.set_mapping(np.random.default_rng(seed + 1).standard_normal((N, V)).astype(np.float32))
+            self.e.set_ct_encode(np.ascontiguousarray(inp["ct_encode"][rs]))
+        self.e.set_mapping(np.ascontiguousarray(np.random.default_rng(seed + 1).standard_normal((N, V)).astype(np.float32)[rs]))
         self.inp = inp
         self.Ke, self.ld, self.splits, _, self.nchunks = (int(x) for x in self.e.debug("shape"))
-        self.S = _g(self.e.debug("Sx").reshape(N, self.Ke))        # fp32 S_ext the contractions read, widened
+        self.S = _g(self.e.debug("Sx").reshape(self.N, self.Ke))   # fp32 S_ext the contractions read, widened
         self.G = _g(inp["G"])
         self.d = _g(inp["d"])
 
@@ -264,7 +268,12 @@ def _check_loss_stage(r, Y_dev, dY_dev, hist, M, mode):
         assert abs(got - want) <= tol, f"{mode} history column {col}: {got} vs {want}"
     colmax = dref.abs().max(dim=0, keepdim=True).values.expand_as(dref)
     c = 4 * n * U
-    _check(f"{mode} dY_ext", dY_dev, dref, colmax, c, 4 * np.sqrt(n) * U, 4 * np.sqrt(n) * U, floor=0.0)
+    if r.precision == "bf16":
+        # dY_ext is kept as one bf16 plane: one round to nearest more, u_b |ref| (tests/test_loss_stage_gpu.py)
+        _check(f"{mode} dY_ext (bf16)", dY_dev, dref, colmax, c * (1 + UB), 4 * np.sqrt(n) * U + UB,
+               4 * np.sqrt(n) * U + UB / 16, floor=UB * dref.abs())
+    else:
+        _check(f"{mode} dY_ext", dY_dev, dref, colmax, c, 4 * np.sqrt(n) * U, 4 * np.sqrt(n) * U, floor=0.0)
     return dref
 
 
@@ -353,7 +362,6 @@ X3_SHAPES = [
 def test_bf16x3_stages(N, V, K, clusters):
     """bf16x3: row pass, forward, loss stage, backward (fp32 dP and row-dot) and the exact update, each from the device's
     own inputs, at step 1 and step 3."""
-    torch = _torch()
     r = Run("bf16x3", N, V, K, seed=N + V + K, clusters=clusters)
     for step in range(1, 4):
         pre = _state(r)
@@ -370,22 +378,33 @@ def test_bf16x3_stages(N, V, K, clusters):
         dY = r.buf("dY", r.Ke)
         hist = r.e.history()[-1]
         _check_loss_stage(r, Yd, dY, hist, pre[0], f"x3[{step}]")
-        # backward: dP = S_ext dY_ext^T over Ke (one chain), the row-dot r_i = sum_j P_ij dP_ij from the fp32 P
-        dpf = r.nv("dpf")
-        dPref = r.S @ dY.t()
-        scale = r.S.abs() @ dY.abs().t()
-        ce, _, _ = _x3_contraction_consts(r.Ke)
-        cf, cb = X3_BWD_FRO, X3_BWD_BIAS
-        _check(f"x3[{step}] dP (Ke {r.Ke})", dpf[:, :V], dPref, scale, ce, cf, cb)
-        assert torch.count_nonzero(dpf[:, V:]) == 0, "pad columns of dP"
-        rdot = r.buf("rdot")
-        rref = (P3[:, :V] * dPref).sum(dim=1)
-        rscale = (P3[:, :V] * scale).sum(dim=1)
-        _check(f"x3[{step}] row-dot", rdot, rref, rscale, ce + (V + 2) * 2 * U, cf + V * U, cb + 4 * U)
-        # the exact update: g = (dP - r) P from the device's fp32 values (the bound check; bit equality below)
-        g = _grad_terms(r, pre[0][:, :V], P3[:, :V], dpf[:, :V] - rdot[:, None], stats[:, 0] + stats[:, 2], stats[:, 3])
+        _check_backward_x3(r, pre, t, stats, P3, dY, f"x3[{step}]")
+
+
+def _check_backward_x3(r, pre, t, stats, P3, dY, mode):
+    """bf16x3 backward from the device's dY_ext: dP = S_ext dY_ext^T over Ke (one chain), the row-dot
+    r_i = sum_j P_ij dP_ij from the fp32 P, and the exact update from the pre-step state `pre` at step count t."""
+    torch = _torch()
+    V = r.V
+    dpf = r.nv("dpf")
+    dPref = r.S @ dY.t()
+    scale = r.S.abs() @ dY.abs().t()
+    ce, _, _ = _x3_contraction_consts(r.Ke)
+    cf, cb = X3_BWD_FRO, X3_BWD_BIAS
+    _check(f"{mode} dP (Ke {r.Ke})", dpf[:, :V], dPref, scale, ce, cf, cb)
+    assert torch.count_nonzero(dpf[:, V:]) == 0, "pad columns of dP"
+    rdot = r.buf("rdot")
+    rref = (P3[:, :V] * dPref).sum(dim=1)
+    rscale = (P3[:, :V] * scale).sum(dim=1)
+    _check(f"{mode} row-dot", rdot, rref, rscale, ce + (V + 2) * 2 * U, cf + V * U, cb + 4 * U)
+    # the exact update: g = (dP - r) P from the device's fp32 values (the bound check; bit equality in
+    # test_bf16x3_update_is_torch_adam)
+    g = _grad_terms(r, pre[0][:, :V], P3[:, :V], dpf[:, :V] - rdot[:, None], stats[:, 0] + stats[:, 2], stats[:, 3])
+    if r.lam:       # entropy / L1 / L2 gradient terms: the bound of test_bf16x3_all_terms_clusters
+        dg = 8 * U * (g.abs() + P3[:, :V] * (dpf[:, :V].abs() + rdot.abs()[:, None] + 1.0))
+    else:
         dg = 4 * U * (g.abs() + P3[:, :V] * (dpf[:, :V].abs() + rdot.abs()[:, None]))
-        _check_update(r, pre, _state(r), g, dg, t + 1, f"x3[{step}]")
+    _check_update(r, pre, _state(r), g, dg, t + 1, mode)
 
 
 @pytest.mark.parametrize("N,V,K", [(2100, 300, 70), (700, 5, 64), (1500, 263, 130)])
@@ -461,7 +480,6 @@ def test_fp32_stages(N, V, K, clusters, lam):
     """fp32 (FFMA): row pass, forward, loss stage, and the fused update (EpiAdam never stores dP: dP is recomputed in
     float64 from the device's S_ext and dY).  FFMA chains are round-to-nearest: |err| <= 2 k u (|A||B|), rel-Fro and bias
     sqrt(k)-class, 4 sqrt(k) u and 4 u."""
-    torch = _torch()
     T = 8 if lam else 0
     r = Run("fp32", N, V, K, seed=N + K, T=T, clusters=clusters, lam=lam)
     for step in range(1, 4):
@@ -474,21 +492,32 @@ def test_fp32_stages(N, V, K, clusters, lam):
         stats = r.buf("stats", 4)
         Pf = r.nv("Pf")
         Pref = _check_row_pass(r, pre[0], Pf, stats, f"fp32[{step}] row pass")
-        chain = -(-N // r.splits)
         Yd = r.buf("Y", r.Ke)
-        _check_forward(r, Yd, Pref, (2 * chain + r.splits + V + 32) * U, 4 * np.sqrt(chain) * U + (r.splits + 16) * U, 20 * U,
-                       f"fp32[{step}]")
+        _check_forward(r, Yd, Pref, *_fp32_forward_consts(r), f"fp32[{step}]")
         dY = r.buf("dY", r.Ke)
         _check_loss_stage(r, Yd, dY, r.e.history()[-1], pre[0], f"fp32[{step}]")
-        dPref = r.S @ dY.t()
-        scale = r.S.abs() @ dY.abs().t()
-        rdot = r.buf("rdot")
-        rref = (Pf[:, :V] * dPref).sum(dim=1)
-        rscale = (Pf[:, :V] * scale).sum(dim=1)
-        _check(f"fp32[{step}] row-dot", rdot, rref, rscale, (2 * (r.Ke + V) + 8) * U, 4 * np.sqrt(r.Ke + V) * U, 4 * U)
-        g = _grad_terms(r, pre[0][:, :V], Pf[:, :V], dPref - rdot[:, None], stats[:, 0] + stats[:, 2], stats[:, 3])
-        dg = Pf[:, :V] * (2 * r.Ke + 8) * U * scale + 8 * U * (g.abs() + Pf[:, :V] * (dPref.abs() + rdot.abs()[:, None] + 1.0))
-        _check_update(r, pre, _state(r), g, dg, t + 1, f"fp32[{step}]")
+        _check_backward_fp32(r, pre, t, stats, Pf, dY, f"fp32[{step}]")
+
+
+def _fp32_forward_consts(r):
+    """FFMA forward over a chain of one split of the cells, the splits summed in fp32, P's row-pass error on top."""
+    chain = -(-r.N // r.splits)
+    return (2 * chain + r.splits + r.V + 32) * U, 4 * np.sqrt(chain) * U + (r.splits + 16) * U, 20 * U
+
+
+def _check_backward_fp32(r, pre, t, stats, Pf, dY, mode):
+    """fp32 backward from the device's dY_ext: the row-dot, and the fused update from the pre-step state `pre` at step
+    count t (EpiAdam never stores dP: dP is recomputed in float64 from the device's S_ext and dY)."""
+    V = r.V
+    dPref = r.S @ dY.t()
+    scale = r.S.abs() @ dY.abs().t()
+    rdot = r.buf("rdot")
+    rref = (Pf[:, :V] * dPref).sum(dim=1)
+    rscale = (Pf[:, :V] * scale).sum(dim=1)
+    _check(f"{mode} row-dot", rdot, rref, rscale, (2 * (r.Ke + V) + 8) * U, 4 * np.sqrt(r.Ke + V) * U, 4 * U)
+    g = _grad_terms(r, pre[0][:, :V], Pf[:, :V], dPref - rdot[:, None], stats[:, 0] + stats[:, 2], stats[:, 3])
+    dg = Pf[:, :V] * (2 * r.Ke + 8) * U * scale + 8 * U * (g.abs() + Pf[:, :V] * (dPref.abs() + rdot.abs()[:, None] + 1.0))
+    _check_update(r, pre, _state(r), g, dg, t + 1, mode)
 
 
 # ------------------------------------------------------------------------------------------------------------------ bf16
@@ -568,28 +597,35 @@ def test_bf16_stages(N, V, K, lam_r):
             _check_forward(r, r.buf("Y", r.Ke), Pt_fwd, *_bf16_forward_consts(r), f"bf16[{step}]", S=Ss)
         if step not in (1, 3):
             continue
-        # the update from the device's dq, rowc = (lse, r', h) and pre-step state
-        dq = r.nv("dq")[:, :V]
-        rowc = r.buf("rowc", 4)
-        assert torch.equal(rowc[:, 0], lseT_now), "rowc carries the row's exact log-sum-exp"
-        Mv = pre[0][:, :V]
-        P = torch.exp(Mv - rowc[:, 0:1])
-        g = _grad_terms(r, Mv, P, dq - rowc[:, 1:2], rowc[:, 0], rowc[:, 2])
-        dg = (UM * (4 + 2 * Mv.abs() + 2 * rowc[:, 0:1].abs()) + 4 * U) * g.abs() + 4 * U * P * (dq.abs() + rowc[:, 1:2].abs())
-        dg = dg + (r.lam.get("lambda_r", 0.0) * P * 8 * U * (Mv.abs() + rowc[:, 0:1].abs() + rowc[:, 2:3].abs()))
-        post = _state(r)
-        _check_update_bf16(r, pre, post, g, dg, t + 1, f"bf16[{step}]")
-        # what the update left for the next forward: P~ = bf16(exp(Mnew - lse)), z~ = sum of the unrounded values
-        Mn = post[0][:, :V]
-        lseA = r.buf("lseA")
-        assert torch.equal(lseA, lseT_now), "after step_end lseA is the offset the new P~ was written with"
-        Pt_ref = torch.exp(Mn - lseA[:, None])
-        Pt = r.nv("Pb")
-        bad = (Pt[:, :V] - Pt_ref).abs() > (UB + UM * (2 + Mn.abs() + lseA.abs()[:, None])) * Pt_ref
-        assert not bool(bad.any()), f"bf16[{step}] P~ after the update: {int(bad.sum())} elements off"
-        assert torch.count_nonzero(Pt[:, V:]) == 0, "pad columns of P~"
-        _check(f"bf16[{step}] z~", r.buf("zsum"), Pt_ref.sum(dim=1), Pt_ref.sum(dim=1),
-               (V + 8) * U + UM * (2 + Mn.abs().max().item() + lseA.abs().max().item()), (V + 8) * U + 4 * UM, (V + 8) * U + 4 * UM)
+        _check_bf16_update_step(r, pre, t, lseT_now, f"bf16[{step}]")
+
+
+def _check_bf16_update_step(r, pre, t, lseT_now, mode):
+    """The bf16 streaming update from the device's dq, rowc = (lse, r', h) and the pre-step state `pre` at step count t
+    (lseT_now: lseT after step_begin), then the P~ and z~ it left for the next forward."""
+    torch = _torch()
+    V = r.V
+    dq = r.nv("dq")[:, :V]
+    rowc = r.buf("rowc", 4)
+    assert torch.equal(rowc[:, 0], lseT_now), "rowc carries the row's exact log-sum-exp"
+    Mv = pre[0][:, :V]
+    P = torch.exp(Mv - rowc[:, 0:1])
+    g = _grad_terms(r, Mv, P, dq - rowc[:, 1:2], rowc[:, 0], rowc[:, 2])
+    dg = (UM * (4 + 2 * Mv.abs() + 2 * rowc[:, 0:1].abs()) + 4 * U) * g.abs() + 4 * U * P * (dq.abs() + rowc[:, 1:2].abs())
+    dg = dg + (r.lam.get("lambda_r", 0.0) * P * 8 * U * (Mv.abs() + rowc[:, 0:1].abs() + rowc[:, 2:3].abs()))
+    post = _state(r)
+    _check_update_bf16(r, pre, post, g, dg, t + 1, mode)
+    # what the update left for the next forward: P~ = bf16(exp(Mnew - lse)), z~ = sum of the unrounded values
+    Mn = post[0][:, :V]
+    lseA = r.buf("lseA")
+    assert torch.equal(lseA, lseT_now), "after step_end lseA is the offset the new P~ was written with"
+    Pt_ref = torch.exp(Mn - lseA[:, None])
+    Pt = r.nv("Pb")
+    bad = (Pt[:, :V] - Pt_ref).abs() > (UB + UM * (2 + Mn.abs() + lseA.abs()[:, None])) * Pt_ref
+    assert not bool(bad.any()), f"{mode} P~ after the update: {int(bad.sum())} elements off"
+    assert torch.count_nonzero(Pt[:, V:]) == 0, "pad columns of P~"
+    _check(f"{mode} z~", r.buf("zsum"), Pt_ref.sum(dim=1), Pt_ref.sum(dim=1),
+           (V + 8) * U + UM * (2 + Mn.abs().max().item() + lseA.abs().max().item()), (V + 8) * U + 4 * UM, (V + 8) * U + 4 * UM)
 
 
 def _bf16_forward_consts(r):
