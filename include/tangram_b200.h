@@ -186,12 +186,11 @@ TGB200_API int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, vo
 /* Mapper.train(val_each=every) (:398-403) without leaving the device: while `every` > 0, tgb200_run and step_begin /
  * step_end validate epoch e -- counted from this call, from 0 -- when e % every == 0, and write _val_loss_fn's four values
  * (:311-356: on the training matrices, over the genes of the loss mask) into history columns TGB200_HIST_VAL_* of that
- * epoch's row.  Values are those of tgb200_validation_terms after the epoch's update: bit for bit, except the sparsity-weighted
- * score, which is summed from the per-gene cosines in fp32 (tgb200_validation_terms recovers them from the loss
- * coefficients on the host).  fp32 / bf16x3: the next iteration of the same tgb200_run call computes the validation from its
- * own forward (identical: same row pass, same contraction); the last iteration of a call and constrained mode run one
- * separate forward.  bf16 mode: one exact row pass and forward per validated epoch, which -- as after
- * tgb200_validation_terms -- the next iteration then starts from.  No allocation and no host sync in the loop.
+ * epoch's row.  Values are those of tgb200_validation_terms after the epoch's update, bit for bit.  fp32 / bf16x3: the next
+ * iteration of the same tgb200_run call computes the validation from its own forward (identical: same row pass, same
+ * contraction); the last iteration of a call and constrained mode run tgb200_validation_terms' forward.  bf16 mode: that
+ * exact row pass and forward once per validated epoch, which the next iteration then starts from, as after
+ * tgb200_validation_terms.  No allocation and no host sync in the loop.
  * every = 0 (the default) turns validation off.  TGB200_ERR_STATE between step_begin and step_end; every > 0 on a sharded
  * handle is TGB200_ERR_UNSUPPORTED.  Allocates the validation's scratch (about 8 (Ke + V) bytes, more when lambda_g2 == 0) on first use;
  * queues no work on `stream`. */
@@ -259,10 +258,15 @@ TGB200_API int tgb200_get_history(tgb200_mapper* h, int64_t first, int64_t count
 /* softmax(M, dim=1) as n_cells x n_voxels f32 (host or device).  Replaces :406-408. */
 TGB200_API int tgb200_get_mapping(tgb200_mapper* h, float* out, void* stream);
 /* _val_loss_fn (:311-356) of the current mapping: out[4] = expression_sim, gv_sim, sp_sparsity_weighted_gv_sim, entropy
- * (HOST).  Synchronous, with scratch allocated per call; tgb200_set_validation computes the same inside the loop. */
+ * (HOST).  One forward on the device and one 16-byte copy, the forward and kernels tgb200_set_validation runs in the loop
+ * (so the values are those bit for bit); allocates the same scratch on first use.  Synchronous on `stream`.
+ * TGB200_ERR_STATE between step_begin and step_end; TGB200_ERR_UNSUPPORTED on a sharded handle. */
 TGB200_API int tgb200_validation_terms(tgb200_mapper* h, float* out4_host, void* stream);
-/* project_genes' GEMM (tangram/utils.py:368): out (n_voxels x n_cols) = softmax(M)^T X,
- * X (n_cells x n_cols) row-major f32, host or device; fp32 accumulate. */
+/* project_genes' GEMM (tangram/utils.py:368): out (n_voxels x n_cols, host or device) = softmax(M)^T X, X (n_cells x
+ * n_cols) row-major f32, host or device.  tgb200_project_map's blocks and arithmetic, with each block's mapping rows
+ * written as bf16 planes by the row pass (no copy of the mapping): the result equals tgb200_project_map on the
+ * tgb200_get_mapping of the same M, bit for bit, in every precision.  Writes the row statistics as tgb200_get_mapping does;
+ * training continues unperturbed.  Device memory: out plus two blocks of staging (see tgb200_project_map).  Synchronous. */
 TGB200_API int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, float* out, void* stream);
 
 /* Run-to-run agreement of R equally shaped arrays (the hyper-parameter tuner's metrics,
@@ -306,9 +310,9 @@ TGB200_API int tgb200_annotate(const float* map, int64_t rows, int64_t cols, int
  *   data     nnz f32 values (host or device)
  *   out      cols x n_genes f32 (host or device)
  *   block_rows  cells staged per block, a multiple of 2048; 0 = about an eighth of the cells, less if free memory needs it
- * Arithmetic as tgb200_project: three bf16 planes per operand, six partial products on the tensor cores; accumulation
- * chains of 512 cells (tgb200_project: at most 2048), added in cell order in fp32 (round-to-nearest); no atomics.  The result does not depend on how
- * the data is staged: dense or CSR X, host or device pointers and any block size give identical bits.
+ * Three bf16 planes per operand, six partial products on the tensor cores; accumulation chains of 512 cells, added in cell
+ * order in fp32 (round-to-nearest); no atomics.  The result does not depend on how the data is staged: dense or CSR X,
+ * host or device pointers and any block size give identical bits.
  * Cell blocks of the mapping and X are double-buffered (the copies of block b + 1 run on a second stream while block b
  * contracts); device memory is out plus two blocks of staging, whatever `rows` is.  A CSR block is turned into the bf16
  * planes directly, one warp per row.  TGB200_ERR_INVALID for bad shapes, a malformed indptr, a column index outside

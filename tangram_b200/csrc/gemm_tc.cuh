@@ -648,7 +648,7 @@ static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs
   return tc_check_launch("tc_gemm_fwd", err, n);
 }
 // cells [row0, row1) only (row0 a multiple of 64): `out` = or += this chunk's partial sum -- the host pipelines cell chunks
-// behind the streaming Adam kernel (and tgb200_project_map adds its 512-cell chains); the chunks run one after the other
+// behind the streaming Adam kernel (and the projection adds its 512-cell chains); the chunks run one after the other
 // on one stream, so the summation order is fixed
 static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int accumulate, int row0, int row1,
                                          int V, int Ke, cudaStream_t s, char* err, size_t n) {
@@ -659,14 +659,6 @@ static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, int n_
   kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, row1, (int)round_up(row1 - row0, TC_BK), tm, tn,
                                                                     1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
   return tc_check_launch("tc_gemm_fwd", err, n);
-}
-// one-shot variant for temporary operands (tgb200_project)
-static inline int tc_forward(TcContext& tc, const __nv_bfloat16* P, size_t p_plane, const __nv_bfloat16* Sx, size_t s_plane,
-                             int n_pairs, float* out, int N, int V, int Ke, int ld, int splits, cudaStream_t s, char* err,
-                             size_t n) {
-  TcPlan pl;
-  if (tc_forward_plan(tc, pl, P, p_plane, Sx, s_plane, n_pairs > 1 ? 3 : 1, N, V, Ke, ld, err, n)) return -2;
-  return tc_forward_launch(tc, pl, n_pairs, out, N, V, Ke, splits, s, err, n);
 }
 
 // Staged backward: dq = bf16(S_ext dY_ext^T - centre) (bf16 mode) or dP in fp32 (bf16x3 mode, three operand planes, six

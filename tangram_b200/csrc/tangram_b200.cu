@@ -133,12 +133,11 @@ struct tgb200_mapper {
   CsrDev W, WT, F, FT, A, AT;
   int nchunk = 0, ncolchunk = 0, nredchunk = 0, n_ct_blocks = 0, loss_rows = 16;
   DevBuf<float> colfin;         // finalised per-gene sums: [3 | 2 | 2][Ke]
-  // training-gene mask of the loss (tgb200_set_loss_genes): gene_act[k] in {0, 1} (Ke floats, device and host) when
-  // `masked`; n_active of the K genes are in the loss
+  // training-gene mask of the loss (tgb200_set_loss_genes): gene_act[k] in {0, 1} (Ke floats) when `masked`; n_active of
+  // the K genes are in the loss
   bool masked = false;
   int n_active = 0;
   DevBuf<float> gene_act;
-  std::vector<float> gene_act_host;
   DevBuf<float> gw;             // Ke: sparsity weight of each gene in the loss (k_gene_weights), for the validation
   // per-epoch validation in the loop (tgb200_set_validation): epoch e (counted from that call) is validated when
   // e % val_every == 0, into history columns 12-15 of its row
@@ -644,8 +643,7 @@ extern "C" int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, vo
   h->n_active = n;
   if (h->masked) {
     if (!h->gene_act.p) CKS(h->gene_act.alloc(h->Ke, false));
-    h->gene_act_host.swap(flags);
-    CK(cudaMemcpyAsync(h->gene_act.p, h->gene_act_host.data(), sizeof(float) * h->Ke, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->gene_act.p, flags.data(), sizeof(float) * h->Ke, cudaMemcpyHostToDevice, s));
   }
   if (h->have_expr) {
     k_row_norms<<<(unsigned)ceil_div(h->V, 8), 256, 0, s>>>(h->V, h->K, h->Ke, h->G.p, h->masked ? h->gene_act.p : nullptr, h->ngr.p);
@@ -656,19 +654,22 @@ extern "C" int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, vo
   return TGB200_OK;
 }
 
-// Per-epoch validation inside tgb200_run / step_end (Mapper.train(val_each=), mapping_optimizer.py:398-403).  The scratch
-// of the validation's loss scalars is allocated here, on first use, never in the loop.
+// The scratch of the validation's loss scalars (val_loss_params), allocated on first use and kept: never in the loop.
+static int alloc_validation(tgb200_mapper* h) {
+  if (!h->val_coef.p) CKS(h->val_coef.alloc(2 * (size_t)h->Ke + 2 * (size_t)h->V));
+  if (!h->val_hist.p) CKS(h->val_hist.alloc(TGB200_HIST_COLS));
+  if (!h->rowpart.p && !h->val_rowpart.p) CKS(h->val_rowpart.alloc((size_t)h->ncolchunk * h->V * 2));
+  return TGB200_OK;
+}
+
+// Per-epoch validation inside tgb200_run / step_end (Mapper.train(val_each=), mapping_optimizer.py:398-403).
 extern "C" int tgb200_set_validation(tgb200_mapper* h, int32_t every, void* stream) {
   if (!h) return fail(TGB200_ERR_INVALID, "null handle");
   if (every < 0) return fail(TGB200_ERR_INVALID, "every = %d < 0", every);
   if (h->in_step) return fail(TGB200_ERR_STATE, "set_validation inside a step");
   if (every > 0 && h->cfg.n_cells_global != h->N) return fail(TGB200_ERR_UNSUPPORTED, "validation on a sharded handle");
   CK(cudaSetDevice(h->cfg.device));
-  if (every > 0) {
-    if (!h->val_coef.p) CKS(h->val_coef.alloc(2 * (size_t)h->Ke + 2 * (size_t)h->V));
-    if (!h->val_hist.p) CKS(h->val_hist.alloc(TGB200_HIST_COLS));
-    if (!h->rowpart.p && !h->val_rowpart.p) CKS(h->val_rowpart.alloc((size_t)h->ncolchunk * h->V * 2));
-  }
+  if (every > 0) CKS(alloc_validation(h));
   (void)stream;                                      // nothing is queued: the switch takes effect at the next step
   h->val_every = every;
   h->val_epoch = 0;
@@ -1200,7 +1201,7 @@ static int reduce_columns(tgb200_mapper* h, cudaStream_t s, LossParams& p, bool 
 // per-voxel partials of the row cosine: the training's own when lambda_g2 != 0, the validation's otherwise
 static float* any_rowpart(tgb200_mapper* h) { return h->rowpart.p ? h->rowpart.p : h->val_rowpart.p; }
 
-// _val_loss_fn's parameters (:311-356, as tgb200_validation_terms sets them): gene-voxel and voxel-gene cosines with weight 1,
+// _val_loss_fn's parameters (:311-356): gene-voxel and voxel-gene cosines with weight 1,
 // no other term; the four values go to `out` (device), everything else k_loss_scalars writes goes to the validation's own
 // scratch, so the training's coefficients, dY and filter scalars are left alone
 static LossParams val_loss_params(tgb200_mapper* h, float* out) {
@@ -1388,9 +1389,9 @@ static int backward_fp32(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
   return TGB200_OK;
 }
 
-// The separate validation forward: what tgb200_validation_terms runs on the device, into out[0..3] (device), on `s`.
-// bf16 mode re-runs the exact row pass, so the per-row entropy exists whatever lambda_r is; P is then fresh and the next
-// iteration starts from it, exactly as after tgb200_validation_terms.
+// The separate validation forward (and all of tgb200_validation_terms), into out[0..3] (device), on `s`.  bf16 mode re-runs
+// the exact row pass, so the per-row entropy exists whatever lambda_r is; P is then fresh and the next iteration starts
+// from it.
 static int validation_forward(tgb200_mapper* h, cudaStream_t s, float* out) {
   if (h->bf16) { h->p_state = PState::stale; h->fwd_ahead = false; }
   CKS(forward_pass(h, s, 1));
@@ -1427,7 +1428,7 @@ extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
   // the validation of this epoch, on the mapping its update produced (mapping_optimizer.py:398-403)
   if (val_due(h)) {
     // fp32 / bf16x3 inside tgb200_run: the next iteration's forward serves it.  Constrained mode keeps the separate forward,
-    // which (as tgb200_validation_terms) still sees the filter of this epoch; the next forward sees the updated one.
+    // which still sees the filter of this epoch; the next forward sees the updated one.
     if (h->val_fuse && !h->bf16 && !h->constrained) {
       h->val_row = h->hist_len;
     } else {
@@ -1682,71 +1683,7 @@ extern "C" int tgb200_set_state(tgb200_mapper* h, const float* M, const float* m
   return TGB200_OK;
 }
 
-extern "C" int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, float* out, void* stream) {
-  if (!h || !X || !out || n_cols <= 0) return fail(TGB200_ERR_INVALID, "bad argument");
-  if (!h->have_mapping) return fail(TGB200_ERR_STATE, "no mapping set");
-  cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaSetDevice(h->cfg.device));
-  // softmax(M)^T X, gene columns streamed through in chunks (tangram/utils.py:368)
-  const int chunk = 2048;
-  if (h->tcm) {
-    // tensor-core modes: the forward contraction kernel with split-bf16 operands (three planes each, six partial
-    // products, accumulation chains cut at 2048 cells) -- fp32-grade results whatever the training precision was
-    const size_t pplane = (size_t)h->N * h->ld;
-    DevBuf<__nv_bfloat16> Pown, Xb;
-    __nv_bfloat16* Pp = h->Pb.p;                    // bf16x3 mode rewrites its P planes every iteration anyway
-    if (!h->x3) { CKS(Pown.alloc(3 * pplane, false)); Pp = Pown.p; }   // bf16 mode: Pb carries the unnormalised P state
-    CKS(launch_softmax_rows<float>(h, s, (float*)nullptr, 0, nullptr, Split3{Pp, pplane}));
-    const int ldc = (int)round_up(n_cols < chunk ? n_cols : chunk, 64);
-    int splits = tc_forward_splits(h->tc.num_sms, h->N, h->V, ldc);
-    { const int c = tc_splits_for_chain(h->N, 2048); if (c > splits) splits = c; }
-    const size_t xplane = (size_t)h->N * ldc, oplane = (size_t)h->V * ldc;
-    DevBuf<float> Xc, Opart, Oc;
-    CKS(Xc.alloc(xplane)); CKS(Xb.alloc(3 * xplane, false)); CKS(Opart.alloc((size_t)splits * oplane, false));
-    if (splits > 1) CKS(Oc.alloc(oplane, false));
-    for (int64_t c0 = 0; c0 < n_cols; c0 += chunk) {
-      const int nc = (int)((n_cols - c0) < chunk ? (n_cols - c0) : chunk);
-      if (nc < ldc) CK(cudaMemsetAsync(Xc.p, 0, xplane * sizeof(float), s));
-      CK(cudaMemcpy2DAsync(Xc.p, (size_t)ldc * sizeof(float), X + c0, (size_t)n_cols * sizeof(float),
-                           (size_t)nc * sizeof(float), h->N, cudaMemcpyDefault, s));
-      k_split3<<<(unsigned)ceil_div(xplane / 4, 256), 256, 0, s>>>(Xc.p, Split3{Xb.p, xplane}, (long long)(xplane / 4));
-      LAUNCH_CHECK("split3");
-      CKS(tc_forward(h->tc, Pp, pplane, Xb.p, xplane, 6, Opart.p, h->N, h->V, ldc, h->ld, splits, s, g_err, sizeof(g_err)));
-      const float* res = Opart.p;
-      if (splits > 1) {
-        k_sum_planes<<<(unsigned)ceil_div(oplane, 256), 256, 0, s>>>(Opart.p, splits, oplane, Oc.p);
-        LAUNCH_CHECK("sum_planes");
-        res = Oc.p;
-      }
-      CK(cudaMemcpy2DAsync(out + c0, (size_t)n_cols * sizeof(float), res, (size_t)ldc * sizeof(float),
-                           (size_t)nc * sizeof(float), h->V, cudaMemcpyDefault, s));
-    }
-    CK(cudaStreamSynchronize(s));
-    return TGB200_OK;
-  }
-  CKS(launch_softmax_rows<float>(h, s, h->Pf.p, 0, nullptr));
-  const int ldc = (int)round_up(n_cols < chunk ? n_cols : chunk, 4);
-  DevBuf<float> Xc, Oc;
-  CKS(Xc.alloc((size_t)h->N * ldc)); CKS(Oc.alloc((size_t)h->V * ldc));
-  for (int64_t c0 = 0; c0 < n_cols; c0 += chunk) {
-    const int nc = (int)((n_cols - c0) < chunk ? (n_cols - c0) : chunk);
-    CK(cudaMemsetAsync(Xc.p, 0, Xc.n * sizeof(float), s));
-    CK(cudaMemcpy2DAsync(Xc.p, (size_t)ldc * sizeof(float), X + c0, (size_t)n_cols * sizeof(float),
-                         (size_t)nc * sizeof(float), h->N, cudaMemcpyDefault, s));
-    GemmArgs g;
-    g.A = h->Pf.p; g.lda = h->ld; g.B = Xc.p; g.ldb = ldc; g.M = h->V; g.N = nc; g.K = h->N;
-    g.k_per_split = (int)round_up(h->N, 16);
-    EpiStorePartial epi{Oc.p, ldc, 0};
-    dim3 grid((unsigned)ceil_div(nc, SG_BN), (unsigned)ceil_div(h->V, SG_BM), 1);
-    k_gemm_simt<false, false, EpiStorePartial><<<grid, SG_THREADS, 0, s>>>(g, epi);
-    LAUNCH_CHECK("simt_gemm_project");
-    CK(cudaMemcpy2DAsync(out + c0, (size_t)n_cols * sizeof(float), Oc.p, (size_t)ldc * sizeof(float),
-                         (size_t)nc * sizeof(float), h->V, cudaMemcpyDefault, s));
-  }
-  CK(cudaStreamSynchronize(s));
-  return TGB200_OK;
-}
-
+// _val_loss_fn (:311-356) on demand: the validation forward tgb200_set_validation runs in the loop, then one 16-byte copy
 extern "C" int tgb200_validation_terms(tgb200_mapper* h, float* out4, void* stream) {
   if (!h || !out4) return fail(TGB200_ERR_INVALID, "null argument");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1754,48 +1691,12 @@ extern "C" int tgb200_validation_terms(tgb200_mapper* h, float* out4, void* stre
   CKS(check_ready(h));
   if (h->in_step) return fail(TGB200_ERR_STATE, "validation_terms inside a step");
   if (h->cfg.n_cells_global != h->N) return fail(TGB200_ERR_UNSUPPORTED, "validation_terms on a sharded handle");
-  // _val_loss_fn (:311-356): a second forward on the train matrices.  bf16 mode: re-run the exact row pass so that the
-  // per-row entropy exists whatever lambda_r is (in steady state it is only carried when the entropy term is on)
-  if (h->bf16) { h->p_state = PState::stale; h->fwd_ahead = false; }
-  CKS(forward_pass(h, s, 1));
-  LossParams p = make_loss_params(h);
-  DevBuf<float> rowpart, coefAr, coefBr, hist;
-  CKS(rowpart.alloc((size_t)h->ncolchunk * h->V * 2)); CKS(coefAr.alloc(h->V)); CKS(coefBr.alloc(h->V));
-  CKS(hist.alloc(TGB200_HIST_COLS));
-  p.rowpart = rowpart.p; p.coefAr = coefAr.p; p.coefBr = coefBr.p;
-  p.lam_g2 = 1.f; p.lam_g1 = 1.f; p.lam_nb = 0.f; p.lam_go = 0.f; p.lam_ct = 0.f; p.density_mode = 0;
-  CKS(reduce_columns(h, s, p, true, 1));
-  k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, nullptr, nullptr, h->N, h->Y.p + (size_t)h->V * h->Ke);
-  LAUNCH_CHECK("row_scalar_reduce");
-  k_loss_scalars<false><<<1, 1024, 0, s>>>(p, 1, h->nredchunk, hist.p);
-  LAUNCH_CHECK("loss_scalars");
-  // sparsity-weighted gene score needs per-gene cosines: recover them from coefA/coefB on the host
-  std::vector<float> hrow(TGB200_HIST_COLS), cA(h->K), cB(h->K), Gh((size_t)h->V * h->Ke), tail(4);
-  CK(cudaMemcpyAsync(hrow.data(), hist.p, sizeof(float) * TGB200_HIST_COLS, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(cA.data(), h->coefA.p, sizeof(float) * h->K, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(cB.data(), h->coefB.p, sizeof(float) * h->K, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(Gh.data(), h->G.p, sizeof(float) * Gh.size(), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(tail.data(), h->Y.p + (size_t)h->V * h->Ke, sizeof(float) * 4, cudaMemcpyDeviceToHost, s));
-  std::vector<float> ngc(h->K);
-  CK(cudaMemcpyAsync(ngc.data(), h->ngc.p, sizeof(float) * h->K, cudaMemcpyDeviceToHost, s));
+  CKS(alloc_validation(h));
+  DevBuf<float> d4;
+  CKS(d4.alloc(4, false));
+  CKS(validation_forward(h, s, d4.p));
+  CK(cudaMemcpyAsync(out4, d4.p, 4 * sizeof(float), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  // cos_k = coefB_k * K' * ny^2 with ny = 1/(coefA_k * K' * ng)  (lam_g1 = 1 here; the K' genes of the loss)
-  double wsum = 0.0, acc = 0.0;
-  const double Kd = h->n_active;
-  for (int k = 0; k < h->K; ++k) {
-    if (h->masked && h->gene_act_host[k] == 0.f) continue;
-    long nz = 0;
-    for (int j = 0; j < h->V; ++j) nz += Gh[(size_t)j * h->Ke + k] != 0.f;
-    const double w = (double)nz / h->V;       // 1 - gene_sparsity (:330)
-    const double ny = 1.0 / ((double)cA[k] * Kd * ngc[k]);
-    const double cosk = (double)cB[k] * Kd * ny * ny;
-    wsum += w; acc += cosk * w;
-  }
-  const float gv = hrow[1], vg = hrow[2];
-  out4[0] = gv + vg;                                   // expression_sim (:328)
-  out4[1] = gv;                                        // gv_sim (:326)
-  out4[2] = (float)(acc / wsum);                       // sp_sparsity_weighted_gv_sim (:331)
-  out4[3] = -(tail[0] / logf((float)h->V)) / h->N;     // entropy (:333)
   return TGB200_OK;
 }
 
@@ -2159,10 +2060,13 @@ struct CopyStream {                      // the second stream and its events, re
 };
 }  // namespace
 
-extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, int64_t ld, const float* X, int64_t x_ld,
-                                  const int64_t* indptr, const int32_t* indices, const float* data, int64_t nnz,
-                                  int64_t n_genes, float* out, int64_t block_rows, int32_t device, void* stream) {
-  if (!map || !out) return fail(TGB200_ERR_INVALID, "null argument");
+// The projection of tgb200_project_map and tgb200_project.  The mapping rows come from `map` (fp32, row stride `ld`,
+// copied on the copy stream, then k_split3) or, with a handle `h` and no `map`, from softmax(M): the row pass writes each
+// block's three planes directly, and the statistics of its rows as tgb200_get_mapping does.  Both write the same planes
+// for the same probabilities, so a handle's projection equals tgb200_project_map of its tgb200_get_mapping, bit for bit.
+static int project_blocks(tgb200_mapper* h, const float* map, int64_t rows, int64_t cols, int64_t ld, const float* X,
+                          int64_t x_ld, const int64_t* indptr, const int32_t* indices, const float* data, int64_t nnz,
+                          int64_t n_genes, float* out, int64_t block_rows, int32_t device, cudaStream_t s) {
   const bool csr = X == nullptr;
   if (csr == (indptr == nullptr)) return fail(TGB200_ERR_INVALID, "give exactly one of X (dense) and indptr (CSR)");
   if (rows <= 0 || cols <= 0 || ld < cols || n_genes <= 0 || rows > INT32_MAX || cols > INT32_MAX || n_genes > INT32_MAX - 64 ||
@@ -2175,7 +2079,6 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
     return fail(TGB200_ERR_INVALID, "block_rows=%lld is not a multiple of %lld", (long long)block_rows, (long long)kProjUnit);
   int n_sms = 0;
   CKS(use_sm90_device(device, &n_sms));
-  cudaStream_t s = (cudaStream_t)stream;
   // the row pointers are read on the host: every block's entry range is then known to lie inside [0, nnz)
   std::vector<int64_t> ip;
   if (csr) {
@@ -2194,10 +2097,10 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
     for (int64_t r0 = 0; csr && r0 < rows; r0 += B) m = std::max(m, ip[std::min(rows, r0 + B)] - ip[r0]);
     return m;
   };
-  // out, then per block: the mapping twice in fp32 (copy target, double-buffered) and once in three bf16 planes, X in three
-  // planes and, double-buffered, in fp32 (dense) or as the block's CSR entries
+  // out, then per block: the mapping in three bf16 planes and, from `map`, twice in fp32 (copy target, double-buffered), X in
+  // three planes and, double-buffered, in fp32 (dense) or as the block's CSR entries
   auto need = [&](int64_t B) {
-    double b = 4.0 * cols * ldx + 2 * 4.0 * B * ldm + 6.0 * B * ldm + 6.0 * B * ldx;
+    double b = 4.0 * cols * ldx + (h ? 0.0 : 2 * 4.0 * B * ldm) + 6.0 * B * ldm + 6.0 * B * ldx;
     return b + (csr ? 2 * (8.0 * max_nnz(B) + 8.0 * (B + 1)) : 2 * 4.0 * B * ldx);
   };
   size_t free_b = 0, total_b = 0;
@@ -2221,7 +2124,7 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
   CKS(bad.alloc(1, false));
   const int64_t block_nnz = max_nnz(B);
   for (int k = 0; k < 2; ++k) {
-    CKS(Mf[k].alloc((size_t)B * ldm, false));
+    if (!h) CKS(Mf[k].alloc((size_t)B * ldm, false));
     if (csr) {
       CKS(P[k].alloc(B + 1, false)); CKS(I[k].alloc(std::max<int64_t>(block_nnz, 1), false));
       CKS(D[k].alloc(std::max<int64_t>(block_nnz, 1), false));
@@ -2233,7 +2136,7 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
   // stream the caller passed: the flag starts at 0 and the staging's pad columns stay finite
   CK(cudaMemsetAsync(bad.p, 0, sizeof(int), s));
   for (int k = 0; k < 2; ++k) {
-    CK(cudaMemsetAsync(Mf[k].p, 0, sizeof(float) * Mf[k].n, s));
+    if (!h) CK(cudaMemsetAsync(Mf[k].p, 0, sizeof(float) * Mf[k].n, s));
     if (!csr) CK(cudaMemsetAsync(Xf[k].p, 0, sizeof(float) * Xf[k].n, s));
   }
   TcContext tc;
@@ -2255,12 +2158,11 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
     const int k = (int)(b & 1);
     const int64_t r0 = b * B, nb = std::min(B, rows - r0), nb64 = round_up(nb, 64);
     if (b >= 2) CK(cudaStreamWaitEvent(cp.s, cp.freed[k], 0));
-    if (nb < nb64) {                                           // the last k-block reads up to nb64 rows: zero the tail
-      CK(cudaMemsetAsync(Mf[k].p + nb * ldm, 0, sizeof(float) * (nb64 - nb) * ldm, cp.s));
-      if (!csr) CK(cudaMemsetAsync(Xf[k].p + nb * ldx, 0, sizeof(float) * (nb64 - nb) * ldx, cp.s));
-    }
-    CK(cudaMemcpy2DAsync(Mf[k].p, sizeof(float) * ldm, map + r0 * ld, sizeof(float) * ld, sizeof(float) * cols, nb,
-                         cudaMemcpyDefault, cp.s));
+    if (nb < nb64 && !csr)                                     // the last k-block reads up to nb64 rows: zero the tail
+      CK(cudaMemsetAsync(Xf[k].p + nb * ldx, 0, sizeof(float) * (nb64 - nb) * ldx, cp.s));
+    if (!h)
+      CK(cudaMemcpy2DAsync(Mf[k].p, sizeof(float) * ldm, map + r0 * ld, sizeof(float) * ld, sizeof(float) * cols, nb,
+                           cudaMemcpyDefault, cp.s));
     if (csr) {
       const int64_t e0 = ip[r0], ne = ip[r0 + nb] - e0;
       CK(cudaMemcpyAsync(P[k].p, ip.data() + r0, sizeof(int64_t) * (nb + 1), cudaMemcpyHostToDevice, cp.s));
@@ -2280,9 +2182,16 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
     const int k = (int)(b & 1);
     const int64_t r0 = b * B, nb = std::min(B, rows - r0), nb64 = round_up(nb, 64);
     CK(cudaStreamWaitEvent(s, cp.copied[k], 0));
-    const long long m4 = nb64 * ldm / 4;
-    k_split3<<<(unsigned)ceil_div(m4, 256), 256, 0, s>>>(Mf[k].p, Split3{Mp.p, (size_t)B * ldm}, m4);
-    CK(cudaGetLastError());
+    const Split3 mp{Mp.p, (size_t)B * ldm};
+    if (h) {
+      CKS(launch_softmax_rows<float>(h, s, (float*)nullptr, 0, nullptr, mp, (int)r0, (int)nb));     // ldm == h->ld
+    } else {
+      const long long m4 = nb * ldm / 4;
+      k_split3<<<(unsigned)ceil_div(m4, 256), 256, 0, s>>>(Mf[k].p, mp, m4);
+      CK(cudaGetLastError());
+    }
+    if (nb < nb64)                                             // the last k-block reads up to nb64 rows: zero the tail
+      for (int p = 0; p < 3; ++p) CK(cudaMemsetAsync(Mp.p + ((size_t)p * B + nb) * ldm, 0, 2 * (nb64 - nb) * ldm, s));
     if (csr) {
       const CsrSplitArgs a{P[k].p, I[k].p, D[k].p, (int)nb, (int)nb64, (int)n_genes, (int)ldx, Split3{Xp.p, (size_t)B * ldx}, bad.p};
       k_csr_split3<<<(unsigned)ceil_div(nb64 * kWarp, kProjThreads), kProjThreads, 0, s>>>(a);
@@ -2308,4 +2217,20 @@ extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
                        cudaMemcpyDefault, s));
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
+}
+
+extern "C" int tgb200_project_map(const float* map, int64_t rows, int64_t cols, int64_t ld, const float* X, int64_t x_ld,
+                                  const int64_t* indptr, const int32_t* indices, const float* data, int64_t nnz,
+                                  int64_t n_genes, float* out, int64_t block_rows, int32_t device, void* stream) {
+  if (!map || !out) return fail(TGB200_ERR_INVALID, "null argument");
+  return project_blocks(nullptr, map, rows, cols, ld, X, x_ld, indptr, indices, data, nnz, n_genes, out, block_rows, device,
+                        (cudaStream_t)stream);
+}
+
+// softmax(M)^T X (tangram/utils.py:368) from the handle's M, X dense
+extern "C" int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, float* out, void* stream) {
+  if (!h || !X || !out || n_cols <= 0) return fail(TGB200_ERR_INVALID, "bad argument");
+  if (!h->have_mapping) return fail(TGB200_ERR_STATE, "no mapping set");
+  return project_blocks(h, nullptr, h->N, h->V, h->ld, X, n_cols, nullptr, nullptr, nullptr, 0, n_cols, out, 0, h->cfg.device,
+                        (cudaStream_t)stream);
 }

@@ -198,7 +198,8 @@ class Engine:
         return out
 
     def project(self, X, out, stream=None):
-        """out (voxels x n_cols, f32) = softmax(M)^T X; X is (cells x n_cols) f32, host or device memory."""
+        """out (voxels x n_cols, f32) = softmax(M)^T X; X is (cells x n_cols) f32, host or device memory.  The same bits as
+        utils.project(get_mapping(), X), in every precision."""
         n_cols = int(X.shape[1])
         _lib.check(self._lib.tgb200_project(self._h, _lib.ptr(X), n_cols, _lib.ptr(out), self._s(stream)))
         return out

@@ -162,7 +162,8 @@ class _EngineMapper:
 
     def project(self, X, out=None):
         """softmax(M)^T @ X on the device (project_genes' GEMM, tangram/utils.py:368) -> (n_voxels, n_cols) float32
-        ndarray; or, with `out` (a contiguous float32 CUDA tensor of that shape on this mapper's device), written there."""
+        ndarray; or, with `out` (a contiguous float32 CUDA tensor of that shape on this mapper's device), written there.
+        Bit for bit what `tangram_b200.utils.project` gives for the mapping this mapper returns."""
         X = np.ascontiguousarray(X, dtype=np.float32)
         if X.shape[0] != self.n_cells:
             raise ValueError("X must have one row per cell")

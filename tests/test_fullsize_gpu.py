@@ -136,7 +136,7 @@ def test_full_size_against_oracle(name):
         torch.cuda.empty_cache()
 
     if name == "c3":
-        # project_genes' GEMM at full size on the device (two column chunks, the second ragged): tensor-core
+        # project_genes' GEMM at full size on the device (cell blocks, 512-cell chains, 2304 genes): tensor-core
         # split-bf16 path vs float64 on the voxel sample
         eng = _engine(name, "bf16", wl)
         Pm = torch.empty((N, V), dtype=torch.float32, device="cuda")

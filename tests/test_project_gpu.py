@@ -123,6 +123,33 @@ def test_staging_does_not_change_a_bit():
     assert np.array_equal(out_h.numpy(), ref), "host CSR, host out"
 
 
+@pytest.mark.parametrize("precision,chunks", [("fp32", None), ("bf16x3", None), ("bf16", None), ("bf16", "2")])
+def test_mapper_project_equals_project_of_its_mapping(precision, chunks, monkeypatch):
+    """Mapper.project (tgb200_project: the row pass writes each block's planes from M) is `project` of the mapping
+    get_mapping returns, bit for bit, after training steps: three 2048-cell blocks, the last one ragged, V ragged, more
+    than 2048 genes, into host and device out.  bf16 with two cell chunks projects while P holds the update's state."""
+    import torch
+    from oracle.tangram_oracle import synthetic_inputs
+    from tangram_b200 import Mapper, utils
+    if chunks:
+        monkeypatch.setenv("TGB200_CHUNKS", chunks)
+    N, V, K = 6000, 333, 40
+    inp = synthetic_inputs(N, V, K, seed=21)
+    M0 = np.random.default_rng(22).standard_normal((N, V)).astype(np.float32)
+    m = Mapper(S=inp["S"], G=inp["G"], d=inp["d"], lambda_d=1.0, M0=M0, precision=precision, device="cuda:0")
+    if chunks:
+        assert int(m._engine.debug("shape")[4]) == int(chunks)
+    m.train(3, print_each=None)
+    P = m._engine.get_mapping(np.empty((N, V), dtype=np.float32))
+    X = np.random.default_rng(23).random((N, 2048 + 77)).astype(np.float32)
+    ref = utils.project(P, X)
+    _check(ref, P, X)
+    assert np.array_equal(m.project(X), ref), "host out"
+    out = torch.empty((V, X.shape[1]), dtype=torch.float32, device="cuda:0")
+    m.project(X, out=out)
+    assert np.array_equal(out.cpu().numpy(), ref), "device out"
+
+
 def test_default_blocks_larger_than_2048_equal_forced_2048():
     """20000 cells: the default block is 4096 cells (five blocks); forced 2048-cell blocks (ten) give the same bits."""
     from tangram_b200 import utils

@@ -142,9 +142,9 @@ def test_degenerate_and_off_tile_shapes(shape, precision):
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16x3", "bf16"])
 def test_project_multi_chunk_matches_float64(precision):
-    """tgb200_project (project_genes' GEMM, tangram/utils.py:368): more gene columns than one 2048-wide chunk, ragged
-    tail, after a few training steps; every mode returns fp32-grade softmax(M)^T X (the tensor-core modes use the
-    split-bf16 forward kernel), and training continues unperturbed afterwards."""
+    """tgb200_project (project_genes' GEMM, tangram/utils.py:368): more than 2048 gene columns, ragged, after a few
+    training steps; every mode returns fp32-grade softmax(M)^T X (split-bf16 operands on the forward kernel), and training
+    continues unperturbed afterwards."""
     from tangram_b200 import Mapper
     N, V, K = 2500, 333, 90
     inp = synthetic_inputs(N, V, K, seed=17)
