@@ -6,7 +6,8 @@
 //   backward  dP = S_ext dY_ext^T  -> stored (bf16 centred / fp32) + row-dot partials in the epilogue (A, B K-major).
 //             The update itself is a streaming kernel (adam_rows.cuh).
 //
-// Persistent, warp-specialised kernel: one CTA per SM loops over 128 x 256 output tiles.
+// Persistent, warp-specialised kernel: one CTA per SM, in clusters of two that loop over pairs of 128 x 256 output tiles
+// sharing their B tile (each CTA loads half of it and multicasts it to both).
 //   warpgroup 0     TMA producer (one thread): keeps the operand ring full across tile boundaries, so the loads of
 //                   tile i+1 run while the consumers drain tile i
 //   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the tile, m64n256k16 wgmma into 128 fp32 registers per
@@ -49,6 +50,24 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (this CTA included).  It only
+// says that this thread's reads of a stage are done (wgmma.wait_group has retired them); the writes it allows are the
+// peer's TMA, so no cluster-scope release fence is needed (that would be a MEMBAR.GPU per k-block).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(cta) : "memory");
+}
+// cluster coordinates, read where they are used (asm volatile: not held in a register across the loops)
+__device__ __forceinline__ int cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return (int)r; }
+__device__ __forceinline__ int cluster_index() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return (int)r; }
+__device__ __forceinline__ int cluster_count() { uint32_t r; asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r)); return (int)r; }
+// every thread of every CTA of the cluster; orders the shared-memory writes before it (barrier init) cluster-wide
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 
 // L2 policy: operand tiles are re-read by many CTAs -> evict_last (CUTLASS TMA::CacheHintSm90::EVICT_LAST)
 constexpr uint64_t kPolicyEvictNormal = 0x1000000000000000ull;
@@ -59,6 +78,13 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy) : "memory");
+}
+// the same box written to `dst` and signalled on `bar` at the same offsets in both CTAs of the cluster
+__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
+      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"((uint16_t)0x3), "l"(policy) : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
@@ -163,6 +189,19 @@ struct OperandTile {
     } else {
 #pragma unroll
       for (int b = 0; b < ROWS / 64; ++b) tma_load_2d(map, bar, dst + b * 8192, mn0 + b * 64, k0, policy);  // box {64 mn, 64 k}
+    }
+  }
+  // MN rows [h ROWS/2, (h + 1) ROWS/2) of the tile, multicast to both CTAs of the cluster: in either layout they are the
+  // 16 KB starting h ROWS/2 * 128 B in
+  static __device__ __forceinline__ void load_half_pair(const CUtensorMap* map, uint64_t* bar, uint8_t* dst, int mn0, int k0, int h,
+                                                        uint64_t policy) {
+    constexpr int HALF = ROWS / 2;
+    if (KMAJOR) {
+      tma_load_2d_pair(map, bar, dst + h * HALF * 128, k0, mn0 + h * HALF, policy);         // box {64 k, ROWS/2 mn}
+    } else {
+#pragma unroll
+      for (int b = 0; b < HALF / 64; ++b)
+        tma_load_2d_pair(map, bar, dst + h * HALF * 128 + b * 8192, mn0 + h * HALF + b * 64, k0, policy);
     }
   }
   static __device__ __forceinline__ uint64_t desc(uint32_t saddr, int k_step /* 0..3 */) {
@@ -385,8 +424,13 @@ __device__ __constant__ int kPairA[6] = {2, 0, 1, 1, 0, 0};
 __device__ __constant__ int kPairB[6] = {0, 2, 1, 0, 1, 0};
 
 // ---- the kernel -------------------------------------------------------------------------------
-// Work item w -> (split z, row tile, column tile), column tile fastest so that CTAs running at the
-// same time share A rows and stream B through L2.
+// Launched as clusters of two CTAs.  Work item w -> (split z, pair of row tiles (2i, 2i + 1), column tile), column tile
+// fastest so that clusters running at the same time share A rows and stream B through L2; the CTA of cluster rank r
+// computes row tile 2i + r.  Both tiles need the same B tile: each CTA's producer loads its own A and one half of B, and
+// multicasts that half into both CTAs' stages, so a stage reaches each CTA's full barrier as one A + two B halves, and
+// it is refilled only once the consumers of both CTAs have released it (each consumer warp arrives on both CTAs' empty
+// barriers).  With an odd number of row tiles the last pairs have a phantom second tile: that CTA loads no A, stores
+// nothing and skips its epilogue, but loads and multicasts its half of B and takes part in every barrier.
 template <bool A_KMAJOR, bool B_KMAJOR, int STAGES, class Epi>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps maps_b, int n_pairs,
@@ -405,30 +449,33 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
   __shared__ __align__(8) uint64_t epi_full[2], epi_free[2];
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
-  const int total = tiles_m * tiles_n * splits;
+  const int tiles_mp = (tiles_m + 1) / 2;                 // row-tile pairs
+  const int total = tiles_mp * tiles_n * splits;
   EpiSmem es{smem + STAGES * kStageBytes, epi_full, epi_free, 0};
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps_a.m[0]);
     tma_prefetch_desc(&maps_b.m[0]);
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2 * kConsumerWarps); }
     if constexpr (Epi::kSmemBytes > 0) {
       for (int h = 0; h < 2; ++h) { mbar_init(&epi_full[h], 1); mbar_init(&epi_free[h], 1); }
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  cluster_sync();                               // the peer's barriers are initialised before the first multicast
 
   if (wg == 0) {
     // ===== TMA producer =====
     setmaxnreg_producer();
     if (threadIdx.x == 0) {
       uint32_t kbg = 0;                         // k-blocks issued so far (ring position)
-      for (int w = blockIdx.x; w < total; w += gridDim.x, es.parity ^= 1) {
-        const int z = w / (tiles_n * tiles_m);
-        int tm_i, tn_i;
-        tile_mn(w - z * tiles_n * tiles_m, tiles_m, tiles_n, group_m, tm_i, tn_i);
+      for (int w = cluster_index(); w < total; w += cluster_count()) {
+        const int z = w / (tiles_n * tiles_mp);
+        int tp_i, tn_i;
+        tile_mn(w - z * tiles_n * tiles_mp, tiles_mp, tiles_n, group_m, tp_i, tn_i);
+        const int tm_i = 2 * tp_i + cluster_rank();
+        const bool live = tm_i < tiles_m;
         const int n0 = tn_i * TC_BN, m0 = (tm_off + tm_i) * TC_BM;
         const int k_begin = k_off + z * k_per_split;
         const int k_end = min(k_total, k_begin + k_per_split);
@@ -436,22 +483,24 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
         for (int pr = 6 - n_pairs; pr < 6; ++pr) {
           const CUtensorMap* ma = &maps_a.m[kPairA[pr]];
           const CUtensorMap* mb = &maps_b.m[kPairB[pr]];
+#pragma unroll 1   // unrolled, the multicast loads do not fit the producer's 40 registers
           for (int kb = 0; kb < num_kb; ++kb, ++kbg) {
             const int s = kbg % STAGES;
             const uint32_t ph = (kbg / STAGES) & 1;
             mbar_wait(&empty_bar[s], ph ^ 1);
             uint8_t* sa = smem + s * kStageBytes;
             uint8_t* sb = sa + TileA::kBytes;
-            mbar_expect_tx(&full_bar[s], kStageBytes);
+            mbar_expect_tx(&full_bar[s], live ? kStageBytes : TileB::kBytes);
             const int k0 = k_begin + kb * TC_BK;
-            TileA::load(ma, &full_bar[s], sa, m0, k0, policy_a);
-            TileB::load(mb, &full_bar[s], sb, n0, k0, policy_b);
+            if (live) TileA::load(ma, &full_bar[s], sa, m0, k0, policy_a);
+            TileB::load_half_pair(mb, &full_bar[s], sb, n0, k0, cluster_rank(), policy_b);
 #ifndef TGB_SKIP_EPI
             // not before: waiting for the previous tile's epilogue to free its buffer would hold up the ring's prefill
-            if (Epi::kSmemBytes > 0 && pr == 6 - n_pairs && kb + 1 == min(STAGES, num_kb)) epi.load(m0, n0, es);
+            if (Epi::kSmemBytes > 0 && live && pr == 6 - n_pairs && kb + 1 == min(STAGES, num_kb)) epi.load(m0, n0, es);
 #endif
           }
         }
+        if (live) es.parity ^= 1;
       }
     }
   } else {
@@ -464,21 +513,23 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
 #pragma unroll
     for (int i = 0; i < TC_ACC; ++i) acc[i] = 0.f;
     uint32_t kbg = 0;
-    for (int w = blockIdx.x; w < total; w += gridDim.x, es.parity ^= 1) {
+    for (int w = cluster_index(); w < total; w += cluster_count()) {
       TileCoord t;
-      t.split = w / (tiles_n * tiles_m);
-      int tm_i;
-      tile_mn(w - t.split * tiles_n * tiles_m, tiles_m, tiles_n, group_m, tm_i, t.tile_n);
+      t.split = w / (tiles_n * tiles_mp);
+      int tp_i;
+      tile_mn(w - t.split * tiles_n * tiles_mp, tiles_mp, tiles_n, group_m, tp_i, t.tile_n);
       t.tiles_n = tiles_n;
       t.n0 = t.tile_n * TC_BN;
-      t.m0 = (tm_off + tm_i) * TC_BM;
+      t.m0 = (tm_off + 2 * tp_i + cluster_rank()) * TC_BM;
+      const bool live = t.m0 < (tm_off + tiles_m) * TC_BM;
       const int k_begin = k_off + t.split * k_per_split;
       const int k_end = min(k_total, k_begin + k_per_split);
       const int total_kb = (k_end - k_begin + TC_BK - 1) / TC_BK * n_pairs;
 #ifndef TGB_SKIP_EPI
-      epi.prologue(t, ct);
+      if (live) epi.prologue(t, ct);
 #endif
       acc_fence(acc);
+      // a phantom tile runs its MMAs on a stale A: the stages are released on the same schedule in both CTAs
       for (int kb = 0; kb < total_kb; ++kb, ++kbg) {
         const int s = kbg % STAGES;
         const uint32_t ph = (kbg / STAGES) & 1;
@@ -491,16 +542,20 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
           wgmma_m64n256k16<kTA, kTB>(acc, TileA::desc(sa, k), TileB::desc(sb, k), (kb > 0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();                        // the MMAs of the previous k-block have retired: release its stage
-        if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(kbg - 1) % STAGES]);
+        if (kb > 0 && lane < 2) mbar_arrive_cluster(&empty_bar[(kbg - 1) % STAGES], lane);
       }
       wgmma_wait<0>();
       acc_fence(acc);
-      if (total_kb > 0 && lane == 0) mbar_arrive(&empty_bar[(kbg - 1) % STAGES]);
+      if (total_kb > 0 && lane < 2) mbar_arrive_cluster(&empty_bar[(kbg - 1) % STAGES], lane);
 #ifndef TGB_SKIP_EPI
-      epi.run(acc, t, t.m0 + row_in_tile, lane, cw, es);
+      if (t.m0 < (tm_off + tiles_m) * TC_BM) {   // live, recomputed: the accumulators leave no register to keep it in
+        epi.run(acc, t, t.m0 + row_in_tile, lane, cw, es);
+        es.parity ^= 1;
+      }
 #endif
     }
   }
+  cluster_sync();                               // no CTA leaves while its peer may still arrive on its barriers
 }
 
 // ---- host side --------------------------------------------------------------------------------
@@ -513,6 +568,7 @@ struct TcContext {
   int num_sms = 132;
   const void* smem_fn[16] = {};   // kernels whose dynamic shared-memory limit this handle has already raised
   int smem_bytes[16] = {};
+  int clusters[16] = {};          // ... and how many of their 2-CTA clusters fit on the device at once
 };
 
 static inline int tc_init(TcContext& tc, char* err, size_t n) {
@@ -548,22 +604,46 @@ static inline int tc_make_map(TcContext& tc, CUtensorMap* map, const void* base,
   return 0;
 }
 
-// cudaFuncSetAttribute once per (handle, kernel): it is a driver call, not something to repeat on every launch
-template <class Kern>
-static inline int tc_set_smem(TcContext& tc, Kern kern, int bytes, char* err, size_t n) {
+// Launches k_gemm_tc as a persistent grid of 2-CTA clusters over `pairs` work items (pairs of row tiles x column tiles x
+// splits): at most as many clusters as can be resident at once, which on H100 may leave some SMs idle (the GPCs do not
+// all hold an even number of SMs that a cluster can use).  cudaFuncSetAttribute and the occupancy query are driver calls:
+// they run once per (handle, kernel), not on every launch.
+template <class Kern, class... Args>
+static inline int tc_launch(TcContext& tc, Kern kern, int smem, long long pairs, cudaStream_t s, const char* name, char* err,
+                            size_t n, Args... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = (size_t)smem;
+  cfg.stream = s;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
   const void* key = reinterpret_cast<const void*>(kern);
   int slot = -1;
   for (int i = 0; i < 16; ++i) {
-    if (tc.smem_fn[i] == key) { if (tc.smem_bytes[i] == bytes) return 0; slot = i; break; }
+    if (tc.smem_fn[i] == key) { slot = i; break; }
     if (tc.smem_fn[i] == nullptr && slot < 0) slot = i;
   }
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) { snprintf(err, n, "cudaFuncSetAttribute(smem=%d): %s", bytes, cudaGetErrorString(e)); return -2; }
-  if (slot >= 0) { tc.smem_fn[slot] = key; tc.smem_bytes[slot] = bytes; }
-  return 0;
-}
-static inline int tc_check_launch(const char* name, char* err, size_t n) {
-  cudaError_t e = cudaGetLastError();
+  if (slot < 0) { snprintf(err, n, "launch %s: more than 16 tensor-core kernels", name); return -2; }
+  if (tc.smem_fn[slot] != key || tc.smem_bytes[slot] != smem) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) { snprintf(err, n, "cudaFuncSetAttribute(smem=%d): %s", smem, cudaGetErrorString(e)); return -2; }
+    cfg.gridDim = dim3(2);
+    int c = 0;
+    e = cudaOccupancyMaxActiveClusters(&c, kern, &cfg);
+    if (e != cudaSuccess || c < 1) {
+      snprintf(err, n, "launch %s: no 2-CTA cluster with %d B of shared memory fits (%s)", name, smem, cudaGetErrorString(e));
+      return -2;
+    }
+    tc.smem_fn[slot] = key; tc.smem_bytes[slot] = smem; tc.clusters[slot] = c;
+  }
+  cfg.gridDim = dim3((unsigned)(2 * (pairs < tc.clusters[slot] ? pairs : tc.clusters[slot])));
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
+  if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { snprintf(err, n, "launch %s: %s", name, cudaGetErrorString(e)); return -2; }
   return 0;
 }
@@ -607,9 +687,8 @@ static inline int tc_forward_splits(int num_sms, int N, int V, int Ke) {
 static inline int tc_kps(int k_total, int splits) {
   return (int)(round_up(ceil_div(k_total, splits), TC_BK));
 }
-static inline unsigned tc_grid(const TcContext& tc, long long total) {
-  return (unsigned)(total < tc.num_sms ? total : tc.num_sms);
-}
+// work items of one launch: pairs of row tiles x column tiles x splits
+static inline long long tc_pairs(int tiles_m, int tiles_n, int splits) { return (long long)(tiles_m + 1) / 2 * tiles_n * splits; }
 
 // Operand planes: plane p of an operand starts at base + p * plane_elems (bf16).  n_pairs = 1 uses plane 0 only.
 static inline int tc_make_maps(TcContext& tc, TcMaps* maps, const __nv_bfloat16* base, size_t plane_elems, int n_planes,
@@ -640,12 +719,10 @@ static inline int tc_forward_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16
 static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int N, int V, int Ke, int splits,
                                     cudaStream_t s, char* err, size_t n) {
   auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
-  if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, 0};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
-  kern<<<tc_grid(tc, (long long)tm * tn * splits), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, N, tc_kps(N, splits), tm, tn,
-                                                                             splits, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, 0, epi);
-  return tc_check_launch("tc_gemm_fwd", err, n);
+  return tc_launch(tc, kern, TC_SMEM, tc_pairs(tm, tn, splits), s, "tc_gemm_fwd", err, n, pl.a, pl.b, n_pairs, N, tc_kps(N, splits),
+                   tm, tn, splits, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, 0, epi);
 }
 // cells [row0, row1) only (row0 a multiple of 64): `out` = or += this chunk's partial sum -- the host pipelines cell chunks
 // behind the streaming Adam kernel (and the projection adds its 512-cell chains); the chunks run one after the other
@@ -653,12 +730,10 @@ static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs
 static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int accumulate, int row0, int row1,
                                          int V, int Ke, cudaStream_t s, char* err, size_t n) {
   auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
-  if (tc_set_smem(tc, kern, TC_SMEM, err, n)) return -2;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, accumulate};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
-  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, TC_SMEM, s>>>(pl.a, pl.b, n_pairs, row1, (int)round_up(row1 - row0, TC_BK), tm, tn,
-                                                                    1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
-  return tc_check_launch("tc_gemm_fwd", err, n);
+  return tc_launch(tc, kern, TC_SMEM, tc_pairs(tm, tn, 1), s, "tc_gemm_fwd", err, n, pl.a, pl.b, n_pairs, row1,
+                   (int)round_up(row1 - row0, TC_BK), tm, tn, 1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
 }
 
 // Staged backward: dq = bf16(S_ext dY_ext^T - centre) (bf16 mode) or dP in fp32 (bf16x3 mode, three operand planes, six
@@ -667,7 +742,7 @@ static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, int n_
 static inline int tc_dpstore_plan(TcContext& tc, TcPlan& pl, const __nv_bfloat16* Sxb, size_t s_plane, const __nv_bfloat16* dYb,
                                   size_t dy_plane, int planes, int N, int V, int Ke, char* err, size_t n) {
   if (tc_make_maps(tc, &pl.a, Sxb, s_plane, planes, Ke, N, Ke, 64, TC_BM, err, n)) return -2;
-  if (tc_make_maps(tc, &pl.b, dYb, dy_plane, planes, Ke, V, Ke, 64, TC_BN, err, n)) return -2;
+  if (tc_make_maps(tc, &pl.b, dYb, dy_plane, planes, Ke, V, Ke, 64, TC_BN / 2, err, n)) return -2;   // one half of a B tile
   pl.ready = true;
   return 0;
 }
@@ -683,11 +758,9 @@ static inline int tc_dpstore_launch(TcContext& tc, const TcPlan& pl, int n_pairs
   const int tn = (int)ceil_div(V, TC_BN);
   auto kern = k_gemm_tc<true, true, tc_stages<Epi>(), Epi>;
   constexpr int smem = tc_smem<Epi>();
-  if (tc_set_smem(tc, kern, smem, err, n)) return -2;
   const int tm0 = row0 / TC_BM, tm = (int)ceil_div(row1, TC_BM) - tm0;
-  kern<<<tc_grid(tc, (long long)tm * tn), TC_THREADS, smem, s>>>(pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
-                                                                 kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
-  return tc_check_launch("tc_gemm_bwd_dp", err, n);
+  return tc_launch(tc, kern, smem, tc_pairs(tm, tn, 1), s, "tc_gemm_bwd_dp", err, n, pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
+                   kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
 }
 
 }  // namespace tgb
