@@ -356,8 +356,12 @@ TGB200_API int tgb200_algorithmic_cost(tgb200_mapper* h, double* hbm_bytes, doub
 TGB200_API int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* out_host, int64_t cap, int64_t* n);
 
 /* Diagnostics: enable != 0 starts recording a CUDA event after every launch on the stream it went to; enable == 0 stops
- * and returns, per launch, its name, stream (0 caller, 1 the handle's contraction stream, 2 its update stream) and
- * completion time in ms relative to the first one -- the only way to see the two-stream pipeline without a tracer. */
+ * and returns, per launch, its name, stream and completion time in ms relative to the first one -- the only way to see
+ * the bf16 chunk pipeline without a tracer.  Streams 1-3 exist only on a bf16 handle with several cell chunks:
+ *   0  the caller's stream (every launch of any other handle, and of tgb200_profile_step)
+ *   1  the handle's contraction stream: forward, loss stage, backward contractions
+ *   2  its update stream: row-dot finalize and the streaming Adam kernel
+ *   3  the stream on which tgb200_run issues the next iteration's forward chunks during the backward */
 TGB200_API int tgb200_debug_timeline(tgb200_mapper* h, int32_t enable, const char** names, int32_t* streams, float* end_ms,
                                      int32_t cap, int32_t* n);
 

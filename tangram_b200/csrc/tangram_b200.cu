@@ -83,7 +83,8 @@ enum class PState {
   updated,                      // exp(Mnew - lse) from the streaming update; k_row_norm normalises it
 };
 
-// one launch while recording is on (tgb200_profile_step / tgb200_debug_timeline): stream 0 caller, 1 hi, 2 lo, 3 sf
+// one launch while recording is on (tgb200_profile_step / tgb200_debug_timeline): stream 1 hi, 2 lo, 3 sf of a handle
+// with streams, 0 any other (the caller's)
 struct LaunchRecord {
   const char* name;
   int stream;
@@ -144,7 +145,6 @@ struct tgb200_mapper {
   int val_every = 0;
   int64_t val_epoch = 0;
   int64_t val_row = -1;         // fp32 / bf16x3: the row whose validation this iteration's forward computes (see loss_stage)
-  bool val_fuse = false;        // tgb200_run, not its last iteration: a validation may wait for the next iteration's forward
   DevBuf<float> val_coef, val_rowpart, val_hist;   // what the validation's k_loss_scalars writes beside its four values
   // history
   DevBuf<float> hist;
@@ -167,22 +167,20 @@ struct tgb200_mapper {
   DevBuf<float> rcenter;        // per row: last iteration's row-dot, the centre dq is stored relative to
   // the same staging for the parity mode (bf16x3): dP in fp32, exact streaming update (no chunk pipeline)
   DevBuf<float> dpf;            // N x ld
-  // Pipelining of the bf16 backward over cell chunks (rows [chunk_row[c], chunk_row[c+1]), multiples of 256):
+  // Pipelining of the bf16 backward over cell chunks (rows [chunk_row[c], chunk_row[c+1]), multiples of 256; {0, N} with
+  // one chunk):
   //   hi (high-priority stream): forward(c) ... loss ... backward contraction(c)        -- tensor-core bound
   //   lo (low-priority stream):  row-dot finalize(c), streaming Adam(c)                 -- HBM bound
   // Adam(c) runs under the contraction of chunk c+1 and, across the iteration boundary, under the next forward's
-  // chunks; forward(c) of the next iteration waits only for Adam(c).  The caller's stream forks into hi at the
-  // start of an API call and joins hi + lo at its end (tgb200_run joins once, after its last iteration).
-  bool pipelined = false;
+  // chunks; forward(c) of the next iteration waits only for Adam(c).  Which stream a launch goes to is the Lanes of its
+  // API call (below).
+  bool pipelined = false;       // several chunks: the handle has the streams hi, lo and sf
   int nchunks = 1, chunk_row[9] = {0};
   cudaStream_t hi = nullptr, lo = nullptr, sf = nullptr;     // sf: the NEXT iteration's forward chunks (see backward_bf16)
   cudaEvent_t ev_fork = nullptr, ev_join_hi = nullptr, ev_join_lo = nullptr, ev_join_sf = nullptr, ev_loss = nullptr;
   cudaEvent_t ev_g[8] = {}, ev_a[8] = {}, ev_f[8] = {};
-  bool a_valid = false;         // ev_a[] were recorded by an earlier step_end and guard the rows of the next forward
-  bool prefetch_next = false;   // tgb200_run, not its last iteration: issue the NEXT forward's chunks between this backward's chunks
-  bool fwd_ahead = false;       // ... and they have been issued: the next step_begin skips its chunk loop
-  bool defer_join = false;      // inside tgb200_run: no fork / join between its iterations
-  bool serial = false;          // tgb200_profile_step: everything on the caller's stream, one kernel at a time
+  bool a_valid = false;         // ev_a[] were recorded by an earlier two-stream update and guard the rows of the next forward
+  bool fwd_ahead = false;       // the previous backward issued this iteration's forward chunks on sf: the forward only waits
   // diagnostics: an event after every launch while recording is on
   bool recording = false;
   std::vector<LaunchRecord> records;
@@ -224,7 +222,8 @@ static void mark(tgb200_mapper* h, cudaStream_t s, const char* name) {
   cudaEvent_t e;
   cudaEventCreate(&e);
   cudaEventRecord(e, s);
-  h->records.push_back({name, s == h->hi ? 1 : (s == h->lo ? 2 : (s == h->sf ? 3 : 0)), e});
+  // without streams, hi == lo == sf == nullptr: the legacy default stream, which a caller may pass
+  h->records.push_back({name, !h->pipelined ? 0 : s == h->hi ? 1 : s == h->lo ? 2 : s == h->sf ? 3 : 0, e});
 }
 #define LAUNCH_CHECK(name)                                                                  \
   do {                                                                                      \
@@ -341,18 +340,21 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   A(h->G.alloc(vk));
   A(h->d.alloc(h->V)); A(h->dsrc.alloc(h->N));
   A(h->stats.alloc(h->N)); A(h->rowaux.alloc((size_t)2 * h->N)); A(h->rdot.alloc(h->N));
+  int nc = 1;
   if (h->bf16) {
     // cell chunks of the pipelined backward: 4 from 32k cells up, 2 from 8k (a rank of an 8-way sharded 100k-cell run):
     // each chunk still fills the GPU several times over
-    int nc = h->N >= 32768 ? 4 : (h->N >= 8192 ? 2 : 1);
+    nc = h->N >= 32768 ? 4 : (h->N >= 8192 ? 2 : 1);
     if (const char* e = getenv("TGB200_CHUNKS")) nc = atoi(e);
     if (nc < 1) nc = 1;
     if (nc > 8) nc = 8;
-    if (h->constrained) nc = 1;              // the filter update couples all rows of an iteration
+    // The filter update couples all rows of an iteration.  So a constrained handle has one chunk and no streams, and
+    // its next k_filter_prepare follows the filter update on the same stream without waiting for an event.
+    if (h->constrained) nc = 1;
     while (nc > 1 && h->N / nc < 1024) --nc;
-    h->nchunks = nc;
-    for (int c = 0; c <= nc; ++c) h->chunk_row[c] = c == nc ? h->N : (int)round_up((int64_t)c * h->N / nc, 256);
   }
+  h->nchunks = nc;
+  for (int c = 0; c <= nc; ++c) h->chunk_row[c] = c == nc ? h->N : (int)round_up((int64_t)c * h->N / nc, 256);
   if (h->nchunks > 1) {                      // one chunk: nothing to overlap, everything stays on the caller's stream
     int lo_p = 0, hi_p = 0;
     cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p);
@@ -1033,37 +1035,48 @@ static int check_ready(tgb200_mapper* h) {
   return TGB200_OK;
 }
 
-// Streams of an API call: the caller's stream `s` forks into the handle's high-priority stream (which in turn feeds the
-// low-priority one through per-chunk events) and joins both at the end.
-static cudaStream_t work_stream(tgb200_mapper* h, cudaStream_t s) { return (h->pipelined && !h->serial) ? h->hi : s; }
-static cudaStream_t update_stream(tgb200_mapper* h, cudaStream_t s) { return (h->pipelined && !h->serial) ? h->lo : s; }
-static int fork_streams(tgb200_mapper* h, cudaStream_t s) {
-  if (!h->pipelined || h->serial || h->defer_join) return TGB200_OK;
-  CK(cudaEventRecord(h->ev_fork, s));
-  CK(cudaStreamWaitEvent(h->hi, h->ev_fork, 0));
+// The streams of one API call, chosen once at its start.  On a handle with streams the caller's stream forks into `work`
+// (hi: forward, loss, backward contractions), which feeds `update` (lo: row-dot finalize, streaming Adam) and `ahead`
+// (sf: the next iteration's forward chunks) through per-chunk events, and all three join the caller's stream at the end.
+// Otherwise, and in tgb200_profile_step, every lane is the caller's stream.
+struct Lanes { cudaStream_t caller, work, update, ahead; };
+static Lanes lanes_of(const tgb200_mapper* h, cudaStream_t s) {
+  return h->pipelined ? Lanes{s, h->hi, h->lo, h->sf} : Lanes{s, s, s, s};
+}
+static int fork_streams(tgb200_mapper* h, const Lanes& L) {
+  if (L.work == L.caller) return TGB200_OK;
+  CK(cudaEventRecord(h->ev_fork, L.caller));
+  CK(cudaStreamWaitEvent(L.work, h->ev_fork, 0));
   return TGB200_OK;
 }
-static int join_streams(tgb200_mapper* h, cudaStream_t s) {
-  if (!h->pipelined || h->serial || h->defer_join) return TGB200_OK;
-  CK(cudaEventRecord(h->ev_join_hi, h->hi));
-  CK(cudaStreamWaitEvent(s, h->ev_join_hi, 0));
-  CK(cudaEventRecord(h->ev_join_lo, h->lo));
-  CK(cudaStreamWaitEvent(s, h->ev_join_lo, 0));
-  CK(cudaEventRecord(h->ev_join_sf, h->sf));
-  CK(cudaStreamWaitEvent(s, h->ev_join_sf, 0));
+static int join_streams(tgb200_mapper* h, const Lanes& L) {
+  if (L.work == L.caller) return TGB200_OK;
+  CK(cudaEventRecord(h->ev_join_hi, L.work));
+  CK(cudaStreamWaitEvent(L.caller, h->ev_join_hi, 0));
+  CK(cudaEventRecord(h->ev_join_lo, L.update));
+  CK(cudaStreamWaitEvent(L.caller, h->ev_join_lo, 0));
+  CK(cudaEventRecord(h->ev_join_sf, L.ahead));
+  CK(cudaStreamWaitEvent(L.caller, h->ev_join_sf, 0));
   return TGB200_OK;
+}
+
+// the tensor maps of the forward contraction, encoded on first use (the buffers never move)
+static int forward_plan(tgb200_mapper* h) {
+  if (h->plan_fwd.ready) return TGB200_OK;
+  const __nv_bfloat16* sB = h->bf16 ? h->Sxs.p : h->Sxb.p;
+  return tc_forward_plan(h->tc, h->plan_fwd, h->Pb.p, (size_t)h->N * h->ld, sB, (size_t)h->N * h->Ke, h->x3 ? 3 : 1, h->N, h->V,
+                         h->Ke, h->ld, g_err, sizeof(g_err));
 }
 
 // bf16 mode, cells of chunk c: exact row statistics from the sums the update left (k_row_norm), the scaled forward operand,
 // and -- when the forward is chunked -- this chunk's contribution to Y_ext.  `lseA` / `lseT` as they are for THAT forward.
 static int forward_chunk(tgb200_mapper* h, cudaStream_t s, int c, int fresh, const float* lseA, float* lseT) {
   float* rowaux = needs_rowaux(h->cfg) ? h->rowaux.p : nullptr;
-  if (!h->plan_fwd.ready)
-    CKS(tc_forward_plan(h->tc, h->plan_fwd, h->Pb.p, (size_t)h->N * h->ld, h->Sxs.p, (size_t)h->N * h->Ke, 1, h->N, h->V, h->Ke, h->ld,
-                        g_err, sizeof(g_err)));
-  const int r0 = h->nchunks > 1 ? h->chunk_row[c] : 0, r1 = h->nchunks > 1 ? h->chunk_row[c + 1] : h->N;
-  // rows of this chunk: the streaming Adam kernel of the previous iteration must have written their P and row sums
-  if (h->a_valid && h->pipelined && !h->serial) CK(cudaStreamWaitEvent(s, h->ev_a[c], 0));
+  CKS(forward_plan(h));
+  const int r0 = h->chunk_row[c], r1 = h->chunk_row[c + 1];
+  // rows of this chunk: the streaming Adam kernel of the previous iteration must have written their P and row sums (on
+  // the caller's stream, after the join of the call that ran it, the wait is already satisfied)
+  if (h->a_valid) CK(cudaStreamWaitEvent(s, h->ev_a[c], 0));
   k_row_norm<<<(unsigned)ceil_div(r1 - r0, 256), 256, 0, s>>>(fresh, h->zsum.p, h->pxsum.p, h->l1sum.p, h->l2sum.p,
                                                              lseA, lseT, h->inv_zt.p, h->stats.p, rowaux, r0, r1);
   LAUNCH_CHECK("row_norm");
@@ -1091,7 +1104,6 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
     if (h->fwd_ahead) {           // issued by the previous iteration's backward (forward_chunk under the streaming Adam kernel)
       h->fwd_ahead = false;
       for (int c = 0; c < h->nchunks; ++c) CK(cudaStreamWaitEvent(s, h->ev_f[c], 0));
-      if (h->nchunks > 1) return TGB200_OK;
     } else {
       for (int c = 0; c < h->nchunks; ++c) CKS(forward_chunk(h, s, c, h->p_state == PState::fresh ? 1 : 0, h->lseA, h->lseT));
     }
@@ -1105,11 +1117,7 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
   const size_t vk = (size_t)h->V * h->Ke;
   float* out = h->fwd_splits > 1 ? h->Ypart.p : h->Y.p;
   if (h->tcm) {
-    if (!h->plan_fwd.ready) {
-      const __nv_bfloat16* sB = h->bf16 ? h->Sxs.p : h->Sxb.p;
-      CKS(tc_forward_plan(h->tc, h->plan_fwd, h->Pb.p, (size_t)h->N * h->ld, sB, (size_t)h->N * h->Ke, h->x3 ? 3 : 1, h->N, h->V, h->Ke,
-                          h->ld, g_err, sizeof(g_err)));
-    }
+    CKS(forward_plan(h));
     CKS(tc_forward_launch(h->tc, h->plan_fwd, h->x3 ? 6 : 1, out, h->N, h->V, h->Ke, h->fwd_splits, s, g_err, sizeof(g_err)));
     mark(h, s, "tc_gemm_fwd");
   } else {
@@ -1125,17 +1133,10 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
   return TGB200_OK;
 }
 
-extern "C" int tgb200_step_begin(tgb200_mapper* h, void* stream) {
-  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
-  cudaStream_t caller = (cudaStream_t)stream;
-  CK(cudaSetDevice(h->cfg.device));
-  CKS(check_ready(h));
-  if (h->in_step) return fail(TGB200_ERR_STATE, "step_begin called twice without step_end");
-  CKS(fork_streams(h, caller));
-  cudaStream_t s = work_stream(h, caller);
+// first half of an iteration, up to the exchange buffer: the forward and the row-scalar partials
+static int iteration_begin(tgb200_mapper* h, const Lanes& L) {
+  cudaStream_t s = L.work;
   if (h->constrained) {
-    // the filter logits were updated on the update stream at the end of the previous iteration
-    if (h->a_valid && h->pipelined && !h->serial) CK(cudaStreamWaitEvent(s, h->ev_a[0], 0));
     // f = sigmoid(F), S_f = f o S_ext (:507, :519) and the operand copies the contractions read
     const long long nq = (long long)h->N * (h->Ke / 4);
     k_filter_prepare<<<(unsigned)ceil_div(nq, 256), 256, 0, s>>>(h->Fl.p, h->Sx.p, h->N, h->Ke, h->fsig.p, h->Sf.p);
@@ -1156,8 +1157,6 @@ extern "C" int tgb200_step_begin(tgb200_mapper* h, void* stream) {
     k_sum_planes<<<(unsigned)ceil_div(vk, 256), 256, 0, s>>>(h->Ypart.p, h->fwd_splits, vk, h->Y.p);
     LAUNCH_CHECK("sum_planes");
   }
-  CKS(join_streams(h, caller));
-  h->in_step = true;
   return TGB200_OK;
 }
 
@@ -1302,15 +1301,18 @@ static int filter_update(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
 
 // Backward of the bf16 mode: dq = bf16(S_ext dY_ext^T - centre) + row-dot partials from the store-only contraction,
 // then one streaming pass does softmax-Jacobian + Adam + the next forward's P.  (mapping_optimizer.py:395-396)
-static int backward_bf16(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, const AdamScalars& a) {
+// `next_forward`: the next iteration of this call starts with a plain forward, which may then be issued ahead.
+static int backward_bf16(tgb200_mapper* h, const Lanes& L, const AdamScalars& a, bool next_forward) {
   if (!h->plan_dp.ready) {
     CKS(tc_dpstore_epi_plan(h->tc, h->plan_dp, h->Pb.p, h->dq.p, h->N, h->ld, g_err, sizeof(g_err)));
     CKS(tc_dpstore_plan(h->tc, h->plan_dp, h->Sxb.p, 0, h->dYb.p, 0, 1, h->N, h->V, h->Ke, g_err, sizeof(g_err)));
   }
+  cudaStream_t s = L.work, su = L.update;
   const bool two_streams = su != s;
-  const bool prefetch = two_streams && h->prefetch_next && h->nchunks > 1 && !h->constrained;
+  const bool prefetch = two_streams && next_forward;
+  if (prefetch) CK(cudaEventRecord(h->ev_loss, s));                   // the loss stage has consumed the partial planes of Y_ext
   for (int c = 0; c < h->nchunks; ++c) {
-    const int r0 = h->nchunks > 1 ? h->chunk_row[c] : 0, r1 = h->nchunks > 1 ? h->chunk_row[c + 1] : h->N;
+    const int r0 = h->chunk_row[c], r1 = h->chunk_row[c + 1];
     TcEpiDpStore epi{h->plan_dp.pt, h->plan_dp.dq, h->ld, h->rcenter.p, h->rpart.p, h->N};
     CKS(tc_dpstore_launch(h->tc, h->plan_dp, 1, epi, r0, r1, h->V, h->Ke, s, g_err, sizeof(g_err)));
     mark(h, s, "tc_gemm_bwd_dp");
@@ -1334,9 +1336,9 @@ static int backward_bf16(tgb200_mapper* h, cudaStream_t s, cudaStream_t su, cons
     // beside it, and nothing queues behind a kernel that still waits for the update.
     // (lseT of this iteration is the offset the new P was written with = lseA of the next; the other buffer is free.)
     if (prefetch) {
-      if (c == 0) CK(cudaStreamWaitEvent(h->sf, h->ev_loss, 0));      // the partial planes of Y_ext were consumed by this iteration's loss
-      CKS(forward_chunk(h, h->sf, c, 0, h->lseT, h->lseA));            // waits for ev_a[c]
-      CK(cudaEventRecord(h->ev_f[c], h->sf));
+      if (c == 0) CK(cudaStreamWaitEvent(L.ahead, h->ev_loss, 0));
+      CKS(forward_chunk(h, L.ahead, c, 0, h->lseT, h->lseA));          // waits for ev_a[c]
+      CK(cudaEventRecord(h->ev_f[c], L.ahead));
     }
   }
   h->fwd_ahead = prefetch;
@@ -1406,43 +1408,62 @@ static int validation_forward(tgb200_mapper* h, cudaStream_t s, float* out) {
 
 static bool val_due(const tgb200_mapper* h) { return h->val_every > 0 && h->val_epoch % h->val_every == 0; }
 
-extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
-  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
-  cudaStream_t caller = (cudaStream_t)stream;
-  CK(cudaSetDevice(h->cfg.device));
-  if (!h->in_step) return fail(TGB200_ERR_STATE, "step_end without step_begin");
-  CKS(ensure_history(h, h->hist_len + 1, caller));
-  CKS(fork_streams(h, caller));              // the caller may have all-reduced the exchange buffer on its stream
-  cudaStream_t s = work_stream(h, caller);
+// second half of an iteration, from the exchange buffer: loss stage, backward and update, and the epoch's validation.
+// `more`: another iteration of the same call follows.  The history must have room for one more row.
+static int iteration_end(tgb200_mapper* h, const Lanes& L, float lr, bool more) {
+  cudaStream_t s = L.work;
   float* hist_row = h->hist.p + (size_t)h->hist_len * TGB200_HIST_COLS;
   // sharded: the caller all-reduced Y (already the sum of every rank's partial planes)
   const bool sharded = h->cfg.n_cells_global != h->N;
   CKS(loss_stage(h, s, hist_row, !sharded));
-  if (h->pipelined && !h->serial) CK(cudaEventRecord(h->ev_loss, s));
 
   const AdamScalars a = adam_scalars(h->cfg, h->step + 1, lr);
-  cudaStream_t su = update_stream(h, caller);
-  if (h->bf16) CKS(backward_bf16(h, s, su, a));
+  // a validated bf16 epoch runs its own row pass after the update: no next forward issued ahead of it
+  if (h->bf16) CKS(backward_bf16(h, L, a, more && !val_due(h)));
   else if (h->x3) CKS(backward_bf16x3(h, s, a));
   else CKS(backward_fp32(h, s, a));
   // the validation of this epoch, on the mapping its update produced (mapping_optimizer.py:398-403)
   if (val_due(h)) {
-    // fp32 / bf16x3 inside tgb200_run: the next iteration's forward serves it.  Constrained mode keeps the separate forward,
-    // which still sees the filter of this epoch; the next forward sees the updated one.
-    if (h->val_fuse && !h->bf16 && !h->constrained) {
+    // fp32 / bf16x3 with an iteration to follow: the next iteration's forward serves it.  Constrained mode keeps the
+    // separate forward, which still sees the filter of this epoch; the next forward sees the updated one.
+    if (more && !h->bf16 && !h->constrained) {
       h->val_row = h->hist_len;
     } else {
-      if (su != s) {                           // the row pass reads every row the update stream wrote
-        CK(cudaEventRecord(h->ev_join_lo, su));
+      if (L.update != s) {                     // the row pass reads every row the update stream wrote
+        CK(cudaEventRecord(h->ev_join_lo, L.update));
         CK(cudaStreamWaitEvent(s, h->ev_join_lo, 0));
       }
       CKS(validation_forward(h, s, val_out_of(h, h->hist_len)));
     }
   }
   if (h->val_every > 0) h->val_epoch++;
-  CKS(join_streams(h, caller));
   h->step++;
   h->hist_len++;
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_step_begin(tgb200_mapper* h, void* stream) {
+  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CKS(check_ready(h));
+  if (h->in_step) return fail(TGB200_ERR_STATE, "step_begin called twice without step_end");
+  const Lanes L = lanes_of(h, (cudaStream_t)stream);
+  CKS(fork_streams(h, L));
+  CKS(iteration_begin(h, L));
+  CKS(join_streams(h, L));
+  h->in_step = true;
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
+  if (!h) return fail(TGB200_ERR_INVALID, "null handle");
+  CK(cudaSetDevice(h->cfg.device));
+  if (!h->in_step) return fail(TGB200_ERR_STATE, "step_end without step_begin");
+  CKS(ensure_history(h, h->hist_len + 1, (cudaStream_t)stream));
+  const Lanes L = lanes_of(h, (cudaStream_t)stream);
+  CKS(fork_streams(h, L));                   // the caller may have all-reduced the exchange buffer on its stream
+  CKS(iteration_end(h, L, lr, false));
+  CKS(join_streams(h, L));
   h->in_step = false;
   return TGB200_OK;
 }
@@ -1551,22 +1572,18 @@ extern "C" int tgb200_run(tgb200_mapper* h, int32_t n_steps, float lr, void* str
   CK(cudaSetDevice(h->cfg.device));
   CKS(ensure_history(h, h->hist_len + n_steps, (cudaStream_t)stream));
   if (n_steps == 0) return TGB200_OK;
-  CKS(fork_streams(h, (cudaStream_t)stream));
-  h->defer_join = true;                      // iterations chain through the handle's own streams and events
+  CKS(check_ready(h));
+  if (h->in_step) return fail(TGB200_ERR_STATE, "run inside a step");
+  const Lanes L = lanes_of(h, (cudaStream_t)stream);
+  CKS(fork_streams(h, L));                   // iterations chain through the handle's own streams and events
   int st = TGB200_OK;
   for (int i = 0; i < n_steps && st == TGB200_OK; ++i) {
-    // a validated bf16 epoch runs its own row pass after the update: no next forward issued ahead of it
-    h->prefetch_next = i + 1 < n_steps && !val_due(h);
-    h->val_fuse = i + 1 < n_steps;
-    st = tgb200_step_begin(h, stream);
-    if (st == TGB200_OK && sharded) st = exchange_partials(h, work_stream(h, (cudaStream_t)stream));
-    if (st == TGB200_OK) st = tgb200_step_end(h, lr, stream);
+    st = iteration_begin(h, L);
+    if (st == TGB200_OK && sharded) st = exchange_partials(h, L.work);
+    if (st == TGB200_OK) st = iteration_end(h, L, lr, i + 1 < n_steps);
   }
-  h->defer_join = false;
-  h->prefetch_next = false;
-  h->val_fuse = false;
   h->val_row = -1;                           // set only when an iteration follows, unless that iteration failed
-  CKS(join_streams(h, (cudaStream_t)stream));
+  CKS(join_streams(h, L));
   return st;
 }
 
@@ -1712,6 +1729,9 @@ extern "C" int tgb200_profile_step(tgb200_mapper* h, float lr, void* stream, con
   if (!h || !names || !ms || !n) return fail(TGB200_ERR_INVALID, "null argument");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
+  CKS(check_ready(h));
+  if (h->in_step) return fail(TGB200_ERR_STATE, "profile_step inside a step");
+  CKS(ensure_history(h, h->hist_len + 1, s));
   cudaEvent_t e0;
   CK(cudaEventCreate(&e0));
   CK(cudaStreamSynchronize(s));
@@ -1720,10 +1740,9 @@ extern "C" int tgb200_profile_step(tgb200_mapper* h, float lr, void* stream, con
   const bool timeline = h->recording;
   const size_t first = h->records.size();
   h->recording = true;
-  h->serial = true;                          // one stream, one kernel at a time: clean per-kernel durations
-  int st = tgb200_step_begin(h, stream);
-  if (st == TGB200_OK) st = tgb200_step_end(h, lr, stream);
-  h->serial = false;
+  const Lanes L{s, s, s, s};                 // one stream, one kernel at a time: clean per-kernel durations
+  int st = iteration_begin(h, L);
+  if (st == TGB200_OK) st = iteration_end(h, L, lr, false);
   h->recording = timeline;
   cudaStreamSynchronize(s);
   int cnt = 0;
