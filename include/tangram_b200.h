@@ -276,9 +276,12 @@ TGB200_API int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, 
  *   pearson_out            R(R-1)/2 doubles (host or device; NULL to skip): np.corrcoef of the flattened arrays at
  *                          np.tril_indices(R, -1), i.e. pearson_corr (:42-53); sums in fp64, reduced in a fixed order
  *   vote_entropy_out       rows floats (host or device; NULL to skip): per row, the entropy of the R runs' argmax votes
- *                          (first column on ties) over log(cols), vote_entropy (:55-69)
+ *                          over log(cols), vote_entropy (:55-69).  The argmax is np.argmax's: first column on ties, a
+ *                          NaN counting as the maximum (the first NaN wins), column 0 for a row that is -inf throughout
  *   consensus_entropy_out  rows floats (host or device; NULL to skip): per row, the entropy of p / sum(p) with
- *                          p = mean over runs, over log(cols), consensus_entropy (:71-82)
+ *                          p = mean over runs, over log(cols), consensus_entropy (:71-82); NaN where p holds a NaN or
+ *                          an infinity, or sums to 0
+ *   With cols == 1 both entropies are NaN on every row, as the reference's division by log(1) = 0 gives.
  * Fails with TGB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  Bit-reproducible on a given device.
  * Synchronous on `stream`. */
 TGB200_API int tgb200_agreement(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,

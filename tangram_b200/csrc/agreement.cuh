@@ -76,7 +76,10 @@ struct AgrAcc {
       float p = v[0];
 #pragma unroll
       for (int r = 0; r < R; ++r) {
-        if (v[r] > best[r]) { best[r] = v[r]; bidx[r] = j; }          // a lane sees its columns in increasing order
+        // argmax_prefer's order, specialised to a lane that sees its columns in increasing order: a larger value or the
+        // first NaN takes the place (!(v <= best) holds for a NaN v), nothing replaces a NaN, and an equal value keeps
+        // the earlier column.  -inf is never taken: a lane that saw only -inf keeps bidx = INT_MAX (see below).
+        if (!(v[r] <= best[r]) && best[r] == best[r]) { best[r] = v[r]; bidx[r] = j; }
         if (r > 0) p += v[r];
       }
       p = p / (float)R;                                               // numpy's float32 mean over the runs
@@ -144,10 +147,15 @@ __global__ void __launch_bounds__(kAgrThreads) k_agreement(AgrArgs a) {
     if (kRows) {
       // argmax per run: largest value, first column on ties (np.argmax)
 #pragma unroll
-      for (int r = 0; r < R; ++r) warp_argmax(acc.best[r], acc.bidx[r]);
+      for (int r = 0; r < R; ++r) {
+        warp_argmax(acc.best[r], acc.bidx[r]);
+        if (acc.bidx[r] == INT_MAX) acc.bidx[r] = 0;                 // every value -inf: np.argmax votes for column 0
+      }
       const double s = warp_sum_d(acc.csum), plogp = warp_sum_d(acc.cplogp);
       if (lane == 0) {
-        const double inv_log_cols = 1.0 / log((double)cols);
+        // one column: the reference divides by log(1) = 0, and the bracket of the consensus entropy need not round to
+        // exactly 0, so both entropies are NaN by definition rather than 0 * inf or +-inf
+        const double inv_log_cols = cols > 1 ? 1.0 / log((double)cols) : (double)NAN;
         if (a.vote) {
           // scipy.stats.entropy of the vote shares c / R, groups taken in column order as numpy sums them
           double h = 0.0, tot = 0.0;

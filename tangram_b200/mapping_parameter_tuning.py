@@ -87,12 +87,15 @@ def pearson_corr(cube, *, device=None):
 
 
 def vote_entropy(pred_probs_cube, *, device=None):
-    """:55-69 -- per row, the entropy of the runs' argmax votes (first column on ties) normalised by log(V): (N,)."""
+    """:55-69 -- per row, the entropy of the runs' argmax votes normalised by log(V): (N,).  The votes are np.argmax's:
+    the first column on ties, a NaN counting as the maximum (the first NaN wins), column 0 for an all -inf row.  NaN on
+    every row when V == 1, as the reference's division by log(1) = 0 gives."""
     return agreement(pred_probs_cube, pearson=False, vote=True, device=device)[1]
 
 
 def consensus_entropy(pred_probs_cube, *, device=None):
-    """:71-82 -- per row, the entropy of the mean over runs (renormalised, 0 log 0 = 0) normalised by log(V): (N,)."""
+    """:71-82 -- per row, the entropy of the mean over runs (renormalised, 0 log 0 = 0) normalised by log(V): (N,).
+    NaN for a row whose mean holds a NaN or an infinity or sums to 0, and on every row when V == 1."""
     return agreement(pred_probs_cube, pearson=False, consensus=True, device=device)[2]
 
 
