@@ -191,9 +191,13 @@ TGB200_API int tgb200_set_loss_genes(tgb200_mapper* h, const uint8_t* active, vo
  * contraction); the last iteration of a call and constrained mode run tgb200_validation_terms' forward.  bf16 mode: that
  * exact row pass and forward once per validated epoch, which the next iteration then starts from, as after
  * tgb200_validation_terms.  No allocation and no host sync in the loop.
+ * A sharded handle (n_cells_global != n_cells) validates the global mapping when it has a communicator (tgb200_comm_init_rank
+ * / tgb200_set_comm): the four values are _val_loss_fn's over all n_cells_global cells, bit-identical on every rank.  The
+ * forward that serves a validation inside tgb200_run carries sum_i h_i in exchange tail slot [5]; the separate forward
+ * sums [Y_ext | tail] over the ranks with one more all-reduce on the handle's communicator, in the exchange buffer.
  * every = 0 (the default) turns validation off.  TGB200_ERR_STATE between step_begin and step_end; every > 0 on a sharded
- * handle is TGB200_ERR_UNSUPPORTED.  Allocates the validation's scratch (about 8 (Ke + V) bytes, more when lambda_g2 == 0) on first use;
- * queues no work on `stream`. */
+ * handle without a communicator, or on a sharded constrained handle, is TGB200_ERR_UNSUPPORTED.  Allocates the
+ * validation's scratch (about 8 (Ke + V) bytes, more when lambda_g2 == 0) on first use; queues no work on `stream`. */
 TGB200_API int tgb200_set_validation(tgb200_mapper* h, int32_t every, void* stream);
 
 /* Constrained mode: initial filter logits F0 (n_cells, host or device; the reference draws them at :490).
@@ -216,7 +220,9 @@ TGB200_API int tgb200_run(tgb200_mapper* h, int32_t n_steps, float learning_rate
  * needs target_count > 0).  The exchange buffer holds n_voxels x Ke floats of Y_ext = P^T S_ext over this rank's cells
  * (gene columns, two density columns, cell-type columns; Ke = n_genes + 2 + n_types rounded up to 64), then an 8-float
  * tail of row sums: [0] the per-row entropy terms (when lambda_r != 0), [1] sum |M| and [2] sum M^2 (the L1 / L2 terms),
- * [3] sum f and [4] sum (f - f^2) (constrained mode), [5..7] zero.  In constrained mode the operand is f o S_ext
+ * [3] sum f and [4] sum (f - f^2) (constrained mode), [5] sum_i h_i on an iteration whose forward serves a pending
+ * validation (tgb200_set_validation) and zero otherwise, [6..7] zero.  On a sharded handle an iteration that serves no
+ * validation writes every slot no row term needs as zero, also right after a validated one.  In constrained mode the operand is f o S_ext
  * (f = sigmoid(F) of this rank's cells), so the density columns already hold the f-weighted column sums, and after the sum
  * [3] / [4] are the filter's global count and regulariser; every scalar of the filter update (lambda_d sum d / sum f,
  * sign(sum f - target_count)) is derived from the summed buffer, so each rank updates its own F entries with global
@@ -236,7 +242,8 @@ TGB200_API int tgb200_step_end(tgb200_mapper* h, float learning_rate, void* stre
  *   tgb200_comm_unique_id   rank 0: 128 opaque bytes (ncclGetUniqueId) to hand to every rank by any means
  *   tgb200_comm_init_rank   every rank: ncclCommInitRank on the handle's device; the handle owns the communicator
  *   tgb200_set_comm         alternatively borrow an existing ncclComm_t (NULL detaches); the caller keeps ownership and must
- *                           detach or destroy the handle before destroying that communicator
+ *                           detach or destroy the handle before destroying that communicator.  Detaching while a sharded
+ *                           handle validates (tgb200_set_validation(every > 0)) is TGB200_ERR_STATE
  * When a communicator arrives the exchange buffer is moved into ncclMemAlloc memory and registered with it (ncclCommRegister,
  * NCCL >= 2.19; silently skipped otherwise), so that the in-place all-reduce runs as an in-switch NVLS reduction on user
  * buffers; pointers obtained earlier from tgb200_exchange_buffer are invalid afterwards. */
@@ -260,7 +267,10 @@ TGB200_API int tgb200_get_mapping(tgb200_mapper* h, float* out, void* stream);
 /* _val_loss_fn (:311-356) of the current mapping: out[4] = expression_sim, gv_sim, sp_sparsity_weighted_gv_sim, entropy
  * (HOST).  One forward on the device and one 16-byte copy, the forward and kernels tgb200_set_validation runs in the loop
  * (so the values are those bit for bit); allocates the same scratch on first use.  Synchronous on `stream`.
- * TGB200_ERR_STATE between step_begin and step_end; TGB200_ERR_UNSUPPORTED on a sharded handle. */
+ * On a sharded handle with a communicator this is a collective: every rank calls it, the forward's [Y_ext | tail] is
+ * summed over the ranks on the handle's communicator, and every rank gets the same four values of the global mapping.
+ * TGB200_ERR_STATE between step_begin and step_end; TGB200_ERR_UNSUPPORTED on a sharded handle without a communicator
+ * and on a sharded constrained handle. */
 TGB200_API int tgb200_validation_terms(tgb200_mapper* h, float* out4_host, void* stream);
 /* project_genes' GEMM (tangram/utils.py:368): out (n_voxels x n_cols, host or device) = softmax(M)^T X, X (n_cells x
  * n_cols) row-major f32, host or device.  tgb200_project_map's blocks and arithmetic, with each block's mapping rows

@@ -183,13 +183,16 @@ k_softmax_rows(const float* __restrict__ M, int ldm, int V, PT* __restrict__ P, 
   }
 }
 
-// Sum of per-row scalars (entropy, L1, L2) over this rank's rows -> 4-float tail of the
+// Sum of per-row scalars (entropy, L1, L2) over this rank's rows -> 8-float tail of the
 // exchange buffer.  Deterministic (fixed tree), one CTA.
-// tail (8 floats): [0] sum_i h_i, [1] sum|M|, [2] sum M^2, [3] sum_i f_i, [4] sum_i (f_i - f_i^2)  (f: constrained mode)
+// tail (8 floats): [0] sum_i h_i, [1] sum|M|, [2] sum M^2, [3] sum_i f_i, [4] sum_i (f_i - f_i^2)  (f: constrained mode),
+// [5] sum_i h_i again when `val` (a sharded handle's validation entropy, read by k_loss_scalars<true>), else 0; [6], [7] 0.
+// stats / rowaux / f may be null: their slots are then 0
 constexpr int kTail = 8;
+constexpr int kTailValEntropy = 5;
 __global__ void __launch_bounds__(1024)
 k_row_scalar_reduce(const RowStat* __restrict__ stats, const float* __restrict__ rowaux, const float* __restrict__ f,
-                    int n_rows, float* __restrict__ tail) {
+                    int n_rows, int val, float* __restrict__ tail) {
   __shared__ float sh[32];
   float h = 0.f, a = 0.f, b = 0.f, fs = 0.f, fr = 0.f;
   for (int i = threadIdx.x; i < n_rows; i += blockDim.x) {
@@ -203,7 +206,7 @@ k_row_scalar_reduce(const RowStat* __restrict__ stats, const float* __restrict__
   fs = block_reduce<false>(fs, sh);
   fr = block_reduce<false>(fr, sh);
   if (threadIdx.x == 0) {
-    tail[0] = h; tail[1] = a; tail[2] = b; tail[3] = fs; tail[4] = fr; tail[5] = 0.f; tail[6] = 0.f; tail[7] = 0.f;
+    tail[0] = h; tail[1] = a; tail[2] = b; tail[3] = fs; tail[4] = fr; tail[5] = val ? h : 0.f; tail[6] = 0.f; tail[7] = 0.f;
   }
 }
 
@@ -298,10 +301,12 @@ struct LossParams {
   // history columns 12-15: 0 with validation off, NaN on the rows a validation does not fill (tgb200_set_validation)
   float hist_fill;
   // validation (_val_loss_fn, mapping_optimizer.py:311-356): k_loss_scalars<true> also writes
-  // val_out[0..3] = (gv + vg, gv, sum_k cos_k w_k / sum_k w_k, -(sum_i h_i / log V) / n_cells)
+  // val_out[0..3] = (gv + vg, gv, sum_k cos_k w_k / sum_k w_k, -(sum_i h_i / log V) / n_cells_global), sum_i h_i from
+  // tail[val_ent] (on a sharded handle kTailValEntropy, over every rank's cells once the exchange buffer is summed)
   const float* gw;                // Ke   w_k: fraction of voxels where G[:, k] != 0 (0 outside the mask)
   float* val_out;
-  float val_log_v, val_n;         // logf(V) as the host computes it, n_cells
+  float val_log_v, val_n;         // logf(V) as the host computes it, n_cells_global
+  int val_ent;                    // tail slot of sum_i h_i
 };
 
 // Y = sum over split partials; per-gene <Y,G>, |Y|^2, colsum(Y) for this row chunk;
@@ -578,7 +583,7 @@ k_loss_scalars(LossParams p, int nchunk, int ncolchunk, float* __restrict__ hist
       p.val_out[0] = gv + vg;                            // expression_sim (:328)
       p.val_out[1] = gv;                                 // gv_sim (:326)
       p.val_out[2] = sw / ws;                            // sp_sparsity_weighted_gv_sim (:329-331)
-      p.val_out[3] = -(tail[0] / p.val_log_v) / p.val_n;  // entropy (:333)
+      p.val_out[3] = -(tail[p.val_ent] / p.val_log_v) / p.val_n;  // entropy (:333)
     }
   }
 }

@@ -145,6 +145,9 @@ struct tgb200_mapper {
   int val_every = 0;
   int64_t val_epoch = 0;
   int64_t val_row = -1;         // fp32 / bf16x3: the row whose validation this iteration's forward computes (see loss_stage)
+  // sharded: a validation wrote the exchange tail (sum h in [0] and [5]); the next iteration rewrites it even when no row
+  // term needs it, so that an exchange that carries no validation sums zeros there
+  bool tail_stale = false;
   DevBuf<float> val_coef, val_rowpart, val_hist;   // what the validation's k_loss_scalars writes beside its four values
   // history
   DevBuf<float> hist;
@@ -664,12 +667,21 @@ static int alloc_validation(tgb200_mapper* h) {
   return TGB200_OK;
 }
 
+// A sharded handle validates only with a communicator of its own to sum the validation forward's [Y_ext | tail] on (a
+// caller-driven exchange has no slot for a second all-reduce), and only in plain mode.
+static int check_validation_supported(const tgb200_mapper* h) {
+  if (h->cfg.n_cells_global == h->N) return TGB200_OK;
+  if (h->constrained) return fail(TGB200_ERR_UNSUPPORTED, "validation on a sharded constrained handle");
+  if (!h->comm) return fail(TGB200_ERR_UNSUPPORTED, "validation on a sharded handle without a communicator");
+  return TGB200_OK;
+}
+
 // Per-epoch validation inside tgb200_run / step_end (Mapper.train(val_each=), mapping_optimizer.py:398-403).
 extern "C" int tgb200_set_validation(tgb200_mapper* h, int32_t every, void* stream) {
   if (!h) return fail(TGB200_ERR_INVALID, "null handle");
   if (every < 0) return fail(TGB200_ERR_INVALID, "every = %d < 0", every);
   if (h->in_step) return fail(TGB200_ERR_STATE, "set_validation inside a step");
-  if (every > 0 && h->cfg.n_cells_global != h->N) return fail(TGB200_ERR_UNSUPPORTED, "validation on a sharded handle");
+  if (every > 0) CKS(check_validation_supported(h));
   CK(cudaSetDevice(h->cfg.device));
   if (every > 0) CKS(alloc_validation(h));
   (void)stream;                                      // nothing is queued: the switch takes effect at the next step
@@ -1133,6 +1145,15 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
   return TGB200_OK;
 }
 
+// sharded: the exchange buffer must hold this rank's complete partial sum of Y_ext, not the forward's partial planes
+static int sum_forward_planes(tgb200_mapper* h, cudaStream_t s) {
+  if (h->cfg.n_cells_global == h->N || h->fwd_splits <= 1) return TGB200_OK;
+  const size_t vk = (size_t)h->V * h->Ke;
+  k_sum_planes<<<(unsigned)ceil_div(vk, 256), 256, 0, s>>>(h->Ypart.p, h->fwd_splits, vk, h->Y.p);
+  LAUNCH_CHECK("sum_planes");
+  return TGB200_OK;
+}
+
 // first half of an iteration, up to the exchange buffer: the forward and the row-scalar partials
 static int iteration_begin(tgb200_mapper* h, const Lanes& L) {
   cudaStream_t s = L.work;
@@ -1147,17 +1168,17 @@ static int iteration_begin(tgb200_mapper* h, const Lanes& L) {
   const bool val = h->val_row >= 0;
   CKS(forward_pass(h, s, h->cfg.lambda_r != 0.f || val ? 1 : 0));
   const size_t vk = (size_t)h->V * h->Ke;
-  if (needs_rowscalars(h->cfg) || h->constrained || val) {
-    k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, needs_rowaux(h->cfg) ? h->rowaux.p : nullptr,
-                                           h->constrained ? h->fsig.p : nullptr, h->N, h->Y.p + vk);
+  const bool sharded = h->cfg.n_cells_global != h->N;
+  const bool rows = needs_rowscalars(h->cfg) || h->constrained || val;
+  if (rows || h->tail_stale) {
+    // sharded: the pending validation's sum of entropies rides in tail[5], so that it is summed over ranks with Y_ext.
+    // Without row data (only a stale tail to clear) every slot is written 0.
+    k_row_scalar_reduce<<<1, 1024, 0, s>>>(rows ? h->stats.p : nullptr, needs_rowaux(h->cfg) ? h->rowaux.p : nullptr,
+                                           h->constrained ? h->fsig.p : nullptr, h->N, val && sharded ? 1 : 0, h->Y.p + vk);
     LAUNCH_CHECK("row_scalar_reduce");
   }
-  if (h->cfg.n_cells_global != h->N && h->fwd_splits > 1) {
-    // sharded: the exchange buffer must hold this rank's complete partial sum
-    k_sum_planes<<<(unsigned)ceil_div(vk, 256), 256, 0, s>>>(h->Ypart.p, h->fwd_splits, vk, h->Y.p);
-    LAUNCH_CHECK("sum_planes");
-  }
-  return TGB200_OK;
+  h->tail_stale = val && sharded;
+  return sum_forward_planes(h, s);
 }
 
 extern "C" int tgb200_exchange_buffer(tgb200_mapper* h, float** device_ptr, int64_t* n_floats) {
@@ -1211,7 +1232,9 @@ static LossParams val_loss_params(tgb200_mapper* h, float* out) {
   p.lam_g2 = 1.f; p.lam_g1 = 1.f; p.lam_nb = 0.f; p.lam_go = 0.f; p.lam_ct = 0.f; p.density_mode = 0;
   p.constrained = 0;
   p.gw = h->gw.p; p.val_out = out;
-  p.val_log_v = logf((float)h->V); p.val_n = (float)h->N;
+  p.val_log_v = logf((float)h->V); p.val_n = (float)h->cfg.n_cells_global;
+  // sharded: sum h travels in its own tail slot ([0] stays the lambda_r term of the exchange); unsharded: [0], as it was
+  p.val_ent = h->cfg.n_cells_global != h->N ? kTailValEntropy : 0;
   return p;
 }
 
@@ -1391,16 +1414,33 @@ static int backward_fp32(tgb200_mapper* h, cudaStream_t s, const AdamScalars& a)
   return TGB200_OK;
 }
 
+// The one exchange of an iteration (SURVEY 8(e)): sum over ranks of [Y_ext partial | row-scalar partials], in place.
+static int exchange_partials(tgb200_mapper* h, cudaStream_t s) {
+  NcclApi* api = nccl_api(g_err, sizeof(g_err));
+  if (!api) return TGB200_ERR_STATE;
+  const size_t count = (size_t)h->V * h->Ke + kTail;
+  const int r = api->AllReduce(h->Y.p, h->Y.p, count, kNcclFloat32, kNcclSum, h->comm, s);
+  if (r != 0) return fail(TGB200_ERR_CUDA, "ncclAllReduce: %s", api->GetErrorString(r));
+  return TGB200_OK;
+}
+
 // The separate validation forward (and all of tgb200_validation_terms), into out[0..3] (device), on `s`.  bf16 mode re-runs
 // the exact row pass, so the per-row entropy exists whatever lambda_r is; P is then fresh and the next iteration starts
-// from it.
+// from it.  A sharded handle sums [Y_ext | tail] over the ranks on its communicator first, in the exchange buffer itself:
+// the iteration that wrote it has consumed it, and the next forward overwrites it.
 static int validation_forward(tgb200_mapper* h, cudaStream_t s, float* out) {
   if (h->bf16) { h->p_state = PState::stale; h->fwd_ahead = false; }
   CKS(forward_pass(h, s, 1));
   LossParams p = val_loss_params(h, out);
-  CKS(reduce_columns(h, s, p, true, 1));
-  k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, nullptr, nullptr, h->N, h->Y.p + (size_t)h->V * h->Ke);
+  const bool sharded = h->cfg.n_cells_global != h->N;
+  k_row_scalar_reduce<<<1, 1024, 0, s>>>(h->stats.p, nullptr, nullptr, h->N, sharded ? 1 : 0, h->Y.p + (size_t)h->V * h->Ke);
   LAUNCH_CHECK("row_scalar_reduce");
+  h->tail_stale = sharded;
+  if (sharded) {
+    CKS(sum_forward_planes(h, s));
+    CKS(exchange_partials(h, s));
+  }
+  CKS(reduce_columns(h, s, p, !sharded, 1));
   k_loss_scalars<true><<<1, 1024, 0, s>>>(p, 1, h->nredchunk, h->val_hist.p);
   LAUNCH_CHECK("loss_scalars");
   return TGB200_OK;
@@ -1465,16 +1505,6 @@ extern "C" int tgb200_step_end(tgb200_mapper* h, float lr, void* stream) {
   CKS(iteration_end(h, L, lr, false));
   CKS(join_streams(h, L));
   h->in_step = false;
-  return TGB200_OK;
-}
-
-// The one exchange of an iteration (SURVEY 8(e)): sum over ranks of [Y_ext partial | row-scalar partials], in place.
-static int exchange_partials(tgb200_mapper* h, cudaStream_t s) {
-  NcclApi* api = nccl_api(g_err, sizeof(g_err));
-  if (!api) return TGB200_ERR_STATE;
-  const size_t count = (size_t)h->V * h->Ke + kTail;
-  const int r = api->AllReduce(h->Y.p, h->Y.p, count, kNcclFloat32, kNcclSum, h->comm, s);
-  if (r != 0) return fail(TGB200_ERR_CUDA, "ncclAllReduce: %s", api->GetErrorString(r));
   return TGB200_OK;
 }
 
@@ -1548,6 +1578,8 @@ extern "C" int tgb200_set_comm(tgb200_mapper* h, void* nccl_comm, int32_t rank, 
   if (!h) return fail(TGB200_ERR_INVALID, "null handle");
   if (nccl_comm && (world < 1 || rank < 0 || rank >= world)) return fail(TGB200_ERR_INVALID, "bad rank %d of %d", rank, world);
   if (nccl_comm && !nccl_api(g_err, sizeof(g_err))) return TGB200_ERR_STATE;
+  if (!nccl_comm && h->val_every > 0 && h->cfg.n_cells_global != h->N)
+    return fail(TGB200_ERR_STATE, "set_comm(NULL) while a sharded handle validates: call tgb200_set_validation(0) first");
   if (h->y_nccl) {              // back to a plain buffer before the communicator it is registered with goes away
     DevBuf<float> plain;
     CKS(plain.alloc(h->Y.n, false));
@@ -1707,7 +1739,7 @@ extern "C" int tgb200_validation_terms(tgb200_mapper* h, float* out4, void* stre
   CK(cudaSetDevice(h->cfg.device));
   CKS(check_ready(h));
   if (h->in_step) return fail(TGB200_ERR_STATE, "validation_terms inside a step");
-  if (h->cfg.n_cells_global != h->N) return fail(TGB200_ERR_UNSUPPORTED, "validation_terms on a sharded handle");
+  CKS(check_validation_supported(h));
   CKS(alloc_validation(h));
   DevBuf<float> d4;
   CKS(d4.alloc(4, false));

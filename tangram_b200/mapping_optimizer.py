@@ -14,8 +14,12 @@ Additions (keyword-only, all optional):
   process_group / shard  cell-sharded multi-GPU operation (one process per GPU): every rank passes the
               full S (/ M0) and keeps rows shard_rows(N, rank, world); with a NCCL process group the handle gets its own
               NCCL communicator (tgb200_comm_init_rank) and the per-iteration exchange runs inside tgb200_run;
-              MapperConstrained takes both with the same meaning (full S, M0 and F0 on every rank)
+              MapperConstrained takes both with the same meaning (full S, M0 and F0 on every rank); on a NCCL group
+              Mapper.train(val_each=) and validation_terms() validate the global mapping, identically on every rank
   n_cells_global         pre-sharded variant (Mapper only): S, M0, d_source, ct_encode already hold only this rank's rows
+  draw_whole_stream      (Mapper only) a sharded rank's seeded draw leaves numpy's generator where the unsharded draw
+              leaves it instead of after the rank's last row, so that draws made one after another from it (cross_val's
+              folds) are the same on every rank
   train(..., resume=True)  continue with the Adam state of the previous train() call (the reference -- and the default
               here -- builds a fresh optimizer in every train() call, mapping_optimizer.py:373)
   train(..., out=tensor)   write softmax(M) into a CUDA tensor instead of returning a host array
@@ -195,6 +199,13 @@ class _EngineMapper:
         sharded_steps(on_stream, n_steps, lr,
                       lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self._pg))   # the one exchange per step
 
+    def _check_validation(self):
+        """A sharded mapper validates the global mapping with one more all-reduce per validation on the handle's own NCCL
+        communicator; the host-driven exchange (a gloo group, or `shard=` without a group) has no slot for it."""
+        if self._sharded and not self._own_comm:
+            raise ValueError("validation of a sharded mapper needs an NCCL process group: with a non-NCCL group (or shard= "
+                             "alone) the host drives the exchange and cannot sum the validation's forward")
+
     def _set_loss_genes(self, active):
         """Cross-validation fold: the loss sees only the genes flagged in `active` (n_genes booleans; None = all), as a
         mapper built on S[:, active], G[:, active] would (Engine.set_loss_genes)."""
@@ -207,6 +218,8 @@ class _EngineMapper:
         this call's rows and returns softmax(M), in `out` or a host array; with fetch=False (cross-validation scores genes
         with project() and needs no mapping on the host) it returns None."""
         every = _validation_period(val_each)
+        if every:
+            self._check_validation()
         if not resume:
             self._engine.reset_adam()
         first = self._engine.history_len()
@@ -277,6 +290,7 @@ class Mapper(_EngineMapper):
         process_group=None,
         shard=None,
         n_cells_global=None,
+        draw_whole_stream=False,
     ):
         if lambda_geary > 0 or lambda_moran > 0:
             # mapping_optimizer.py:173-185: not on the accelerated path (Geary builds V x V x K)
@@ -321,6 +335,7 @@ class Mapper(_EngineMapper):
         # cell-sharded operation: this rank keeps rows [r0, r1)
         r0, r1 = self._select_rows(n_rows_given, n_cells_global, shard, process_group, presharded)
         self._presharded = presharded
+        self._draw_whole_stream = bool(draw_whole_stream)
         if M0 is not None:
             M0 = M0[r0:r1]
 
@@ -365,16 +380,19 @@ class Mapper(_EngineMapper):
     def _draw_initial_mapping(self):
         """The reference's initial mapping (:147-157): np.random.normal(0, 1, (N, V)) from numpy's legacy global generator,
         seeded first only if random_state is truthy, cast to float32.  A rank of a sharded run draws the same stream and
-        keeps only its rows (pre-sharded callers get a per-rank draw).  The draw runs on the device (legacy_rng) unless
-        this numpy's arithmetic differs from the device formula; either way the generator ends where the host draw leaves
-        it.  Resets the Adam state and the history."""
+        keeps only its rows (pre-sharded callers get a per-rank draw); the generator then ends after row r1, or, with
+        draw_whole_stream, where the unsharded draw leaves it.  The draw runs on the device (legacy_rng) unless this
+        numpy's arithmetic differs from the device formula; either way the generator ends where the host draw leaves it.
+        Resets the Adam state and the history."""
         r0, r1 = self._rows
+        end_row = self._engine.cfg.n_cells_global if self._draw_whole_stream and not self._presharded else r1
         if not self._presharded and legacy_rng.device_draw_supported():
             if self.random_state:
                 np.random.seed(seed=self.random_state)
-            legacy_rng.draw_global(self._engine, 0, r0, r1 * self.n_voxels)   # the generator ends after row r1
+            legacy_rng.draw_global(self._engine, 0, r0, end_row * self.n_voxels)   # the generator ends after row end_row
         else:
             M0 = legacy_normal_rows(self.random_state, r1, self.n_voxels, r0, r1)
+            discard_normal_rows(end_row - r1, self.n_voxels)
             self._engine.set_mapping(np.ascontiguousarray(M0, dtype=np.float32))
 
     # ------------------------------------------------------------------------------
@@ -403,7 +421,10 @@ class Mapper(_EngineMapper):
     # --- extras beyond the reference surface -------------------------------------------
     def validation_terms(self):
         """The reference's validation scores (_val_loss_fn, mapping_optimizer.py:311-356) of the current mapping:
-        {val_total_loss, val_gene_sim, val_sp_sparsity_weighted_sim, val_entropy} as floats."""
+        {val_total_loss, val_gene_sim, val_sp_sparsity_weighted_sim, val_entropy} as floats.
+        Sharded on an NCCL group this is a collective: every rank must call it, and every rank gets the same values of the
+        global mapping (all n_cells_global cells)."""
+        self._check_validation()
         return {k: float(x) for k, x in zip(_VAL_KEYS, self._engine.validation_terms())}
 
     def state(self):

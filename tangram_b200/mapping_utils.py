@@ -204,6 +204,25 @@ def _prepare_mapping(adata_sc, adata_sp, cv_train_genes, cluster_label, mode, sc
     return adata_sc, training_genes, S, G, mapper_kw
 
 
+def _check_shardable(mode, process_group):
+    if process_group is not None and mode == "clusters":
+        raise ValueError("process_group shards the cells axis: only mode='cells' can be sharded, and mode='constrained' "
+                         "(clusters mode has too few rows).")
+
+
+def _sum_over_group(partial, mapper, process_group):
+    """A projection of this rank's cells (softmax(M)[r0:r1]^T X) -> the sum over the group's ranks, the projection of every
+    cell, the same on every rank; unchanged without a group."""
+    if process_group is None:
+        return partial
+    import torch
+    import torch.distributed as dist
+    t = torch.from_numpy(np.ascontiguousarray(partial))
+    t = t.cuda(mapper._cfg.device) if dist.get_backend(process_group) == "nccl" else t
+    dist.all_reduce(t, group=process_group)
+    return t.cpu().numpy()
+
+
 def _make_mapper(mode, mapper_kw, **kw):
     """The mode's mapper class, looked up on the module `mo` at call time (a test can stand another class in there)."""
     if mode == "constrained":
@@ -232,9 +251,7 @@ def map_cells_to_space(
                     other ranks return None.
     keep_on_device  keep the trained mapper (device state ~20 B per mapping element) attached to the result so that
                     project_genes contracts on the GPU; default: release it (`adata_map.X` is all project_genes needs)."""
-    if process_group is not None and mode == "clusters":
-        raise ValueError("process_group shards the cells axis: only mode='cells' can be sharded, and mode='constrained' "
-                         "(clusters mode has too few rows).")
+    _check_shardable(mode, process_group)
     adata_sc, training_genes, S, G, mapper_kw = _prepare_mapping(
         adata_sc, adata_sp, cv_train_genes, cluster_label, mode, scale, density_prior, lambda_d, lambda_g1, lambda_g2,
         lambda_r, lambda_l1, lambda_l2, lambda_count, lambda_f_reg, target_count, lambda_neighborhood_g1,
@@ -264,14 +281,7 @@ def map_cells_to_space(
         adata_map.obs["F_out"] = F_out                                            # :398-399
 
     # per-gene training score (:401-410): softmax(M)^T S on the device instead of a host GEMM
-    G_predicted = mapper.project(S[r0:r1])
-    if process_group is not None:             # sum of the ranks' partial projections: the same V x K on every rank
-        import torch
-        import torch.distributed as dist
-        t = torch.from_numpy(np.ascontiguousarray(G_predicted))
-        t = t.cuda(mapper._cfg.device) if dist.get_backend(process_group) == "nccl" else t
-        dist.all_reduce(t, group=process_group)
-        G_predicted = t.cpu().numpy()
+    G_predicted = _sum_over_group(mapper.project(S[r0:r1]), mapper, process_group)
     num = (G * G_predicted).sum(axis=0)
     den = np.linalg.norm(G, axis=0) * np.linalg.norm(G_predicted, axis=0)
     df_cs = pd.DataFrame(num / den, list(training_genes), columns=["train_score"])

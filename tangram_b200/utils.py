@@ -432,7 +432,7 @@ def cv_data_gen(adata_sc, adata_sp, cv_mode="loo"):
 def cross_val(adata_sc, adata_sp, cluster_label=None, mode="clusters", scale=True, lambda_d=0, lambda_g1=1, lambda_g2=0,
               lambda_r=0, lambda_count=1, lambda_f_reg=1, target_count=None, num_epochs=1000, device="cuda:0",
               learning_rate=0.1, cv_mode="loo", return_gene_pred=False, density_prior=None, random_state=None,
-              verbose=False, *, precision="bf16x3"):
+              verbose=False, *, precision="bf16x3", process_group=None):
     """:503-668 -- gene cross-validation: for each fold of cv_data_gen, a mapping trained on the fold's training genes
     (as map_cells_to_space(cv_train_genes=...) trains it) scores the held-out genes with compare_spatial_geneexp.
     Returns cv_dict {"avg_test_score", "avg_train_score"} (nanmean over the folds; a fold's train score is the last
@@ -444,18 +444,38 @@ def cross_val(adata_sc, adata_sp, cluster_label=None, mode="clusters", scale=Tru
     training genes (a handle masked to S[:, train] computes what a handle built on those columns computes), redraws
     the initial mapping from numpy's global generator exactly as a fresh mapper would (reseeded when random_state is
     truthy), trains num_epochs with a fresh Adam, and projects only the test genes on the device.  `precision` as in
-    map_cells_to_space."""
+    map_cells_to_space.
+
+    process_group (mode="cells" or "constrained"): the folds' mappings are cell-sharded as in map_cells_to_space -- every
+    rank passes the same AnnDatas, trains its block of cells, projects the test genes from its own rows, and the
+    projections are summed over the group.  The folds and the gene columns follow rank 0's order of the training genes,
+    and every rank returns the same results."""
     logging.getLogger().disabled = True
     logging.getLogger("anndata").disabled = True
+    mu._check_shardable(mode, process_group)
     folds = list(cv_data_gen(adata_sc, adata_sp, cv_mode))
+    sharding = {}
+    if process_group is not None:
+        # uns["training_genes"] comes from a set in pp_adatas, so its order (and with it the folds) can differ between
+        # processes: every rank takes rank 0's folds, as _prepare_mapping takes rank 0's gene order
+        import torch.distributed as dist
+        box = [folds]
+        dist.broadcast_object_list(box, src=dist.get_global_rank(process_group, 0), group=process_group)
+        folds = box[0]
+        sharding = dict(process_group=process_group)
+        if mode == "cells":
+            # the folds draw one after another from numpy's generator: every rank must leave it where the unsharded draw
+            # does (a sharded Mapper's draw stops after the rank's last row otherwise)
+            sharding["draw_whole_stream"] = True
     adata_ref, genes, S, _, mapper_kw = mu._prepare_mapping(
         adata_sc, adata_sp, None, cluster_label, mode, scale, density_prior, lambda_d, lambda_g1, lambda_g2, lambda_r,
-        0, 0, lambda_count, lambda_f_reg, target_count, 0, 0, 0, 0, 0)
+        0, 0, lambda_count, lambda_f_reg, target_count, 0, 0, 0, 0, 0, process_group)
     if mode != "clusters":
         adata_ref = adata_sc
     column = {g: k for k, g in enumerate(genes)}
     test_genes_list, test_pred_list, test_score_list, train_score_list, test_df_list = [], [], [], [], []
-    mapper = mu._make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision)
+    mapper = mu._make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision, **sharding)
+    r0, r1 = getattr(mapper, "_rows", (0, S.shape[0]))
     try:
         for fold, (train_genes, test_genes) in enumerate(folds):
             if fold > 0:                      # the constructor made the first fold's draw
@@ -465,7 +485,8 @@ def cross_val(adata_sc, adata_sp, cluster_label=None, mode="clusters", scale=Tru
             mapper._set_loss_genes(active)
             mapper._fit(num_epochs, float(learning_rate), None, False, fetch=False)
             train_score = float(mapper.history_matrix[-1, 1])                    # main_loss (:622)
-            pred = mapper.project(S[:, [column[g] for g in test_genes]])          # (spots, test genes)
+            pred = mu._sum_over_group(mapper.project(S[r0:r1, [column[g] for g in test_genes]]), mapper,
+                                      process_group)                              # (spots, test genes)
             var = pd.DataFrame({"is_training": np.zeros(len(test_genes), dtype=bool)}, index=test_genes)
             adata_ge = make_adata(X=pred, obs=adata_sp.obs.copy(), var=var, uns=adata_ref.uns)
             df_g = compare_spatial_geneexp(adata_ge, adata_sp, adata_ref, test_genes)
