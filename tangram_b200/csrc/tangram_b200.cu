@@ -1868,6 +1868,11 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
   else if ((nm == "dq" || nm == "Pb") && h->bf16) return widened(nm == "dq" ? h->dq.p : h->Pb.p, nv, 1);
   else if (nm == "rcenter" && h->bf16) { src = h->rcenter.p; cnt = h->N; }
   else if (nm == "rdot") { src = h->rdot.p; cnt = h->N; }
+  // the loss's constant norms of G (per gene, per voxel) and of the graph products W G, (A + I) G (per gene)
+  else if (nm == "ngc") { src = h->ngc.p; cnt = h->K; }
+  else if (nm == "ngr") { src = h->ngr.p; cnt = h->V; }
+  else if (nm == "nwg" && h->nwg.p) { src = h->nwg.p; cnt = h->K; }
+  else if (nm == "nag" && h->nag.p) { src = h->nag.p; cnt = h->K; }
   else if (nm == "Sx") { src = h->Sx.p; cnt = (int64_t)h->N * h->Ke; }
   else if (nm == "tail") { src = h->Y.p + vk; cnt = kTail; }       // the row-scalar sums after Y_ext (k_row_scalar_reduce)
   else if (h->constrained && (nm == "F" || nm == "f" || nm == "mF" || nm == "vF")) {
