@@ -298,6 +298,33 @@ TGB200_API int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
                                 double* pearson_out, float* vote_entropy_out, float* consensus_entropy_out,
                                 int32_t device, void* stream);
 
+/* tgb200_agreement's Pearson pass split around sums over row shards, for a mapping cube whose rows are spread over
+ * several devices or processes (the sharded tuner trial).  Each shard passes its own rows as tgb200_agreement takes
+ * them (same `arrays`, R, rows, cols, ld and checks); the caller sums the outputs over the shards (an all-reduce), which
+ * these entry points never do themselves.  In order:
+ *   tgb200_agreement_sample    sample_out (R + 1 doubles, host or device): the sums of the shard's shift sample of each
+ *                              array (min(rows cols, 4096) elements spread evenly over its rows), then the sample size.
+ *                              Summed over the shards, shift[r] = sum[r] / size is the same on every shard and near the
+ *                              global mean, so that the one-pass cross products keep the accuracy of a centred sum.
+ *   tgb200_agreement_partials  `shift` (R doubles, host or device): that shared shift.  sums_out (R + R(R+1)/2
+ *                              doubles, host or device): sum dx_r, then sum dx_r dx_s for r <= s (row-major upper
+ *                              triangle), dx_r = x_r - shift[r], over the shard's elements in fp64, its per-block partials
+ *                              added in block order.  vote_entropy_out / consensus_entropy_out (rows floats, host or
+ *                              device; NULL to skip): the shard's rows of tgb200_agreement's per-row entropies, bit for bit.
+ *   tgb200_agreement_pearson   sums (R + R(R+1)/2 doubles, host or device): the partials summed over the shards;
+ *                              rows_global x cols: the element count of one whole array.  pearson_out (R(R-1)/2 doubles,
+ *                              host or device): np.corrcoef at np.tril_indices(R, -1); nothing is written for R = 1.
+ * One shard holding every row gives tgb200_agreement's Pearson bits.  Scratch is O(R^2 grid + rows) as there; nothing of
+ * size rows x cols.  TGB200_ERR_INVALID for a null argument, R outside 1..8 or a bad shape; TGB200_ERR_NO_DEVICE without
+ * an sm_90 device.  Synchronous on `stream`. */
+TGB200_API int tgb200_agreement_sample(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                       double* sample_out, int32_t device, void* stream);
+TGB200_API int tgb200_agreement_partials(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                         const double* shift, double* sums_out, float* vote_entropy_out,
+                                         float* consensus_entropy_out, int32_t device, void* stream);
+TGB200_API int tgb200_agreement_pearson(const double* sums, int32_t R, int64_t rows_global, int64_t cols,
+                                        double* pearson_out, int32_t device, void* stream);
+
 /* Annotation transfer from cells onto space (tangram/utils.py:126-153 project_cell_annotations, 205-285
  * count_cell_annotations, 820-842 cell_type_mapping), in one streaming pass over a DEVICE mapping `map` (rows x cols
  * row-major f32, leading dimension ld >= cols, on `device`).  `labels_host`: a HOST array of `rows` int32 labels in

@@ -98,6 +98,12 @@ SIGNATURES = {
     "tgb200_project": (ctypes.c_int, [_P, _P, ctypes.c_int64, _P, _P]),
     "tgb200_agreement": (ctypes.c_int, [ctypes.POINTER(_P), ctypes.c_int32, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                         _P, _P, _P, ctypes.c_int32, _P]),
+    "tgb200_agreement_sample": (ctypes.c_int, [ctypes.POINTER(_P), ctypes.c_int32, ctypes.c_int64, ctypes.c_int64,
+                                               ctypes.c_int64, _P, ctypes.c_int32, _P]),
+    "tgb200_agreement_partials": (ctypes.c_int, [ctypes.POINTER(_P), ctypes.c_int32, ctypes.c_int64, ctypes.c_int64,
+                                                 ctypes.c_int64, _P, _P, _P, _P, ctypes.c_int32, _P]),
+    "tgb200_agreement_pearson": (ctypes.c_int, [_P, ctypes.c_int32, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int32,
+                                                _P]),
     "tgb200_annotate": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int32,
                                        _P, _P, ctypes.c_int32, _P]),
     "tgb200_project_map": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int64,

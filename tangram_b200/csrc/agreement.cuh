@@ -7,6 +7,11 @@
 // block order (no float atomics), so a re-run on the same device gives identical bits.
 // Cancellation: the cross products are taken about a per-array shift (the mean of a fixed strided sample), which makes the
 // one-pass  sum(dx dy) - sum(dx) sum(dy) / n  as accurate as a two-pass centred sum when the shift is near the mean.
+// Row shards (the sharded tuner trial): each shard returns its sample's sums and size (k_agreement_shift with sums = 1);
+// the caller adds them over the shards, so every shard takes its cross products about the same shift, near the global
+// mean; each shard's k_agreement partials are summed in block order (k_agreement_total), the caller adds those over the
+// shards, and k_agreement_pearson finishes with the global element count.  One shard holding every row computes exactly
+// what k_agreement_shift / k_agreement / k_agreement_finish compute.
 #pragma once
 #include "common.cuh"
 
@@ -32,8 +37,9 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
-// shift[r] = mean of kAgrSample elements spread evenly over array r (grid = R blocks of kAgrThreads)
-__global__ void __launch_bounds__(kAgrThreads) k_agreement_shift(AgrArgs a, double* shift) {
+// shift[r] = mean of kAgrSample elements spread evenly over array r (grid = R blocks of kAgrThreads).  With sums != 0
+// shift[r] is the sample's sum instead and shift[R] its size, for a caller that adds the samples of several row shards.
+__global__ void __launch_bounds__(kAgrThreads) k_agreement_shift(AgrArgs a, double* shift, int sums) {
   __shared__ double sh[kAgrThreads];
   const float* x = a.x[0];
 #pragma unroll
@@ -52,7 +58,8 @@ __global__ void __launch_bounds__(kAgrThreads) k_agreement_shift(AgrArgs a, doub
     if (threadIdx.x < w) sh[threadIdx.x] += sh[threadIdx.x + w];
     __syncthreads();
   }
-  if (threadIdx.x == 0) shift[blockIdx.x] = sh[0] / ns;
+  if (threadIdx.x == 0) shift[blockIdx.x] = sums ? sh[0] : sh[0] / ns;
+  if (sums && blockIdx.x == 0 && threadIdx.x == 0) shift[gridDim.x] = (double)ns;
 }
 
 template <int R, bool kRows>
@@ -202,18 +209,18 @@ __global__ void __launch_bounds__(kAgrThreads) k_agreement(AgrArgs a) {
   }
 }
 
-// One block: sums the per-block partials in block order and forms np.corrcoef's pairwise correlations in
-// np.tril_indices(R, -1) order: (1,0), (2,0), (2,1), (3,0), ...
-__global__ void k_agreement_finish(const double* part, int nblocks, int R, double n, double* corr) {
-  __shared__ double tot[kAgrMaxRuns + kAgrMaxRuns * (kAgrMaxRuns + 1) / 2];
-  const int NS = R + R * (R + 1) / 2;
+// Threads [0, NS) of one block: tot[k] = sum of the per-block partials part[b][k] in block order.
+__device__ __forceinline__ void agr_total(const double* part, int nblocks, int NS, double* tot) {
   if (threadIdx.x < NS) {
     double t = 0.0;
     for (int b = 0; b < nblocks; ++b) t += part[(size_t)b * NS + threadIdx.x];
     tot[threadIdx.x] = t;
   }
-  __syncthreads();
-  if (threadIdx.x != 0) return;
+}
+
+// One thread: np.corrcoef's pairwise correlations from the sums tot (sum dx_r, then sum dx_r dx_s for r <= s) of n
+// elements per array, in np.tril_indices(R, -1) order: (1,0), (2,0), (2,1), (3,0), ...
+__device__ __forceinline__ void agr_pearson(const double* tot, int R, double n, double* corr) {
   auto pidx = [R](int r, int s) { return R + r * R - r * (r - 1) / 2 + (s - r); };   // r <= s
   auto cov = [&](int r, int s) { return (tot[pidx(r, s)] - tot[r] * tot[s] / n) / (n - 1.0); };
   int k = 0;
@@ -222,6 +229,25 @@ __global__ void k_agreement_finish(const double* part, int nblocks, int R, doubl
       double c = cov(j, i) / sqrt(cov(i, i)) / sqrt(cov(j, j));
       corr[k] = c > 1.0 ? 1.0 : (c < -1.0 ? -1.0 : c);           // np.corrcoef clips to [-1, 1]
     }
+}
+
+// One block: sums the per-block partials in block order and forms the correlations (tgb200_agreement).
+__global__ void k_agreement_finish(const double* part, int nblocks, int R, double n, double* corr) {
+  __shared__ double tot[kAgrMaxRuns + kAgrMaxRuns * (kAgrMaxRuns + 1) / 2];
+  agr_total(part, nblocks, R + R * (R + 1) / 2, tot);
+  __syncthreads();
+  if (threadIdx.x == 0) agr_pearson(tot, R, n, corr);
+}
+
+// The two halves of k_agreement_finish for row shards (tgb200_agreement_partials, tgb200_agreement_pearson): one block
+// of at least R + R(R+1)/2 threads sums a shard's partials into tot; one thread forms the correlations from the sums
+// of every shard.
+__global__ void k_agreement_total(const double* part, int nblocks, int R, double* tot) {
+  agr_total(part, nblocks, R + R * (R + 1) / 2, tot);
+}
+
+__global__ void k_agreement_pearson(const double* tot, int R, double n, double* corr) {
+  if (threadIdx.x == 0) agr_pearson(tot, R, n, corr);
 }
 
 }  // namespace tgb

@@ -1951,28 +1951,41 @@ static void launch_agreement(const AgrArgs& a, int grid, bool rows, cudaStream_t
   else k_agreement<R, false><<<grid, kAgrThreads, 0, s>>>(a);
 }
 
-extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
-                                double* pearson_out, float* vote_out, float* cons_out, int32_t device, void* stream) {
-  if (!arrays) return fail(TGB200_ERR_INVALID, "null argument");
+static void launch_agreement(const AgrArgs& a, int R, int grid, bool rows, cudaStream_t s) {
+  switch (R) {
+    case 1: launch_agreement<1>(a, grid, rows, s); break;
+    case 2: launch_agreement<2>(a, grid, rows, s); break;
+    case 3: launch_agreement<3>(a, grid, rows, s); break;
+    case 4: launch_agreement<4>(a, grid, rows, s); break;
+    case 5: launch_agreement<5>(a, grid, rows, s); break;
+    case 6: launch_agreement<6>(a, grid, rows, s); break;
+    case 7: launch_agreement<7>(a, grid, rows, s); break;
+    default: launch_agreement<8>(a, grid, rows, s); break;
+  }
+}
+
+// The checks every agreement entry point makes on its arrays, in this order: R, the shape, the device, each array.
+// Fills the arrays, shape and load width of *a and, if grid is given, the grid of k_agreement<R, rows>: enough blocks
+// for every row, at most what fits on the device at once.
+static int agreement_setup(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld, int32_t device,
+                           bool per_row, AgrArgs* a, int* grid) {
   if (R < 1 || R > kAgrMaxRuns) return fail(TGB200_ERR_INVALID, "R=%d runs, supported 1..%d", R, kAgrMaxRuns);
   if (rows <= 0 || cols <= 0 || ld < cols || cols > INT32_MAX)
     return fail(TGB200_ERR_INVALID, "bad shape rows=%lld cols=%lld ld=%lld", (long long)rows, (long long)cols, (long long)ld);
   int n_sms = 0;
   CKS(use_sm90_device(device, &n_sms));
-  AgrArgs a{};
-  a.rows = rows; a.cols = cols; a.ld = ld;
-  a.vec = ld % 4 == 0;
+  *a = AgrArgs{};
+  a->rows = rows; a->cols = cols; a->ld = ld;
+  a->vec = ld % 4 == 0;
   for (int r = 0; r < R; ++r) {
     if (!arrays[r]) return fail(TGB200_ERR_INVALID, "array %d is null", r);
     char what[32];
     snprintf(what, sizeof(what), "array %d", r);
     CKS(require_device_memory(arrays[r], device, what));
-    a.x[r] = arrays[r];
-    if (reinterpret_cast<uintptr_t>(arrays[r]) % 16) a.vec = 0;
+    a->x[r] = arrays[r];
+    if (reinterpret_cast<uintptr_t>(arrays[r]) % 16) a->vec = 0;
   }
-  cudaStream_t s = (cudaStream_t)stream;
-  const bool per_row = vote_out || cons_out;
-  const int NS = R + R * (R + 1) / 2;
+  if (!grid) return TGB200_OK;
   int per_sm = 0;
 #define AGR_OCC(RR) \
   case RR: CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, per_row ? k_agreement<RR, true> : k_agreement<RR, false>, kAgrThreads, 0)); break;
@@ -1980,7 +1993,19 @@ extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
 #undef AGR_OCC
   const int warps = kAgrThreads / kWarp;
   const int64_t need = ceil_div(rows, warps);
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)std::max(per_sm, 1) * n_sms));
+  *grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)std::max(per_sm, 1) * n_sms));
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                double* pearson_out, float* vote_out, float* cons_out, int32_t device, void* stream) {
+  if (!arrays) return fail(TGB200_ERR_INVALID, "null argument");
+  const bool per_row = vote_out || cons_out;
+  AgrArgs a;
+  int grid = 0;
+  CKS(agreement_setup(arrays, R, rows, cols, ld, device, per_row, &a, &grid));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int NS = R + R * (R + 1) / 2;
   // scratch is O(R^2 grid + rows): the per-block partials, the shifts, the correlations, the per-row results
   DevBuf<double> shift, part, corr;
   DevBuf<float> vote, cons;
@@ -1988,18 +2013,9 @@ extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
   if (vote_out) CKS(vote.alloc(rows, false));
   if (cons_out) CKS(cons.alloc(rows, false));
   a.shift = shift.p; a.part = part.p; a.vote = vote.p; a.cons = cons.p;
-  k_agreement_shift<<<R, kAgrThreads, 0, s>>>(a, shift.p);
+  k_agreement_shift<<<R, kAgrThreads, 0, s>>>(a, shift.p, 0);
   CK(cudaGetLastError());
-  switch (R) {
-    case 1: launch_agreement<1>(a, grid, per_row, s); break;
-    case 2: launch_agreement<2>(a, grid, per_row, s); break;
-    case 3: launch_agreement<3>(a, grid, per_row, s); break;
-    case 4: launch_agreement<4>(a, grid, per_row, s); break;
-    case 5: launch_agreement<5>(a, grid, per_row, s); break;
-    case 6: launch_agreement<6>(a, grid, per_row, s); break;
-    case 7: launch_agreement<7>(a, grid, per_row, s); break;
-    default: launch_agreement<8>(a, grid, per_row, s); break;
-  }
+  launch_agreement(a, R, grid, per_row, s);
   CK(cudaGetLastError());
   if (R > 1) {
     k_agreement_finish<<<1, 64, 0, s>>>(part.p, grid, R, (double)rows * (double)cols, corr.p);
@@ -2008,6 +2024,71 @@ extern "C" int tgb200_agreement(const float* const* arrays, int32_t R, int64_t r
   }
   if (vote_out) CK(cudaMemcpyAsync(vote_out, vote.p, sizeof(float) * rows, cudaMemcpyDefault, s));
   if (cons_out) CK(cudaMemcpyAsync(cons_out, cons.p, sizeof(float) * rows, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+// tgb200_agreement in three steps around the caller's sums over row shards.
+extern "C" int tgb200_agreement_sample(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                       double* sample_out, int32_t device, void* stream) {
+  if (!arrays || !sample_out) return fail(TGB200_ERR_INVALID, "null argument");
+  AgrArgs a;
+  CKS(agreement_setup(arrays, R, rows, cols, ld, device, false, &a, nullptr));
+  cudaStream_t s = (cudaStream_t)stream;
+  DevBuf<double> out;
+  CKS(out.alloc(R + 1, false));
+  k_agreement_shift<<<R, kAgrThreads, 0, s>>>(a, out.p, 1);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(sample_out, out.p, sizeof(double) * (R + 1), cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_agreement_partials(const float* const* arrays, int32_t R, int64_t rows, int64_t cols, int64_t ld,
+                                         const double* shift, double* sums_out, float* vote_out, float* cons_out,
+                                         int32_t device, void* stream) {
+  if (!arrays || !shift || !sums_out) return fail(TGB200_ERR_INVALID, "null argument");
+  const bool per_row = vote_out || cons_out;
+  AgrArgs a;
+  int grid = 0;
+  CKS(agreement_setup(arrays, R, rows, cols, ld, device, per_row, &a, &grid));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int NS = R + R * (R + 1) / 2;
+  DevBuf<double> sh, part, tot;
+  DevBuf<float> vote, cons;
+  CKS(sh.alloc(R, false)); CKS(part.alloc((size_t)grid * NS, false)); CKS(tot.alloc(NS, false));
+  if (vote_out) CKS(vote.alloc(rows, false));
+  if (cons_out) CKS(cons.alloc(rows, false));
+  CK(cudaMemcpyAsync(sh.p, shift, sizeof(double) * R, cudaMemcpyDefault, s));
+  a.shift = sh.p; a.part = part.p; a.vote = vote.p; a.cons = cons.p;
+  launch_agreement(a, R, grid, per_row, s);
+  CK(cudaGetLastError());
+  k_agreement_total<<<1, 64, 0, s>>>(part.p, grid, R, tot.p);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(sums_out, tot.p, sizeof(double) * NS, cudaMemcpyDefault, s));
+  if (vote_out) CK(cudaMemcpyAsync(vote_out, vote.p, sizeof(float) * rows, cudaMemcpyDefault, s));
+  if (cons_out) CK(cudaMemcpyAsync(cons_out, cons.p, sizeof(float) * rows, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_agreement_pearson(const double* sums, int32_t R, int64_t rows_global, int64_t cols,
+                                        double* pearson_out, int32_t device, void* stream) {
+  if (!sums || !pearson_out) return fail(TGB200_ERR_INVALID, "null argument");
+  if (R < 1 || R > kAgrMaxRuns) return fail(TGB200_ERR_INVALID, "R=%d runs, supported 1..%d", R, kAgrMaxRuns);
+  if (rows_global <= 0 || cols <= 0)
+    return fail(TGB200_ERR_INVALID, "bad shape rows=%lld cols=%lld", (long long)rows_global, (long long)cols);
+  int n_sms = 0;
+  CKS(use_sm90_device(device, &n_sms));
+  if (R == 1) return TGB200_OK;                        // no pair
+  cudaStream_t s = (cudaStream_t)stream;
+  const int NS = R + R * (R + 1) / 2, NP = R * (R - 1) / 2;
+  DevBuf<double> tot, corr;
+  CKS(tot.alloc(NS, false)); CKS(corr.alloc(NP, false));
+  CK(cudaMemcpyAsync(tot.p, sums, sizeof(double) * NS, cudaMemcpyDefault, s));
+  k_agreement_pearson<<<1, 32, 0, s>>>(tot.p, R, (double)rows_global * (double)cols, corr.p);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(pearson_out, corr.p, sizeof(double) * NP, cudaMemcpyDefault, s));
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
 }

@@ -13,7 +13,8 @@ streaming pass each (tgb200_agreement), with no N x V scratch and no float64 cop
     metrics = train_multiple_Mapper(config, data)     # the five numbers the reference reports to ray.train.report
 
 makes a Ray trainable a one-line wrapper.  The Ray / Optuna driver `mapping_hyperparameter_tuning` itself stays with the
-reference.
+reference.  With `process_group=` (NCCL, one process per GPU) the trial shards the cells of every run over the group, and
+`agreement(..., process_group=)` scores a cube whose rows are spread over the ranks.
 """
 import ctypes
 
@@ -22,6 +23,7 @@ import numpy as np
 from . import _lib
 from .engine import _require_device
 from .mapping_optimizer import Mapper
+from .sharded import shard_rows
 
 _CONFIG_LAMBDAS = ["lambda_d", "lambda_g1", "lambda_g2", "lambda_neighborhood_g1", "lambda_r", "lambda_l1",
                    "lambda_l2", "lambda_ct_islands", "lambda_getis_ord"]     # :97
@@ -61,10 +63,15 @@ def _runs_on_device(cube, device):
     return out, dev
 
 
-def agreement(cube, *, pearson=True, vote=False, consensus=False, device=None):
+def agreement(cube, *, pearson=True, vote=False, consensus=False, device=None, process_group=None):
     """One pass of tgb200_agreement over the R runs of `cube`: -> (pearson (R(R-1)/2,) float64 or None,
     vote entropy (N,) float32 or None, consensus entropy (N,) float32 or None).  `device` places host data (default:
-    the current CUDA device); device data is read where it lives."""
+    the current CUDA device); device data is read where it lives.
+
+    process_group: `cube` holds this rank's rows of a cube whose rows are spread over the group's ranks (the same R and
+    V everywhere, any number of rows each).  A collective: the ranks' shift samples and Pearson sums are summed over the
+    group (tgb200_agreement_sample / _partials / _pearson), so every rank gets the same Pearson values, those of the
+    whole cube; the entropies are this rank's rows.  With one rank the result is tgb200_agreement's, bit for bit."""
     import torch
     runs, dev = _runs_on_device(cube, device)
     R = len(runs)
@@ -75,8 +82,36 @@ def agreement(cube, *, pearson=True, vote=False, consensus=False, device=None):
     v = np.empty(rows, dtype=np.float32) if vote else None
     c = np.empty(rows, dtype=np.float32) if consensus else None
     stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(lib.tgb200_agreement(ptrs, R, rows, cols, runs[0].stride(0), _lib.ptr(p), _lib.ptr(v), _lib.ptr(c),
-                                    dev, stream))
+    if process_group is None:
+        _lib.check(lib.tgb200_agreement(ptrs, R, rows, cols, runs[0].stride(0), _lib.ptr(p), _lib.ptr(v),
+                                        _lib.ptr(c), dev, stream))
+        return p, v, c
+    import torch.distributed as dist
+    ld = runs[0].stride(0)
+
+    def all_reduce(t):
+        """in-place sum over the group: on the device for NCCL, on the host for other backends"""
+        if dist.get_backend(process_group) == "nccl":
+            dist.all_reduce(t, group=process_group)
+            return t
+        h = t.cpu()
+        dist.all_reduce(h, group=process_group)
+        return h.to(t.device)
+
+    f64 = dict(dtype=torch.float64, device=f"cuda:{dev}")
+    # [R sample sums, sample size, rows]: the shared shift and the global row count from one all-reduce
+    sample = torch.empty(R + 2, **f64)
+    _lib.check(lib.tgb200_agreement_sample(ptrs, R, rows, cols, ld, _lib.ptr(sample), dev, stream))
+    sample[R + 1] = rows
+    sample = all_reduce(sample).cpu().numpy()
+    shift = sample[:R] / sample[R]        # what k_agreement_shift divides on the device: the same bits for one rank
+    rows_global = int(sample[R + 1])
+    sums = torch.empty(R + R * (R + 1) // 2, **f64)
+    _lib.check(lib.tgb200_agreement_partials(ptrs, R, rows, cols, ld, _lib.ptr(shift), _lib.ptr(sums), _lib.ptr(v),
+                                             _lib.ptr(c), dev, stream))
+    sums = all_reduce(sums)
+    if pearson:
+        _lib.check(lib.tgb200_agreement_pearson(_lib.ptr(sums), R, rows_global, cols, _lib.ptr(p), dev, stream))
     return p, v, c
 
 
@@ -99,7 +134,7 @@ def consensus_entropy(pred_probs_cube, *, device=None):
     return agreement(pred_probs_cube, pearson=False, consensus=True, device=device)[2]
 
 
-def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details=None):
+def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details=None, process_group=None):
     """:86-139 -- train the configuration `config` n_runs times (random_state = 0, 1, 2, ...) on `data`, the reference's
     12-entry list [S, G, d_source, d, device, print_each, voxel_weights, ct_encode, neighborhood_filter, spatial_weights,
     train_genes_idx, val_genes_idx], and return the five metrics the reference reports:
@@ -112,12 +147,28 @@ def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details
     global generator.  The mappings stay on the device (an R x N x V cube), the validation genes are projected there,
     and each run's handle is released before the next starts.  `details`, if a dict, receives the device cubes
     ("cell_cube" R x N x V, "gene_cube" R x V x n_val), the per-run "val_gene_sim" and the seconds spent in "train_s",
-    "project_s" and "score_s"."""
+    "project_s" and "score_s".
+
+    process_group: a torch.distributed NCCL group, one process per GPU, shards the cells as Mapper(process_group=) does.
+    Every rank passes the same `data` with its own device in data[4], and every rank must enter with the same state of
+    numpy's global generator (run 0 draws from it; nothing broadcasts it): each rank then leaves it where the unsharded
+    trial leaves it.  Each rank holds an R x N_r x V cube of its rows shard_rows(N, rank, world) (the memory check
+    counts those rows only); the validation genes projected from a rank's rows are summed over the group, so every rank
+    holds the whole gene cube; the cell metrics come from agreement(process_group=) and from the entropies summed over
+    the group.  Every rank returns the same five metrics.  `details` also receives "shard_rows" (r0, r1), and
+    "cell_cube" is the rank's own rows.  A non-NCCL group and n_runs > 8 are refused before any training."""
     import time
 
     import torch
     (S, G, d_source, d, device, print_each, voxel_weights, ct_encode, neighborhood_filter, spatial_weights,
      train_genes_idx, val_genes_idx) = data
+    if process_group is not None:
+        import torch.distributed as dist
+        if n_runs > 8:
+            raise ValueError(f"a sharded trial scores at most 8 runs (the agreement pass takes 1..8), got n_runs={n_runs}")
+        if dist.get_backend(process_group) != "nccl":
+            raise ValueError("a sharded trial needs an NCCL process group: each run's final validation of the sharded "
+                             "mapping sums its forward on the group's NCCL communicator, which a non-NCCL group lacks")
     dev = _require_device(device)
     hyperparameters = {"d_source": d_source}
     for param in _CONFIG_LAMBDAS:
@@ -128,20 +179,24 @@ def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details
 
     S = np.asarray(S, dtype=np.float32)
     N, V = S.shape[0], np.shape(G)[0]
-    S_val = np.ascontiguousarray(S[:, val_genes_idx] if val_genes_idx is not None else S)
+    r0, r1 = (0, N) if process_group is None else shard_rows(N, dist.get_rank(process_group),
+                                                                 dist.get_world_size(process_group))
+    N_r = r1 - r0
+    S_val = np.ascontiguousarray(S[r0:r1, val_genes_idx] if val_genes_idx is not None else S[r0:r1])
     n_val = S_val.shape[1]
     k_train = len(train_genes_idx) if train_genes_idx is not None else S.shape[1]
-    cube_bytes = 4 * n_runs * N * V + 4 * n_runs * V * n_val
-    handle_bytes = _HANDLE_BYTES_PER_ELEMENT * N * V + 16 * (N + V) * (k_train + n_val)
+    cube_bytes = 4 * n_runs * N_r * V + 4 * n_runs * V * n_val
+    handle_bytes = _HANDLE_BYTES_PER_ELEMENT * N_r * V + 16 * (N_r + V) * (k_train + n_val)
     free, _ = torch.cuda.mem_get_info(dev)
     if cube_bytes + handle_bytes > free:
         raise _lib.TangramB200Error(
             f"train_multiple_Mapper needs about {(cube_bytes + handle_bytes) / 2**30:.1f} GiB on cuda:{dev} "
-            f"({n_runs} mappings of {N} x {V} = {cube_bytes / 2**30:.1f} GiB, plus one mapper of "
+            f"({n_runs} mappings of {N_r} x {V} = {cube_bytes / 2**30:.1f} GiB, plus one mapper of "
             f"{handle_bytes / 2**30:.1f} GiB); {free / 2**30:.1f} GiB are free")
 
+    sharding = {} if process_group is None else dict(process_group=process_group, draw_whole_stream=True)
     t_train = t_proj = 0.0
-    cell_cube = torch.empty((n_runs, N, V), dtype=torch.float32, device=f"cuda:{dev}")
+    cell_cube = torch.empty((n_runs, N_r, V), dtype=torch.float32, device=f"cuda:{dev}")
     gene_cube = torch.empty((n_runs, V, n_val), dtype=torch.float32, device=f"cuda:{dev}")   # (S_val^T P)^T
     val_gene_scores = []
     for run in range(n_runs):
@@ -149,15 +204,18 @@ def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details
         mapper = Mapper(S=S, G=G, d=d, train_genes_idx=train_genes_idx, val_genes_idx=val_genes_idx,
                         voxel_weights=voxel_weights, neighborhood_filter=neighborhood_filter, ct_encode=ct_encode,
                         spatial_weights=spatial_weights, device=f"cuda:{dev}", random_state=run, precision=precision,
-                        **hyperparameters)
+                        **hyperparameters, **sharding)
         try:
             # the reference validates after every update (val_each=1) and keeps only the last score: one evaluation
-            # after the final update is the same number
+            # after the final update is the same number (sharded: a collective over the group)
             mapper.train(num_epochs, learning_rate=learning_rate, print_each=print_each, out=cell_cube[run])
             val_gene_scores.append(mapper.validation_terms()["val_gene_sim"])
             t1 = time.perf_counter()
             # :134 -- S[:, val]^T @ mapping, stored transposed: Pearson over flattened runs does not see the order
             mapper.project(S_val, out=gene_cube[run])
+            if process_group is not None:
+                dist.all_reduce(gene_cube[run], group=process_group)     # the projection of every cell
+                torch.cuda.current_stream(dev).synchronize()
             t2 = time.perf_counter()
         finally:
             mapper.release()
@@ -165,14 +223,24 @@ def train_multiple_Mapper(config, data, *, n_runs=3, precision="bf16x3", details
         t_proj += t2 - t1
 
     t0 = time.perf_counter()
-    cell_p, cell_v, cell_c = agreement(cell_cube, vote=True, consensus=True)
+    cell_p, cell_v, cell_c = agreement(cell_cube, vote=True, consensus=True, process_group=process_group)
     gene_p = agreement(gene_cube)[0]
+    if process_group is None:
+        vote_mean, cons_mean = cell_v.astype(np.float64).mean(), cell_c.astype(np.float64).mean()
+    else:
+        # sum over every rank's rows / n_cells_global: with one rank, the operation .mean() performs
+        sums = torch.tensor([cell_v.astype(np.float64).sum(), cell_c.astype(np.float64).sum()], dtype=torch.float64,
+                            device=f"cuda:{dev}")
+        dist.all_reduce(sums, group=process_group)
+        vote_mean, cons_mean = sums.cpu().numpy() / N
     t_score = time.perf_counter() - t0
     if isinstance(details, dict):
         details.update(cell_cube=cell_cube, gene_cube=gene_cube, val_gene_sim=val_gene_scores, train_s=t_train,
                        project_s=t_proj, score_s=t_score)
+        if process_group is not None:
+            details["shard_rows"] = (r0, r1)
     return {"cell_map_consistency": float(cell_p.mean()),
-            "cell_map_agreement": float(1 - cell_v.astype(np.float64).mean()),
-            "cell_map_certainty": float(1 - cell_c.astype(np.float64).mean()),
+            "cell_map_agreement": float(1 - vote_mean),
+            "cell_map_certainty": float(1 - cons_mean),
             "gene_expr_consistency": float(gene_p.mean()),
             "gene_expr_correctness": float(np.mean(val_gene_scores))}
