@@ -7,6 +7,15 @@
     tg.project_cell_annotations(ad_map, ad_sp, annotation="cell_type")   # ad_sp.obsm["tangram_ct_pred"]
     cv_dict = tg.cross_val(ad_sc, ad_sp, cluster_label="cell_type", cv_mode="10fold")   # gene cross-validation
     metrics = tg.train_multiple_Mapper(config, data)     # the tuner's trial: five run-to-run agreement metrics
+
+One process per GPU (process_group=pg, cells and constrained mode): every rank passes the same AnnDatas and gets its
+block of the mapping; project_genes, project_cell_annotations, cell_type_mapping and count_cell_annotations then take that
+block with the same process_group= and return (or write) the result of the whole mapping on every rank.  They run on
+torch's current CUDA device, so each rank selects its GPU first:
+    torch.cuda.set_device(rank)
+    ad_map = tg.map_cells_to_space(ad_sc, ad_sp, device=f"cuda:{rank}", process_group=pg)   # this rank's cells
+    ad_ge = tg.project_genes(ad_map, ad_sc, process_group=pg)
+    tg.count_cell_annotations(ad_map, ad_sc, ad_sp, annotation="cell_type", process_group=pg)
 """
 from .mapping_optimizer import Mapper, MapperConstrained  # noqa: F401
 from .sharded import shard_rows  # noqa: F401

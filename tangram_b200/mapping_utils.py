@@ -14,6 +14,7 @@ import pandas as pd
 from . import mapping_optimizer as mo
 from . import spatial_weights as sw
 from .adata import make_adata
+from .engine import _device_index
 
 
 def _dense_f32(X):
@@ -210,15 +211,17 @@ def _check_shardable(mode, process_group):
                          "(clusters mode has too few rows).")
 
 
-def _sum_over_group(partial, mapper, process_group):
-    """A projection of this rank's cells (softmax(M)[r0:r1]^T X) -> the sum over the group's ranks, the projection of every
-    cell, the same on every rank; unchanged without a group."""
+def _sum_over_group(partial, device, process_group):
+    """A sum over this rank's cells (a projection softmax(M)[r0:r1]^T X, per-label sums, counts) -> the sum over the
+    group's ranks, the sum over every cell, the same on every rank, in the partial's dtype; unchanged without a group.
+    An NCCL group sums on CUDA device `device` (an ordinal; None: torch's current device), any other backend on the
+    host."""
     if process_group is None:
         return partial
     import torch
     import torch.distributed as dist
     t = torch.from_numpy(np.ascontiguousarray(partial))
-    t = t.cuda(mapper._cfg.device) if dist.get_backend(process_group) == "nccl" else t
+    t = t.cuda(device) if dist.get_backend(process_group) == "nccl" else t
     dist.all_reduce(t, group=process_group)
     return t.cpu().numpy()
 
@@ -281,7 +284,7 @@ def map_cells_to_space(
         adata_map.obs["F_out"] = F_out                                            # :398-399
 
     # per-gene training score (:401-410): softmax(M)^T S on the device instead of a host GEMM
-    G_predicted = _sum_over_group(mapper.project(S[r0:r1]), mapper, process_group)
+    G_predicted = _sum_over_group(mapper.project(S[r0:r1]), _device_index(device), process_group)
     num = (G * G_predicted).sum(axis=0)
     den = np.linalg.norm(G, axis=0) * np.linalg.norm(G_predicted, axis=0)
     df_cs = pd.DataFrame(num / den, list(training_genes), columns=["train_score"])

@@ -10,6 +10,11 @@
 The annotation calls read the mapping once on the device (`annotate`, tgb200_annotate): per-label fp64 column sums
 instead of the reference's float64 upcast GEMM, and the row argmax instead of np.argmax over the host array.  There is
 no CPU path.
+
+project_genes and the three annotation calls take process_group=: `adata_map` is then the rank's block of a cell-sharded
+mapping (map_cells_to_space(process_group=)), each rank computes its partial sums from its own rows with the same
+kernels, the partials are added over the group, and every rank gets the result of the whole mapping, with no gather.
+They run (and an NCCL group sums) on torch's current CUDA device: each rank calls torch.cuda.set_device(rank) first.
 """
 import ctypes
 import logging
@@ -20,7 +25,7 @@ import pandas as pd
 from . import _lib
 from . import mapping_utils as mu
 from .adata import make_adata
-from .engine import _require_device
+from .engine import _device_index, _require_device
 
 _ANN_CHUNK, _ANN_SLAB = 128, 1024       # rows per work item and columns per slab of tgb200_annotate
 
@@ -39,26 +44,91 @@ def _sm90_device(mapping):
     return dev if torch.cuda.get_device_capability(dev) == (9, 0) else None
 
 
-def project_genes(adata_map, adata_sc, cluster_label=None, scale=True):
+def _agree_on_shards(adata_map, process_group, n_cells=None, refusal=None, labels=None):
+    """The first collective of a transfer call on a cell-sharded mapping (`adata_map`: the AnnData that
+    map_cells_to_space(process_group=) returned on this rank): one all_gather_object of every rank's uns["shard_rows"],
+    of what `refusal(r0, r1)` finds wrong on this rank (a message or None) and of `labels`.  Every rank then checks the
+    same facts -- every rank has its rows, each mapping holds as many rows as its block, the blocks tile [0, n_cells)
+    (default: up to the last block's end) in rank order, no rank refused -- and raises the same ValueError, so no rank is
+    left waiting in a reduction the others never enter.  -> (r0, r1, every rank's `labels` in rank order)."""
+    import torch.distributed as dist
+    rows, refused = adata_map.uns.get("shard_rows"), None
+    if rows is not None:
+        try:
+            r0, r1 = (int(r) for r in rows)
+        except (TypeError, ValueError):
+            r0 = r1 = None
+        if r0 is None:
+            rows, refused = None, f"uns['shard_rows'] = {rows!r} is not a pair of rows"
+        else:
+            rows = (r0, r1)
+            if adata_map.X.shape[0] != r1 - r0:
+                refused = f"its mapping has {adata_map.X.shape[0]} rows for uns['shard_rows'] = {rows}"
+            elif refusal is not None:
+                refused = refusal(r0, r1)
+    box = [None] * dist.get_world_size(process_group)
+    dist.all_gather_object(box, (rows, refused, labels), group=process_group)
+    missing = [k for k, (r, _, _) in enumerate(box) if r is None]
+    if missing:
+        raise ValueError(f"rank(s) {missing} passed a mapping without uns['shard_rows']: every rank must pass the AnnData "
+                         "that map_cells_to_space(process_group=) returned on it"
+                         + "".join(f"; rank {k}: {box[k][1]}" for k in missing if box[k][1]))
+    blocks = [r for r, _, _ in box]
+    end = 0
+    for r0, r1 in blocks:
+        if r0 != end or r1 < r0:
+            raise ValueError(f"the ranks' mapping rows {blocks} do not tile the cells in rank order")
+        end = r1
+    if n_cells is not None and end != n_cells:
+        raise ValueError(f"the ranks' mapping rows {blocks} cover {end} cells of the {n_cells} in adata_sc")
+    refusals = [f"rank {k}: {e}" for k, (_, e, _) in enumerate(box) if e]
+    if refusals:
+        raise ValueError("; ".join(refusals))
+    r0, r1 = blocks[dist.get_rank(process_group)]
+    return r0, r1, [lab for _, _, lab in box]
+
+
+def project_genes(adata_map, adata_sc, cluster_label=None, scale=True, *, process_group=None):
     """:338-374 -- adata_map.X^T adata_sc.X over every gene kept, as a (spots x genes) AnnData.  With the mapper kept on
     the device (map_cells_to_space(keep_on_device=True)) it projects through that handle; otherwise, on an sm_90 device,
-    through `project` (a sparse adata_sc.X is streamed as CSR, never densified on the host); without one, on the host."""
+    through `project` (a sparse adata_sc.X is streamed as CSR, never densified on the host); without one, on the host.
+
+    process_group: `adata_map` is this rank's block of a cell-sharded mapping (map_cells_to_space(process_group=)),
+    `adata_sc` the full AnnData, the same on every rank.  A collective: each rank filters the genes of the whole adata_sc
+    (so the columns agree), projects adata_sc.X[r0:r1] through its rows and the (spots x genes) partials are summed over
+    the group; every rank returns the same AnnData, the projection of every cell.  Refused with ValueError on every rank
+    when a rank has no uns["shard_rows"], the blocks do not tile adata_sc's cells in rank order, a rank's obs index is not
+    its block of adata_sc.obs.index, or cluster_label is given (clusters mode is never sharded)."""
     adata_sc.var.index = [g.lower() for g in adata_sc.var.index]                 # :353
     adata_sc.var_names_make_unique()                                              # :356
     keep = np.asarray((adata_sc.X != 0).sum(axis=0)).reshape(-1) >= 1             # :359
     if not keep.all():
         adata_sc = adata_sc[:, keep]
-    if cluster_label:
-        adata_sc = mu.adata_to_cluster_expression(adata_sc, cluster_label, scale=scale)
-    if not adata_map.obs.index.equals(adata_sc.obs.index):
-        raise ValueError("The two AnnDatas need to have same `obs` index.")
-    mapper = getattr(adata_map, "_tgb200_mapper", None)
-    if mapper is not None and mapper.n_cells == adata_sc.X.shape[0]:
-        X_space = mapper.project(_dense(adata_sc.X))   # softmax(M)^T X on the device (:368 is a host GEMM)
-    elif (dev := _sm90_device(adata_map.X)) is not None:
-        X_space = project(adata_map.X, adata_sc.X, device=f"cuda:{dev}")
+    X_sc = adata_sc.X
+    if process_group is not None:
+        def refusal(r0, r1):
+            if cluster_label:
+                return "cluster_label projects a clusters-mode mapping, and clusters mode is never sharded"
+            if not adata_map.obs.index.equals(adata_sc.obs.index[r0:r1]):
+                return f"its mapping's obs index is not rows [{r0}, {r1}) of adata_sc.obs.index"
+            return None
+        r0, r1, _ = _agree_on_shards(adata_map, process_group, adata_sc.X.shape[0], refusal)
+        X_sc = X_sc[r0:r1]
     else:
-        X_space = np.asarray(adata_map.X).T @ _dense(adata_sc.X)
+        if cluster_label:
+            adata_sc = mu.adata_to_cluster_expression(adata_sc, cluster_label, scale=scale)
+            X_sc = adata_sc.X
+        if not adata_map.obs.index.equals(adata_sc.obs.index):
+            raise ValueError("The two AnnDatas need to have same `obs` index.")
+    mapper = getattr(adata_map, "_tgb200_mapper", None)
+    if mapper is not None and process_group is None and mapper.n_cells == X_sc.shape[0]:
+        X_space = mapper.project(_dense(X_sc))   # softmax(M)^T X on the device (:368 is a host GEMM)
+    else:
+        if (dev := _sm90_device(adata_map.X)) is not None:
+            X_space = project(adata_map.X, X_sc, device=f"cuda:{dev}")
+        else:
+            X_space = np.asarray(adata_map.X).T @ _dense(X_sc)
+        X_space = mu._sum_over_group(X_space, dev, process_group)
     adata_ge = make_adata(X=X_space, obs=adata_map.var, var=adata_sc.var, uns=adata_sc.uns)
     training_genes = adata_map.uns["train_genes_df"].index.values
     adata_ge.var["is_training"] = adata_ge.var.index.isin(training_genes)
@@ -214,20 +284,37 @@ def project(mapping, X, *, device=None, _block_rows=0):
     return out
 
 
-def _label_columns(series):
+def _label_columns(series, columns=None):
     """-> (the one-hot columns of tangram/utils.py:105-123 for `series`: its unique values in order of first appearance, a
-    NaN included, each row's position among them).  The positions are taken by position, whatever the index."""
+    NaN included, each row's position among them).  The positions are taken by position, whatever the index.  Given
+    `columns` (a list holding every value of `series`), the positions are taken among those instead."""
     values = pd.Series(series).reset_index(drop=True)
-    columns = pd.unique(values)
+    if columns is None:
+        columns = pd.unique(values)
     codes = pd.Index(columns).get_indexer(values)
     return columns, values, codes
 
 
-def _one_hot_codes(series):
+def _one_hot_codes(series, columns=None):
     """-> (one-hot columns, per-row column for the one-hot product): a NaN label has a column but matches no row there
     (NaN == NaN is false in one_hot_encoding), so its rows add nothing."""
-    columns, values, codes = _label_columns(series)
+    columns, values, codes = _label_columns(series, columns)
     return columns, np.where(values.isna().to_numpy(), -1, codes)
+
+
+def _annotation_codes(adata_map, key, process_group):
+    """_one_hot_codes of adata_map.obs[key].  With a group (`adata_map` one rank's block of a cell-sharded mapping) this is
+    the call's agreement step (_agree_on_shards), and the columns are the whole mapping's: pd.unique of the ranks' labels
+    in their order of first appearance, concatenated in rank order.  The blocks are contiguous, so that is the global
+    order of first appearance, with one NaN column where the first NaN appears.  The concatenation is taken in the
+    column's own dtype, so pd.unique compares the labels as it does on the whole column: in an object Series the float
+    NaNs that come back from the gather are not taken as equal, and float labels would get a NaN column per rank."""
+    if process_group is None:
+        return _one_hot_codes(adata_map.obs[key])
+    values = pd.Series(adata_map.obs[key]).reset_index(drop=True)
+    _, _, firsts = _agree_on_shards(adata_map, process_group, labels=list(pd.unique(values)))
+    columns = list(pd.unique(pd.Series([v for f in firsts for v in f], dtype=values.dtype)))
+    return _one_hot_codes(values, columns)
 
 
 def _mapping_of(adata_map):
@@ -235,30 +322,41 @@ def _mapping_of(adata_map):
     return X.toarray() if hasattr(X, "toarray") else X
 
 
-def project_cell_annotations(adata_map, adata_sp, annotation="cell_type", threshold=0.5):
+def project_cell_annotations(adata_map, adata_sp, annotation="cell_type", threshold=0.5, *, process_group=None):
     """:126-153 -- transfer `annotation` from the cells onto space: adata_sp.obsm["tangram_ct_pred"] becomes a float64
     (spots x annotations) DataFrame indexed by adata_map.var.index, its columns the annotations in order of first
     appearance, entry [j, t] the mapping probability of spot j summed over the cells annotated t.
 
     `threshold` has no effect, as in the reference: it filters the cells by adata_map.obs["F_out"] > threshold into a
-    variable that is overwritten before use (:144-147), so every cell counts.  The sums are taken on the device in fp64."""
-    columns, codes = _one_hot_codes(adata_map.obs[annotation])
+    variable that is overwritten before use (:144-147), so every cell counts.  The sums are taken on the device in fp64.
+
+    process_group: `adata_map` is this rank's block of a cell-sharded mapping (map_cells_to_space(process_group=)) and
+    `adata_sp` the same AnnData on every rank.  A collective: the columns are the labels of every rank's cells in global
+    order of first appearance, each rank sums its own rows on the device and the sums are added over the group, so every
+    rank writes the frame the unsharded call writes for the whole mapping (to rounding).  Refused with ValueError on every
+    rank when a rank has no uns["shard_rows"] or the blocks do not tile the cells in rank order."""
+    columns, codes = _annotation_codes(adata_map, annotation, process_group)
     sums, _ = annotate(_mapping_of(adata_map), codes, len(columns))
+    sums = mu._sum_over_group(sums, None, process_group)
     adata_sp.obsm["tangram_ct_pred"] = pd.DataFrame(sums.T, index=adata_map.var.index, columns=pd.Index(list(columns)))
 
 
-def cell_type_mapping(adata_map, cell_types_key="cell_types"):
+def cell_type_mapping(adata_map, cell_types_key="cell_types", *, process_group=None):
     """:820-842 -- adata_map.varm["ct_map"]: the (spots x cell types) sums of project_cell_annotations, min-max
     normalised per cell type (a constant column gives NaN, as in the reference).
 
     Where adata_map.obs has "F_out" (constrained mode), only the cells with F_out >= 0.5 count, each with its own label.
     The reference raises a shape error there whenever a cell is filtered out (:835 multiplies the filtered mapping by the
     unfiltered one-hot frame); where no cell is filtered out the result is the reference's.  The columns are the labels of
-    all cells, so a type whose cells are all filtered out has a zero, and so NaN, column."""
-    columns, codes = _one_hot_codes(adata_map.obs[cell_types_key])
+    all cells, so a type whose cells are all filtered out has a zero, and so NaN, column.
+
+    process_group: as in project_cell_annotations; the sums are added over the group before the normalisation, so every
+    rank's adata_map.varm["ct_map"] is that of the whole mapping."""
+    columns, codes = _annotation_codes(adata_map, cell_types_key, process_group)
     if "F_out" in adata_map.obs.keys():
         codes = np.where(np.asarray(adata_map.obs["F_out"]) >= 0.5, codes, -1)
     sums, _ = annotate(_mapping_of(adata_map), codes, len(columns))
+    sums = mu._sum_over_group(sums, None, process_group)
     df = pd.DataFrame(sums.T, index=adata_map.var.index, columns=pd.Index(list(columns)))
     vmin, vmax = df.min(), df.max()
     adata_map.varm["ct_map"] = (df - vmin) / (vmax - vmin)
@@ -284,14 +382,23 @@ def create_segment_cell_df(adata_sp):
     adata_sp.obsm["tangram_spot_centroids"] = per_spot["centroids_idx"]
 
 
-def count_cell_annotations(adata_map, adata_sc, adata_sp, annotation="cell_type", threshold=0.5):
+def count_cell_annotations(adata_map, adata_sc, adata_sp, annotation="cell_type", threshold=0.5, *,
+                           process_group=None):
     """:205-285 -- adata_sp.obsm["tangram_ct_count"]: per spot its coordinates 'x', 'y', its segmented cell count
     'cell_n', its cell ids 'centroids', and per annotation (adata_sc.obs[annotation], in order of first appearance) the
     number of cells whose most probable spot it is.  Where adata_map.obs has "F_out", only the cells with
     F_out > threshold are counted.
 
     The most probable spot of each counted cell is the device row argmax of the mapping (first spot on ties, as
-    np.argmax); the counts are one np.bincount.  Annotations are read by position in adata_sc.obs."""
+    np.argmax); the counts are one np.bincount.  Annotations are read by position in adata_sc.obs.
+
+    process_group: `adata_map` is this rank's block of a cell-sharded mapping (map_cells_to_space(process_group=)),
+    `adata_sc` and `adata_sp` the same AnnDatas on every rank.  A collective: the columns come from the whole
+    adata_sc.obs[annotation], the cell in row i of rows [r0, r1) takes the label at position r0 + i (positions past
+    adata_sc's cells are not counted, as without a group), each rank counts its own cells and the int64 counts are added
+    over the group, so every rank writes the frame the unsharded call writes for the whole mapping, exactly.  Refused
+    with ValueError on every rank when a rank has no uns["shard_rows"] or the blocks do not tile the cells in rank
+    order."""
     if "spatial" not in adata_sp.obsm.keys():
         raise ValueError(
             "Missing spatial information in AnnDatas. Please make sure coordinates are saved with AnnData.obsm['spatial']")
@@ -304,17 +411,22 @@ def count_cell_annotations(adata_map, adata_sc, adata_sp, annotation="cell_type"
                             "cell_n": adata_sp.obsm["image_features"]["segmentation_label"],
                             "centroids": adata_sp.obsm["tangram_spot_centroids"]},
                       index=list(adata_sp.obs.index))
+    r0 = 0                                              # the global position of this mapping's first cell
+    if process_group is not None:
+        r0, _, _ = _agree_on_shards(adata_map, process_group)
     columns, _, codes = _label_columns(adata_sc.obs[annotation])
     X = _mapping_of(adata_map)
-    N, n = X.shape[0], min(X.shape[0], len(codes))     # cells beyond adata_sc's are not counted (the reference zips)
+    N = X.shape[0]
+    n = min(N, max(len(codes) - r0, 0))                # cells beyond adata_sc's are not counted (the reference zips)
     labels = np.full(N, -1, dtype=np.int64)
-    labels[:n] = codes[:n]
+    labels[:n] = codes[r0:r0 + n]
     if "F_out" in adata_map.obs.keys():
         labels[~(np.asarray(adata_map.obs["F_out"]) > threshold)] = -1
     keep = labels >= 0
     _, spot = annotate(X, np.minimum(labels, 0), 1, sums=False, argmax=True)
     counts = np.bincount(spot[keep].astype(np.int64) * len(columns) + labels[keep],
                          minlength=len(df) * len(columns)).reshape(len(df), len(columns))
+    counts = mu._sum_over_group(counts, None, process_group)
     for t, c in enumerate(columns):
         df[c] = counts[:, t].astype(np.int64)
     adata_sp.obsm["tangram_ct_count"] = df
@@ -485,7 +597,7 @@ def cross_val(adata_sc, adata_sp, cluster_label=None, mode="clusters", scale=Tru
             mapper._set_loss_genes(active)
             mapper._fit(num_epochs, float(learning_rate), None, False, fetch=False)
             train_score = float(mapper.history_matrix[-1, 1])                    # main_loss (:622)
-            pred = mu._sum_over_group(mapper.project(S[r0:r1, [column[g] for g in test_genes]]), mapper,
+            pred = mu._sum_over_group(mapper.project(S[r0:r1, [column[g] for g in test_genes]]), _device_index(device),
                                       process_group)                              # (spots, test genes)
             var = pd.DataFrame({"is_training": np.zeros(len(test_genes), dtype=bool)}, index=test_genes)
             adata_ge = make_adata(X=pred, obs=adata_sp.obs.copy(), var=var, uns=adata_ref.uns)
