@@ -89,7 +89,7 @@ enum {
 
 /* Replaces the keyword arguments of Mapper.__init__ (mapping_optimizer.py:19-45). */
 typedef struct tgb200_config {
-  int32_t struct_size;     /* = sizeof(tgb200_config); ABI guard                              */
+  int32_t struct_size;     /* = sizeof(tgb200_config); ABI guard (the size without state_memory is accepted too) */
   int32_t device;          /* CUDA device ordinal                                             */
   int32_t n_cells;         /* rows of M / S held by THIS handle (S.shape[0], :150)            */
   int32_t n_voxels;        /* G.shape[0]                                                      */
@@ -115,7 +115,23 @@ typedef struct tgb200_config {
   float lambda_count;      /* :426 */
   float lambda_f_reg;      /* :427 */
   float target_count;      /* :428, :480-483 */
+  int32_t state_memory;    /* tgb200_state_memory: where M and Adam's moments live (0: on the device) */
 } tgb200_config;
+
+/* Placement of the optimizer state M, m (bf16 mode: mb) and v.  TGB200_STATE_HOST keeps them in pinned host memory
+ * (cudaHostAlloc).  Every pass that reads or writes them -- the row pass (also that of get_mapping, the projection and the
+ * validation) and the streaming update in both modes -- walks them in row blocks through a ring of two device slots: the
+ * copy-in of block b+1 and the copy-out of block b-1 run on the copy engines while block b's kernel runs, and in bf16 mode
+ * the blocks nest inside the cell chunks of the pipeline.  The slots are sized from free device memory (at most 128 MiB in
+ * all; the environment variable TGB200_STATE_BLOCK_ROWS sets the rows per block).  The draws, the zeroing and the state
+ * get / set reach the host state directly.  The device then holds about 4 B per mapping element in bf16 mode and 10 B in
+ * bf16x3 mode (the contraction operands) instead of 14 B and 22 B; the host holds 10 B (bf16) or 12 B (bf16x3).  The
+ * kernels run their resident arithmetic on the staged rows, so results are bit-identical to TGB200_STATE_DEVICE.  fp32
+ * mode fuses Adam into its FFMA contraction's epilogue and is refused with TGB200_ERR_UNSUPPORTED. */
+typedef enum tgb200_state_memory {
+  TGB200_STATE_DEVICE = 0,
+  TGB200_STATE_HOST = 1
+} tgb200_state_memory;
 
 /* ---- lifetime -------------------------------------------------------------------- */
 

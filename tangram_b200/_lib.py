@@ -13,6 +13,8 @@ HIST_VAL_TOTAL, HIST_VAL_GENE_SIM, HIST_VAL_SPARSITY, HIST_VAL_ENTROPY = 12, 13,
 PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 DENSITY_NONE, DENSITY_CELLS, DENSITY_SOURCE = 0, 1, 2
 GRAPH_VOXEL_WEIGHTS, GRAPH_NEIGHBORHOOD_FILTER, GRAPH_SPATIAL_WEIGHTS = 0, 1, 2
+# where M and Adam's moments live (tgb200_state_memory)
+STATE_MEMORY = {"device": 0, "host": 1}
 
 
 class Config(ctypes.Structure):
@@ -28,7 +30,7 @@ class Config(ctypes.Structure):
         ("lambda_getis_ord", ctypes.c_float),
         ("adam_beta1", ctypes.c_float), ("adam_beta2", ctypes.c_float), ("adam_eps", ctypes.c_float),
         ("constrained", ctypes.c_int32), ("lambda_count", ctypes.c_float), ("lambda_f_reg", ctypes.c_float),
-        ("target_count", ctypes.c_float),
+        ("target_count", ctypes.c_float), ("state_memory", ctypes.c_int32),
     ]
 
 

@@ -724,6 +724,11 @@ __global__ void k_bf16_to_f32(const __nv_bfloat16* __restrict__ src, float* __re
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = __bfloat162float(src[i]);
 }
+// zero n 16-byte words, stream-ordered: the cudaMemsetAsync of optimizer state held in mapped host memory
+__global__ void k_zero16(uint4* __restrict__ p, long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) p[i] = make_uint4(0, 0, 0, 0);
+}
 // M0 ~ N(0,1) on device (Philox4x32-10), pad columns zero.  Throughput runs only; the
 // reference draw (:150) is a host MT19937 float64 draw and is uploaded via set_mapping.
 __global__ void k_init_normal(float* __restrict__ M, int rows, int V, int ld, unsigned long long seed, long long first_row) {

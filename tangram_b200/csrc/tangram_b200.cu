@@ -49,13 +49,21 @@ static int fail(int code, const char* fmt, ...) {
     if (s__ != TGB200_OK) return s__; \
   } while (0)
 
+// `host`: mapped pinned host memory (TGB200_STATE_HOST) that kernels address directly; otherwise device memory
 template <typename T>
 struct DevBuf {
   T* p = nullptr;
   size_t n = 0;
+  bool host = false;
   int alloc(size_t count, bool zero = true) {
     release();
     if (count == 0) return TGB200_OK;
+    if (host) {
+      cudaError_t e = cudaHostAlloc(&p, count * sizeof(T), cudaHostAllocMapped);
+      if (e != cudaSuccess) { p = nullptr; return fail(TGB200_ERR_CUDA, "cudaHostAlloc(%zu B): %s", count * sizeof(T), cudaGetErrorString(e)); }
+      n = count;                    // zeroed by the handle on the device side (zero_state), not here
+      return TGB200_OK;
+    }
     cudaError_t e = cudaMalloc(&p, count * sizeof(T));
     if (e != cudaSuccess) { p = nullptr; return fail(TGB200_ERR_CUDA, "cudaMalloc(%zu B): %s", count * sizeof(T), cudaGetErrorString(e)); }
     n = count;
@@ -65,7 +73,7 @@ struct DevBuf {
     }
     return TGB200_OK;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
+  void release() { if (p) { if (host) cudaFreeHost(p); else cudaFree(p); } p = nullptr; n = 0; }
   ~DevBuf() { release(); }
 };
 
@@ -178,6 +186,16 @@ struct tgb200_mapper {
   // chunks; forward(c) of the next iteration waits only for Adam(c).  Which stream a launch goes to is the Lanes of its
   // API call (below).
   bool pipelined = false;       // several chunks: the handle has the streams hi, lo and sf
+  // host state (TGB200_STATE_HOST): M, m / mb and v in pinned host memory, and a ring of two device slots of `ring_rows`
+  // rows each through which every per-iteration pass streams them (staged_rows): copy-in of block b+1 on `cin` and
+  // copy-out of block b-1 on `cout` run on the copy engines under block b's kernel
+  bool host_state = false;
+  int ring_rows = 0;
+  DevBuf<float> rM[2], rm[2], rv[2];
+  DevBuf<__nv_bfloat16> rmb[2];
+  cudaStream_t cin = nullptr, cout = nullptr;
+  cudaEvent_t ev_in[2] = {}, ev_comp[2] = {}, ev_free[2] = {}, ev_start = nullptr, ev_last = nullptr;
+  bool ring_used = false;       // ev_last was recorded by an earlier staged pass
   int nchunks = 1, chunk_row[9] = {0};
   cudaStream_t hi = nullptr, lo = nullptr, sf = nullptr;     // sf: the NEXT iteration's forward chunks (see backward_bf16)
   cudaEvent_t ev_fork = nullptr, ev_join_hi = nullptr, ev_join_lo = nullptr, ev_join_sf = nullptr, ev_loss = nullptr;
@@ -212,6 +230,10 @@ struct tgb200_mapper {
     if (hi) cudaStreamDestroy(hi);
     if (lo) cudaStreamDestroy(lo);
     if (sf) cudaStreamDestroy(sf);
+    if (cin) cudaStreamDestroy(cin);
+    if (cout) cudaStreamDestroy(cout);
+    for (cudaEvent_t e : {ev_in[0], ev_in[1], ev_comp[0], ev_comp[1], ev_free[0], ev_free[1], ev_start, ev_last})
+      if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : {ev_fork, ev_join_hi, ev_join_lo, ev_join_sf, ev_loss}) if (e) cudaEventDestroy(e);
     for (int i = 0; i < 8; ++i)
       for (cudaEvent_t e : {ev_g[i], ev_a[i], ev_f[i]}) if (e) cudaEventDestroy(e);
@@ -272,11 +294,19 @@ extern "C" int tgb200_host_unpin(void* buf) {
 extern "C" const char* tgb200_last_error(void) { return g_err; }
 extern "C" const char* tgb200_version(void) { return "tangram_b200 0.3.0 (sm_90a)"; }
 
+static int setup_host_state(tgb200_mapper* h);
+
 extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (!cfg || !out) return fail(TGB200_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (cfg->struct_size != (int32_t)sizeof(tgb200_config))
+  // a caller written before `state_memory` existed passes the struct without it: its state stays on the device
+  const size_t size_v1 = offsetof(tgb200_config, state_memory);
+  if (cfg->struct_size != (int32_t)sizeof(tgb200_config) && cfg->struct_size != (int32_t)size_v1)
     return fail(TGB200_ERR_INVALID, "tgb200_config.struct_size=%d, expected %zu", cfg->struct_size, sizeof(tgb200_config));
+  tgb200_config full{};
+  memcpy(&full, cfg, (size_t)cfg->struct_size);
+  full.struct_size = (int32_t)sizeof(tgb200_config);
+  cfg = &full;
   if (cfg->n_cells <= 0 || cfg->n_voxels <= 0 || cfg->n_genes <= 0 || cfg->n_types < 0)
     return fail(TGB200_ERR_INVALID, "bad shape cells=%d voxels=%d genes=%d types=%d", cfg->n_cells, cfg->n_voxels, cfg->n_genes, cfg->n_types);
   if (cfg->lambda_g1 == 0.f) return fail(TGB200_ERR_INVALID, "lambda_g1 cannot be 0.");  // mapping_utils.py:206-207
@@ -293,6 +323,10 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
       return fail(TGB200_ERR_INVALID, "constrained mode has no spatial / L1 / L2 terms (mapping_optimizer.py:417-432)");
     if (cfg->n_cells_global > 0 && cfg->n_cells_global != cfg->n_cells && cfg->target_count <= 0.f) return fail(TGB200_ERR_INVALID, "target_count must be given");
   }
+  if (cfg->state_memory != TGB200_STATE_DEVICE && cfg->state_memory != TGB200_STATE_HOST)
+    return fail(TGB200_ERR_INVALID, "unknown state_memory %d", cfg->state_memory);
+  if (cfg->state_memory == TGB200_STATE_HOST && cfg->precision == TGB200_PREC_FP32)
+    return fail(TGB200_ERR_UNSUPPORTED, "state_memory = host needs precision bf16 or bf16x3: fp32 fuses Adam into its FFMA contraction");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
@@ -323,6 +357,8 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   const size_t nv = (size_t)h->N * h->ld, vk = (size_t)h->V * h->Ke;
   int st = TGB200_OK;
   auto A = [&](int s) { if (st == TGB200_OK) st = s; };
+  h->host_state = cfg->state_memory == TGB200_STATE_HOST;
+  h->M.host = h->m.host = h->mb.host = h->v.host = h->host_state;
   if (h->x3) A(h->dpf.alloc(nv, false));
   A(h->M.alloc(nv)); A(h->v.alloc(nv));
   if (h->bf16) A(h->mb.alloc(nv)); else A(h->m.alloc(nv));
@@ -421,6 +457,7 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
     A(h->H.alloc((size_t)h->V * h->T)); A(h->ctpart.alloc(h->n_ct_blocks));
   }
   if (st == TGB200_OK && h->tcm) st = tc_init(h->tc, g_err, sizeof(g_err));
+  if (st == TGB200_OK && h->host_state) st = setup_host_state(h);
   if (st != TGB200_OK) { delete h; return st; }
   CK(cudaDeviceSynchronize());
   *out = h;
@@ -590,10 +627,108 @@ extern "C" int tgb200_set_graph(tgb200_mapper* h, int which, const int32_t* indp
   return TGB200_OK;
 }
 
+// cudaMemsetAsync(0) of M, m / mb or v; in host memory a kernel writes the zeros (rows of ld elements: 16-byte multiples)
+template <typename T>
+static int zero_state(tgb200_mapper* h, DevBuf<T>& b, cudaStream_t s) {
+  const size_t bytes = b.n * sizeof(T);
+  if (!b.host) {
+    CK(cudaMemsetAsync(b.p, 0, bytes, s));
+    return TGB200_OK;
+  }
+  const long long n16 = (long long)(bytes / 16);
+  k_zero16<<<(unsigned)std::min<long long>(ceil_div(n16, 256), 2048), 256, 0, s>>>(reinterpret_cast<uint4*>(b.p), n16);
+  LAUNCH_CHECK("zero16");
+  return TGB200_OK;
+}
+
+// Host state: zero M, m / mb and v once (as the device path's cudaMalloc'd state is), then the ring.  Its two slots take at
+// most an eighth of the free device memory and 128 MiB in all -- a block of 64 MiB is copied at link speed, and the
+// device keeps room for the projection's and validation's scratch; TGB200_STATE_BLOCK_ROWS sets the rows per block.
+static int setup_host_state(tgb200_mapper* h) {
+  CKS(zero_state(h, h->M, nullptr));
+  if (h->bf16) CKS(zero_state(h, h->mb, nullptr)); else CKS(zero_state(h, h->m, nullptr));
+  CKS(zero_state(h, h->v, nullptr));
+  const size_t row_bytes = (size_t)h->ld * (h->bf16 ? 4 + 2 + 4 : 4 + 4 + 4);
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const size_t budget = std::min<size_t>(free_b / 8, (size_t)128 << 20);
+  int64_t rows = (int64_t)(budget / (2 * row_bytes));
+  if (const char* e = getenv("TGB200_STATE_BLOCK_ROWS")) rows = atoll(e);
+  h->ring_rows = (int)std::clamp<int64_t>(rows, 1, h->N);
+  const size_t n = (size_t)h->ring_rows * h->ld;
+  for (int k = 0; k < 2; ++k) {
+    CKS(h->rM[k].alloc(n, false)); CKS(h->rv[k].alloc(n, false));
+    if (h->bf16) CKS(h->rmb[k].alloc(n, false)); else CKS(h->rm[k].alloc(n, false));
+  }
+  CK(cudaStreamCreateWithFlags(&h->cin, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(&h->cout, cudaStreamNonBlocking));
+  for (cudaEvent_t* e : {&h->ev_in[0], &h->ev_in[1], &h->ev_comp[0], &h->ev_comp[1], &h->ev_free[0], &h->ev_free[1],
+                         &h->ev_start, &h->ev_last})
+    CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  return TGB200_OK;
+}
+
+// a row-shifted base: row i of the slot block that starts at row b0 is at base + i * ld for i in [b0, b0 + ring_rows), so
+// the kernels index the slot with the mapping's own row numbers and run exactly their resident arithmetic
+template <typename T>
+static T* shifted(T* slot, int b0, int ld) {
+  return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(slot) - (uintptr_t)b0 * ld * sizeof(T));
+}
+
+struct StagedPtrs { float* M; float* m; __nv_bfloat16* mb; float* v; };
+
+// Rows [r0, r1) of the host state through the ring, in blocks of ring_rows, each block's kernel on `s`:
+// `launch(b0, b1, ptrs)` with row-shifted slot bases.  The copy-in of block b+1 (stream cin) and the copy-out of block
+// b-1 (stream cout, `write` passes only: M, m / mb, v) overlap block b's kernel.  The pass starts after the work queued on
+// `s` and after the previous staged pass (whatever stream ran it) has finished with the slots and written the host copy
+// back; `s` continues after the last copy-out.  Without host state, one launch on the resident buffers.
+template <typename F>
+static int staged_rows(tgb200_mapper* h, cudaStream_t s, int r0, int r1, bool write, F launch) {
+  if (!h->host_state) return launch(r0, r1, StagedPtrs{h->M.p, h->m.p, h->mb.p, h->v.p});
+  if (r1 <= r0) return TGB200_OK;
+  const int ld = h->ld;
+  CK(cudaEventRecord(h->ev_start, s));
+  CK(cudaStreamWaitEvent(h->cin, h->ev_start, 0));
+  if (h->ring_used) CK(cudaStreamWaitEvent(h->cin, h->ev_last, 0));
+  int k = 0;
+  for (int b0 = r0; b0 < r1; b0 += h->ring_rows, ++k) {
+    const int b1 = std::min(r1, b0 + h->ring_rows), sl = k & 1;
+    const size_t off = (size_t)b0 * ld, n = (size_t)(b1 - b0) * ld;
+    if (k >= 2) CK(cudaStreamWaitEvent(h->cin, h->ev_free[sl], 0));       // block k - 2 is done with this slot
+    CK(cudaMemcpyAsync(h->rM[sl].p, h->M.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
+    if (write) {
+      if (h->bf16) CK(cudaMemcpyAsync(h->rmb[sl].p, h->mb.p + off, n * sizeof(__nv_bfloat16), cudaMemcpyHostToDevice, h->cin));
+      else CK(cudaMemcpyAsync(h->rm[sl].p, h->m.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
+      CK(cudaMemcpyAsync(h->rv[sl].p, h->v.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
+    }
+    CK(cudaEventRecord(h->ev_in[sl], h->cin));
+    CK(cudaStreamWaitEvent(s, h->ev_in[sl], 0));
+    CKS(launch(b0, b1, StagedPtrs{shifted(h->rM[sl].p, b0, ld), h->rm[sl].p ? shifted(h->rm[sl].p, b0, ld) : nullptr,
+                                  h->rmb[sl].p ? shifted(h->rmb[sl].p, b0, ld) : nullptr, shifted(h->rv[sl].p, b0, ld)}));
+    CK(cudaEventRecord(h->ev_comp[sl], s));
+    if (write) {
+      CK(cudaStreamWaitEvent(h->cout, h->ev_comp[sl], 0));
+      CK(cudaMemcpyAsync(h->M.p + off, h->rM[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
+      if (h->bf16) CK(cudaMemcpyAsync(h->mb.p + off, h->rmb[sl].p, n * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost, h->cout));
+      else CK(cudaMemcpyAsync(h->m.p + off, h->rm[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
+      CK(cudaMemcpyAsync(h->v.p + off, h->rv[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
+      CK(cudaEventRecord(h->ev_free[sl], h->cout));
+    } else {
+      CK(cudaEventRecord(h->ev_free[sl], s));
+    }
+  }
+  // everything of this pass: the last kernel on s and, for a write pass, the copy-outs (cout is in order)
+  if (write) CK(cudaEventRecord(h->ev_last, h->cout));
+  else CK(cudaEventRecord(h->ev_last, s));
+  CK(cudaStreamWaitEvent(s, h->ev_last, 0));
+  h->ring_used = true;
+  return TGB200_OK;
+}
+
 static int zero_moments(tgb200_mapper* h, cudaStream_t s) {
-  if (h->bf16) CK(cudaMemsetAsync(h->mb.p, 0, h->mb.n * sizeof(__nv_bfloat16), s));
-  else CK(cudaMemsetAsync(h->m.p, 0, h->m.n * sizeof(float), s));
-  CK(cudaMemsetAsync(h->v.p, 0, h->v.n * sizeof(float), s));
+  if (h->bf16) CKS(zero_state(h, h->mb, s));
+  else CKS(zero_state(h, h->m, s));
+  CKS(zero_state(h, h->v, s));
   return TGB200_OK;
 }
 
@@ -695,7 +830,7 @@ extern "C" int tgb200_set_mapping(tgb200_mapper* h, const float* M0, void* strea
   if (!h || !M0) return fail(TGB200_ERR_INVALID, "null argument");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemsetAsync(h->M.p, 0, h->M.n * sizeof(float), s));
+  CKS(zero_state(h, h->M, s));
   CK(cudaMemcpy2DAsync(h->M.p, (size_t)h->ld * sizeof(float), M0, (size_t)h->V * sizeof(float),
                        (size_t)h->V * sizeof(float), h->N, cudaMemcpyDefault, s));
   CKS(reset_optimizer(h, s));
@@ -843,7 +978,7 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
   std::fill(stats, stats + 8, 0.f);
   EventSet ev;
   for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
-  CK(cudaMemsetAsync(h->M.p, 0, h->M.n * sizeof(float), s));
+  CKS(zero_state(h, h->M, s));
   EndRecord end_h{-1, {0, 0, 0, 0}};
   int64_t n_fixed = 0, n_changed = 0;
   std::vector<float> patch_vals;
@@ -939,20 +1074,20 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
     std::vector<Flagged> fl(nf);
     std::vector<float> dev_vals(nf);
     if (nf) CK(cudaMemcpy(fl.data(), flags.p, nf * sizeof(Flagged), cudaMemcpyDeviceToHost));
-    for (int i = 0; i < nf; ++i) CK(cudaMemcpyAsync(&dev_vals[i], h->M.p + fl[i].idx, sizeof(float), cudaMemcpyDeviceToHost, s));
+    for (int i = 0; i < nf; ++i) CK(cudaMemcpyAsync(&dev_vals[i], h->M.p + fl[i].idx, sizeof(float), cudaMemcpyDefault, s));
     CK(cudaStreamSynchronize(s));
     patch_vals.resize(nf);
     for (int i = 0; i < nf; ++i) {
       patch_vals[i] = (float)polar_value_host(fl[i].w, fl[i].comp);
       if (std::memcmp(&patch_vals[i], &dev_vals[i], sizeof(float)) != 0) {
-        CK(cudaMemcpyAsync(h->M.p + fl[i].idx, &patch_vals[i], sizeof(float), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->M.p + fl[i].idx, &patch_vals[i], sizeof(float), cudaMemcpyDefault, s));
         ++n_changed;
       }
     }
     n_fixed = nf;
   }
   float cached = (float)start->gauss;
-  if (hg && t_lo == 0) CK(cudaMemcpyAsync(h->M.p, &cached, sizeof(float), cudaMemcpyHostToDevice, s));   // normal 0
+  if (hg && t_lo == 0) CK(cudaMemcpyAsync(h->M.p, &cached, sizeof(float), cudaMemcpyDefault, s));   // normal 0
   if (a_end >= 0) CK(cudaEventRecord(ev.e[4], s));
   CKS(reset_optimizer(h, s));
   h->have_mapping = true;
@@ -989,26 +1124,36 @@ static int launch_softmax_rows(tgb200_mapper* h, cudaStream_t s, PT* P, int want
                                Split3 split = Split3{nullptr, 0}, int row0 = 0, int nrows = -1) {
   const int nvec = h->ld / 4;
   if (nrows < 0) nrows = h->N - row0;
-  const float* Mp = h->M.p + (size_t)row0 * h->ld;
-  RowStat* st = h->stats.p + row0;
-  // One CTA per row, the row cached in registers between the max / exp-sum / emit passes.  Wide rows use more threads with
-  // fewer float4 slots each: registers/thread stay <= 40..64, so 48-64 warps stay resident per SM (256 x 12 slots held 24,
-  // and the row pass was latency-bound at 0.46 of the HBM peak).  Rows wider than 6144 float4 re-read M.
+  // rows [b0, b1): one launch over the resident M, or one per ring block of host state (`o` rows into P / rowaux / split)
+  auto rows = [&](int b0, int b1, const StagedPtrs& sp) -> int {
+    const int nr = b1 - b0;
+    const size_t o = (size_t)(b0 - row0);
+    const float* Mp = sp.M + (size_t)b0 * h->ld;
+    RowStat* st = h->stats.p + b0;
+    PT* Po = P ? P + o * h->ld : nullptr;
+    float* ra = rowaux ? rowaux + 2 * o : nullptr;
+    Split3 sp3 = split;
+    if (sp3.base) sp3.base += o * h->ld;
+    // One CTA per row, the row cached in registers between the max / exp-sum / emit passes.  Wide rows use more threads
+    // with fewer float4 slots each: registers/thread stay <= 40..64, so 48-64 warps stay resident per SM (256 x 12 slots
+    // held 24, and the row pass was latency-bound at 0.46 of the HBM peak).  Rows wider than 6144 float4 re-read M.
 #define SMX(T, ITEMS, MINB)                                                                         \
-  k_softmax_rows<PT, T, ITEMS, MINB><<<nrows, T, 0, s>>>(Mp, h->ld, h->V, P, h->ld, st, rowaux, want_entropy, split)
-  if (nvec <= 256 * 1) SMX(256, 1, 1);
-  else if (nvec <= 256 * 2) SMX(256, 2, 1);
-  else if (nvec <= 256 * 4) SMX(256, 4, 1);
-  else if (nvec <= 512 * 3) SMX(512, 3, 3);
-  else if (nvec <= 512 * 4) SMX(512, 4, 3);
-  else if (nvec <= 512 * 5) SMX(512, 5, 3);
-  else if (nvec <= 1024 * 3) SMX(1024, 3, 2);
-  else if (nvec <= 1024 * 4) SMX(1024, 4, 1);
-  else if (nvec <= 1024 * 6) SMX(1024, 6, 1);
-  else SMX(1024, 0, 1);
+  k_softmax_rows<PT, T, ITEMS, MINB><<<nr, T, 0, s>>>(Mp, h->ld, h->V, Po, h->ld, st, ra, want_entropy, sp3)
+    if (nvec <= 256 * 1) SMX(256, 1, 1);
+    else if (nvec <= 256 * 2) SMX(256, 2, 1);
+    else if (nvec <= 256 * 4) SMX(256, 4, 1);
+    else if (nvec <= 512 * 3) SMX(512, 3, 3);
+    else if (nvec <= 512 * 4) SMX(512, 4, 3);
+    else if (nvec <= 512 * 5) SMX(512, 5, 3);
+    else if (nvec <= 1024 * 3) SMX(1024, 3, 2);
+    else if (nvec <= 1024 * 4) SMX(1024, 4, 1);
+    else if (nvec <= 1024 * 6) SMX(1024, 6, 1);
+    else SMX(1024, 0, 1);
 #undef SMX
-  LAUNCH_CHECK("softmax_rows");
-  return TGB200_OK;
+    LAUNCH_CHECK("softmax_rows");
+    return TGB200_OK;
+  };
+  return staged_rows(h, s, row0, row0 + nrows, false, rows);
 }
 
 static LossParams make_loss_params(tgb200_mapper* h) {
@@ -1347,11 +1492,15 @@ static int backward_bf16(tgb200_mapper* h, const Lanes& L, const AdamScalars& a,
                                                                                h->stats.p, h->rcenter.p, h->rdot.p, h->rowc.p);
     { cudaStream_t s = su; LAUNCH_CHECK("rowdot_finalize"); }
     if (h->constrained) CKS(filter_update(h, su, a));
-    AdamRowsArgs ar{h->M.p, h->mb.p, h->v.p, h->dq.p, h->Pb.p, reinterpret_cast<const RowConst*>(h->rowc.p),
-                    h->zsum.p, h->pxsum.p, h->l1sum.p, h->l2sum.p, h->ld, h->V, r0, r1,
-                    h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
-    if (adam_rows_launch(ar, su)) return fail(TGB200_ERR_CUDA, "launch adam_rows: %s", cudaGetErrorString(cudaGetLastError()));
-    mark(h, su, "adam_rows");
+    // host state: the ring blocks nest inside the chunk, so chunk c's update still runs under chunk c+1's contraction
+    CKS(staged_rows(h, su, r0, r1, true, [&](int b0, int b1, const StagedPtrs& sp) -> int {
+      AdamRowsArgs ar{sp.M, sp.mb, sp.v, h->dq.p, h->Pb.p, reinterpret_cast<const RowConst*>(h->rowc.p),
+                      h->zsum.p, h->pxsum.p, h->l1sum.p, h->l2sum.p, h->ld, h->V, b0, b1,
+                      h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
+      if (adam_rows_launch(ar, su)) return fail(TGB200_ERR_CUDA, "launch adam_rows: %s", cudaGetErrorString(cudaGetLastError()));
+      mark(h, su, "adam_rows");
+      return TGB200_OK;
+    }));
     if (two_streams) CK(cudaEventRecord(h->ev_a[c], su));
     h->a_valid = two_streams;
     // The next iteration's forward for this chunk goes to a third stream as soon as its rows are updated: the backward
@@ -1385,11 +1534,13 @@ static int backward_bf16x3(tgb200_mapper* h, cudaStream_t s, const AdamScalars& 
   k_rowdot_finalize<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->rpart.p, h->r_parts, h->N, h->rdot.p);
   LAUNCH_CHECK("rowdot_finalize");
   if (h->constrained) CKS(filter_update(h, s, a));
-  AdamRowsExactArgs ar{h->M.p, h->m.p, h->v.p, h->dpf.p, h->stats.p, h->rdot.p, h->ld, h->V, 0, h->N,
-                       h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
-  if (adam_rows_exact_launch(ar, s)) return fail(TGB200_ERR_CUDA, "launch adam_rows_exact: %s", cudaGetErrorString(cudaGetLastError()));
-  mark(h, s, "adam_rows");
-  return TGB200_OK;
+  return staged_rows(h, s, 0, h->N, true, [&](int b0, int b1, const StagedPtrs& sp) -> int {
+    AdamRowsExactArgs ar{sp.M, sp.m, sp.v, h->dpf.p, h->stats.p, h->rdot.p, h->ld, h->V, b0, b1,
+                         h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
+    if (adam_rows_exact_launch(ar, s)) return fail(TGB200_ERR_CUDA, "launch adam_rows_exact: %s", cudaGetErrorString(cudaGetLastError()));
+    mark(h, s, "adam_rows");
+    return TGB200_OK;
+  });
 }
 
 // Backward of the fp32 cross-check mode: FFMA contractions (row-dot GEMM, then the backward GEMM with the fused exact
@@ -1813,7 +1964,7 @@ extern "C" int tgb200_debug_timeline(tgb200_mapper* h, int32_t enable, const cha
 // n elements of `planes` bf16 planes, summed from the last plane to the first in fp32 on the host
 static int widen_bf16(const __nv_bfloat16* src, int64_t n, int planes, float* out) {
   std::vector<__nv_bfloat16> tmp((size_t)n * planes);
-  CK(cudaMemcpy(tmp.data(), src, tmp.size() * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(tmp.data(), src, tmp.size() * sizeof(__nv_bfloat16), cudaMemcpyDefault));
   for (int64_t i = 0; i < n; ++i) {
     float acc = __bfloat162float(tmp[(size_t)(planes - 1) * n + i]);
     for (int pl = planes - 2; pl >= 0; --pl) acc += __bfloat162float(tmp[(size_t)pl * n + i]);
@@ -1888,6 +2039,12 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
     out_host[0] = (float)h->Ke; out_host[1] = (float)h->ld; out_host[2] = (float)h->fwd_splits; out_host[3] = (float)h->r_parts;
     out_host[4] = (float)h->nchunks;
     return TGB200_OK;
+  } else if (nm == "ring") {    // rows per staging block of host state (0: resident state)
+    *n = 1;
+    if (!out_host) return TGB200_OK;
+    if (cap < 1) return fail(TGB200_ERR_INVALID, "cap < 1");
+    out_host[0] = (float)h->ring_rows;
+    return TGB200_OK;
   } else if (nm == "legacy_init") {
     *n = 8;
     if (!out_host) return TGB200_OK;
@@ -1898,7 +2055,7 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
   *n = cnt;
   if (out_host) {
     if (cap < cnt) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)cnt);
-    CK(cudaMemcpy(out_host, src, cnt * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(out_host, src, cnt * sizeof(float), cudaMemcpyDefault));
   }
   return TGB200_OK;
 }

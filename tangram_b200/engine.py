@@ -45,12 +45,71 @@ def _csr(mat, n):
             np.ascontiguousarray(csr.data, dtype=np.float32))
 
 
+# state_memory="host": bytes per mapping element (on the device, in pinned host memory).  The device keeps the contraction
+# operands: bf16 P and dq in bf16 mode; three P planes and the fp32 dP in bf16x3 mode.  The host keeps M, m (bf16 in bf16
+# mode) and v.
+HOST_STATE_BYTES_PER_ELEMENT = {"bf16": (4, 10), "bf16x3": (10, 12)}
+
+
+def host_memory_available():
+    """MemAvailable of /proc/meminfo in bytes (None where the file or the field is missing)."""
+    try:
+        with open("/proc/meminfo") as f:
+            for line in f:
+                if line.startswith("MemAvailable:"):
+                    return int(line.split()[1]) * 1024
+    except OSError:
+        return None
+    return None
+
+
+def check_state_memory(state_memory, precision):
+    """Validate Engine's `state_memory` argument for `precision`."""
+    if state_memory not in _lib.STATE_MEMORY:
+        raise ValueError(f"state_memory must be one of {list(_lib.STATE_MEMORY)}, got {state_memory!r}")
+    if state_memory == "host" and precision not in HOST_STATE_BYTES_PER_ELEMENT:
+        raise ValueError(f"state_memory='host' needs precision 'bf16' or 'bf16x3', not {precision!r}: fp32 fuses Adam "
+                         "into its FFMA contraction's epilogue, which reads the optimizer state of every row on the device")
+
+
+def check_host_state_fits(n_cells, n_voxels, n_genes, precision, device, host_available=None, device_free=None):
+    """Before a state_memory="host" handle is allocated: raise TangramB200Error when the pinned host state would not fit in
+    MemAvailable, or the device part (the contraction operands, estimated as the tuner estimates a handle) would not fit
+    in the device's free memory.  `host_available` / `device_free` (bytes) default to /proc/meminfo and
+    torch.cuda.mem_get_info."""
+    dev_b, host_b = HOST_STATE_BYTES_PER_ELEMENT[precision]
+    elems = n_cells * (-(-n_voxels // 64) * 64)
+    need_host = host_b * elems
+    if host_available is None:
+        host_available = host_memory_available()
+    if host_available is not None and need_host > host_available:
+        raise _lib.TangramB200Error(
+            f"state_memory='host' needs about {need_host / 2**30:.1f} GiB of pinned host memory for M, m and v of "
+            f"{n_cells} x {n_voxels} ({host_b} B per element in {precision} mode); MemAvailable is "
+            f"{host_available / 2**30:.1f} GiB")
+    need_dev = dev_b * elems + 16 * (n_cells + n_voxels) * n_genes
+    if device_free is None:
+        import torch
+        device_free, _ = torch.cuda.mem_get_info(device)
+    if need_dev > device_free:
+        raise _lib.TangramB200Error(
+            f"state_memory='host' still needs about {need_dev / 2**30:.1f} GiB on cuda:{device} for the contraction "
+            f"operands of {n_cells} x {n_voxels} ({dev_b} B per element in {precision} mode, plus the expression "
+            f"operands); {device_free / 2**30:.1f} GiB are free")
+
+
 class Engine:
-    """Config fields not given default to 0, except lambda_g1 (1) and lambda_d (1 when there is a density)."""
+    """Config fields not given default to 0, except lambda_g1 (1) and lambda_d (1 when there is a density).
+    state_memory="host" keeps M and Adam's moments in pinned host memory (TGB200_STATE_HOST), after checking that both
+    the host and the device side fit."""
 
     def __init__(self, n_cells, n_voxels, n_genes, *, n_types=0, n_cells_global=None, device=0,
-                 precision="fp32", density_mode=_lib.DENSITY_CELLS, constrained=False, **lambdas):
+                 precision="fp32", density_mode=_lib.DENSITY_CELLS, constrained=False, state_memory="device",
+                 **lambdas):
+        check_state_memory(state_memory, precision)
         self._lib = _lib.load()
+        if state_memory == "host":
+            check_host_state_fits(n_cells, n_voxels, n_genes, precision, device)
         cfg = _lib.Config()
         cfg.struct_size = ctypes.sizeof(_lib.Config)
         cfg.device = device
@@ -67,12 +126,13 @@ class Engine:
             raise TypeError(f"unknown arguments {sorted(lambdas)}")
         cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps = 0.9, 0.999, 1e-8      # torch.optim.Adam defaults
         cfg.constrained = int(constrained)
+        cfg.state_memory = _lib.STATE_MEMORY[state_memory]
         self.cfg = cfg
         self._h = ctypes.c_void_p()
         _lib.check(self._lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(self._h)))
 
     def close(self):
-        """Free the device state now (M, m, v, operands: ~20 bytes per mapping element) instead of at garbage collection."""
+        """Free the handle's state now (M, m, v, operands: ~20 bytes per mapping element) instead of at garbage collection."""
         if self._h:
             self._lib.tgb200_destroy(self._h)
             self._h = None

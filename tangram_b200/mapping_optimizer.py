@@ -20,6 +20,8 @@ Additions (keyword-only, all optional):
   draw_whole_stream      (Mapper only) a sharded rank's seeded draw leaves numpy's generator where the unsharded draw
               leaves it instead of after the rank's last row, so that draws made one after another from it (cross_val's
               folds) are the same on every rank
+  state_memory "device" (default) | "host": keep M and Adam's moments in pinned host memory, so that a mapping about
+              3.5x (bf16) or 2.2x (bf16x3) larger fits one GPU, with bit-identical results; fp32 is refused
   train(..., resume=True)  continue with the Adam state of the previous train() call (the reference -- and the default
               here -- builds a fresh optimizer in every train() call, mapping_optimizer.py:373)
   train(..., out=tensor)   write softmax(M) into a CUDA tensor instead of returning a host array
@@ -291,6 +293,7 @@ class Mapper(_EngineMapper):
         shard=None,
         n_cells_global=None,
         draw_whole_stream=False,
+        state_memory="device",
     ):
         if lambda_geary > 0 or lambda_moran > 0:
             # mapping_optimizer.py:173-185: not on the accelerated path (Geary builds V x V x K)
@@ -344,7 +347,7 @@ class Mapper(_EngineMapper):
             precision=precision, density_mode=density_mode, lambda_g1=lambda_g1, lambda_d=lambda_d,
             lambda_g2=lambda_g2, lambda_r=lambda_r, lambda_l1=lambda_l1, lambda_l2=lambda_l2,
             lambda_neighborhood_g1=lambda_neighborhood_g1, lambda_ct_islands=lambda_ct_islands,
-            lambda_getis_ord=lambda_getis_ord)
+            lambda_getis_ord=lambda_getis_ord, state_memory=state_memory)
         self._cfg = e.cfg
         self.n_cells, self.n_voxels, self.n_genes = r1 - r0, n_voxels, n_genes
 
@@ -458,7 +461,7 @@ class MapperConstrained(_EngineMapper):
 
     def __init__(self, S, G, d, lambda_d=1, lambda_g1=1, lambda_g2=1, lambda_r=0, lambda_count=1, lambda_f_reg=1,
                  target_count=None, device="cuda:0", adata_map=None, random_state=None, *, precision="bf16x3",
-                 M0=None, F0=None, process_group=None, shard=None):
+                 M0=None, F0=None, process_group=None, shard=None, state_memory="device"):
         if adata_map is not None:
             raise NotImplementedError      # the reference raises here too (:476-477)
         if precision not in _lib.PREC:
@@ -479,7 +482,8 @@ class MapperConstrained(_EngineMapper):
             density_mode=_lib.DENSITY_CELLS if self.target_density_enabled else _lib.DENSITY_NONE,
             lambda_g1=lambda_g1, lambda_d=lambda_d, lambda_g2=lambda_g2, lambda_r=lambda_r, constrained=True,
             lambda_count=lambda_count, lambda_f_reg=lambda_f_reg,
-            target_count=float(n_voxels if target_count is None else target_count))      # :480-483
+            target_count=float(n_voxels if target_count is None else target_count),      # :480-483
+            state_memory=state_memory)
         self._cfg = e.cfg
         self.n_cells, self.n_voxels, self.n_genes = r1 - r0, n_voxels, n_genes
         self._n_cells_global = n_cells

@@ -240,7 +240,7 @@ def map_cells_to_space(
     lambda_count=1, lambda_f_reg=1, target_count=None,
     lambda_neighborhood_g1=0, lambda_ct_islands=0, lambda_getis_ord=0, lambda_moran=0, lambda_geary=0,
     random_state=None, verbose=True, density_prior="rna_count_based", precision="bf16x3",
-    process_group=None, gather=False, keep_on_device=False,
+    process_group=None, gather=False, keep_on_device=False, state_memory="device",
 ):
     """Same contract as the reference (mapping_utils.py:141-428); `device` must be CUDA.  Added keywords:
     precision       "bf16x3" parity-grade on tensor cores (default) | "fp32" FFMA | "bf16" throughput
@@ -252,6 +252,9 @@ def map_cells_to_space(
                     (first, last)); the per-gene scores, the history and `uns` are global and identical on every rank.
                     gather=True: rank 0 additionally receives the full mapping (all cells, and the full F_out) and the
                     other ranks return None.
+    state_memory    "device" (default) | "host": keep the mapping and Adam's moments in pinned host memory (each rank its
+                    own shard), so that a mapping too large for the GPU trains there with bit-identical results; bf16 and
+                    bf16x3 only
     keep_on_device  keep the trained mapper (device state ~20 B per mapping element) attached to the result so that
                     project_genes contracts on the GPU; default: release it (`adata_map.X` is all project_genes needs)."""
     _check_shardable(mode, process_group)
@@ -262,6 +265,8 @@ def map_cells_to_space(
     print_each = 100 if verbose else None
 
     F_out = None
+    if state_memory != "device":       # the mapper classes' default; a stand-in class need not know the keyword
+        mapper_kw = dict(mapper_kw, state_memory=state_memory)
     mapper = _make_mapper(mode, mapper_kw, device=device, random_state=random_state, precision=precision,
                           process_group=process_group)
     if mode == "constrained":                                                     # :366-389
