@@ -127,11 +127,36 @@ typedef struct tgb200_config {
  * get / set reach the host state directly.  The device then holds about 4 B per mapping element in bf16 mode and 10 B in
  * bf16x3 mode (the contraction operands) instead of 14 B and 22 B; the host holds 10 B (bf16) or 12 B (bf16x3).  The
  * kernels run their resident arithmetic on the staged rows, so results are bit-identical to TGB200_STATE_DEVICE.  fp32
- * mode fuses Adam into its FFMA contraction's epilogue and is refused with TGB200_ERR_UNSUPPORTED. */
+ * mode fuses Adam into its FFMA contraction's epilogue and is refused with TGB200_ERR_UNSUPPORTED.
+ * TGB200_STATE_AUTO keeps as many rows on the device as fit and only the rest in host memory: tgb200_create plans the
+ * split with tgb200_plan_state on the device's free memory.  When every row fits, the handle is a TGB200_STATE_DEVICE
+ * handle (same allocations, kernels and launches; no pinned memory, ring or copy streams).  Otherwise rows [0, R) of M,
+ * m / mb and v live in device memory and rows [R, N) in pinned host memory; every pass over a row range launches its
+ * resident rows directly, in pieces between the staged blocks, so the ring's copies run under the resident rows' kernels.
+ * The environment variable TGB200_STATE_RESIDENT_ROWS forces R.  Results are bit-identical to the other placements;
+ * fp32 is refused as for TGB200_STATE_HOST. */
 typedef enum tgb200_state_memory {
   TGB200_STATE_DEVICE = 0,
-  TGB200_STATE_HOST = 1
+  TGB200_STATE_HOST = 1,
+  TGB200_STATE_AUTO = 2
 } tgb200_state_memory;
+
+/* Where a handle of `cfg` would keep its state given `device_free` bytes of free device memory: pure arithmetic, no
+ * allocation and no device needed (tgb200_create uses it with cudaMemGetInfo).  device_bytes bounds what tgb200_create
+ * allocates on the device (the operands, rows [0, R) of the state and the ring, each allocation rounded up to 2 MiB);
+ * reserve_bytes is what the handle keeps free for what it allocates later (validation scratch, the CSR graphs, the
+ * history, get_mapping's and the projection's blocks, the legacy draw's scratch, CUDA's loading of the kernels).
+ * TGB200_STATE_AUTO picks the largest R with device_bytes + reserve_bytes <= device_free, R = N when every row fits;
+ * TGB200_STATE_BLOCK_ROWS and TGB200_STATE_RESIDENT_ROWS override the block rows and R as they do in tgb200_create.
+ * TGB200_STATE_DEVICE plans R = N, TGB200_STATE_HOST R = 0.  fp32 with host or auto state: TGB200_ERR_UNSUPPORTED. */
+typedef struct tgb200_state_plan {
+  int32_t resident_rows;   /* R: rows [0, R) of M, m / mb and v on the device */
+  int32_t block_rows;      /* rows per ring slot (0: no ring) */
+  int64_t device_bytes;    /* device memory tgb200_create allocates */
+  int64_t reserve_bytes;   /* device memory left free for later allocations */
+  int64_t host_bytes;      /* pinned host memory for rows [R, N) */
+} tgb200_state_plan;
+TGB200_API int tgb200_plan_state(const tgb200_config* cfg, uint64_t device_free, tgb200_state_plan* out);
 
 /* ---- lifetime -------------------------------------------------------------------- */
 
@@ -386,6 +411,8 @@ TGB200_API int tgb200_set_state(tgb200_mapper* h, const float* M, const float* m
 
 /* ---- introspection ----------------------------------------------------------------- */
 
+/* Rows [0, *out) of M, m / mb and v are in device memory, the rest in pinned host memory (n_cells: device state). */
+TGB200_API int tgb200_resident_rows(tgb200_mapper* h, int32_t* out);
 /* Kernels launched by this handle since creation (for bench.py's gpu_launches). */
 TGB200_API int tgb200_kernel_launches(tgb200_mapper* h, int64_t* n);
 /* Runs ONE full iteration with CUDA events around each kernel on `stream`;

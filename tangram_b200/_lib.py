@@ -14,7 +14,7 @@ PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 DENSITY_NONE, DENSITY_CELLS, DENSITY_SOURCE = 0, 1, 2
 GRAPH_VOXEL_WEIGHTS, GRAPH_NEIGHBORHOOD_FILTER, GRAPH_SPATIAL_WEIGHTS = 0, 1, 2
 # where M and Adam's moments live (tgb200_state_memory)
-STATE_MEMORY = {"device": 0, "host": 1}
+STATE_MEMORY = {"device": 0, "host": 1, "auto": 2}
 
 
 class Config(ctypes.Structure):
@@ -32,6 +32,12 @@ class Config(ctypes.Structure):
         ("constrained", ctypes.c_int32), ("lambda_count", ctypes.c_float), ("lambda_f_reg", ctypes.c_float),
         ("target_count", ctypes.c_float), ("state_memory", ctypes.c_int32),
     ]
+
+
+class StatePlan(ctypes.Structure):
+    """tgb200_state_plan: where a handle keeps M and Adam's moments (tgb200_plan_state)."""
+    _fields_ = [("resident_rows", ctypes.c_int32), ("block_rows", ctypes.c_int32), ("device_bytes", ctypes.c_int64),
+                ("reserve_bytes", ctypes.c_int64), ("host_bytes", ctypes.c_int64)]
 
 
 class MtState(ctypes.Structure):
@@ -112,6 +118,8 @@ SIGNATURES = {
                                           _P, _P, _P, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int64, ctypes.c_int32, _P]),
     "tgb200_get_state":(ctypes.c_int, [_P, _P, _P, _P, _I64, _P]),
     "tgb200_set_state": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int64, _P]),
+    "tgb200_plan_state": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_uint64, ctypes.POINTER(StatePlan)]),
+    "tgb200_resident_rows": (ctypes.c_int, [_P, _I32]),
     "tgb200_kernel_launches": (ctypes.c_int, [_P, _I64]),
     "tgb200_profile_step": (ctypes.c_int, [_P, ctypes.c_float, _P, ctypes.POINTER(ctypes.c_char_p), _F,
                                            ctypes.c_int32, _I32]),

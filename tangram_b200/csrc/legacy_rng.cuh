@@ -109,7 +109,9 @@ struct DrawParams {
   long long t_lo, t_hi;        // stream normals written: [t_lo, t_hi) -> M element t - t_lo
   int has_gauss;               // normal 0 is numpy's cached value (written by the host)
   int V, ld;
-  float* M;
+  float* M;                    // elements [0, split) of the mapping (row * ld + column)
+  float* Mh;                   // elements from split on (host state: rows [R, N) in pinned host memory)
+  long long split;
   long long a_end;             // accepted attempt that ends the draw: its attempt index and words go to *end
   EndRecord* end;
   Flagged* flags;
@@ -187,7 +189,7 @@ __global__ void __launch_bounds__(kN) k_legacy_pass(DrawParams p) {
             const double v = __dmul_rn(f, comp ? x1 : x2);
             const long long e = tc - p.t_lo, row = e / p.V;
             const long long idx = row * p.ld + (e - row * p.V);
-            p.M[idx] = __double2float_rn(v);
+            (idx < p.split ? p.M + idx : p.Mh + (idx - p.split))[0] = __double2float_rn(v);
             const long long low = __double_as_longlong(v) & ((1LL << 29) - 1);
             if (llabs(low - (1LL << 28)) <= kFlagUlps) {
               const int slot = atomicAdd(p.n_flags, 1);

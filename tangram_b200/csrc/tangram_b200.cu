@@ -186,11 +186,15 @@ struct tgb200_mapper {
   // chunks; forward(c) of the next iteration waits only for Adam(c).  Which stream a launch goes to is the Lanes of its
   // API call (below).
   bool pipelined = false;       // several chunks: the handle has the streams hi, lo and sf
-  // host state (TGB200_STATE_HOST): M, m / mb and v in pinned host memory, and a ring of two device slots of `ring_rows`
-  // rows each through which every per-iteration pass streams them (staged_rows): copy-in of block b+1 on `cin` and
-  // copy-out of block b-1 on `cout` run on the copy engines under block b's kernel
-  bool host_state = false;
+  // host state (TGB200_STATE_HOST, TGB200_STATE_AUTO): rows [0, R) of M, m / mb and v stay in the device buffers above,
+  // rows [R, N) are in pinned host memory (Mh, mh / mbh, vh; R = 0 with host state), and a ring of two device slots of
+  // `ring_rows` rows each through which every per-iteration pass streams the host rows (staged_rows): copy-in of block
+  // b+1 on `cin` and copy-out of block b-1 on `cout` run on the copy engines under block b's kernel
+  bool host_state = false;      // R < N
+  int R = 0;
   int ring_rows = 0;
+  DevBuf<float> Mh, mh, vh;
+  DevBuf<__nv_bfloat16> mbh;
   DevBuf<float> rM[2], rm[2], rv[2];
   DevBuf<__nv_bfloat16> rmb[2];
   cudaStream_t cin = nullptr, cout = nullptr;
@@ -294,7 +298,142 @@ extern "C" int tgb200_host_unpin(void* buf) {
 extern "C" const char* tgb200_last_error(void) { return g_err; }
 extern "C" const char* tgb200_version(void) { return "tangram_b200 0.3.0 (sm_90a)"; }
 
-static int setup_host_state(tgb200_mapper* h);
+static int setup_host_state(tgb200_mapper* h, int block_rows);
+static const char* state_memory_name(int32_t sm) { return sm == TGB200_STATE_HOST ? "host" : "auto"; }
+
+// ---- state placement (tgb200_plan_state) ----------------------------------------------
+// what cudaMalloc takes for one allocation at most: 2 MiB pages (small allocations share them)
+static int64_t alloc_bytes(int64_t b) { return b <= 0 ? 0 : round_up(b, (int64_t)2 << 20); }
+constexpr int kMaxSms = 132;                 // the most SMs an sm_90 part has: the forward's split count is largest there
+
+// The device memory tgb200_create allocates besides M, m / mb, v and the ring: its buffers in the order it allocates
+// them, each rounded up as alloc_bytes does.  Keep in step with tgb200_create (test_state_auto_gpu checks the bound).
+static int64_t operand_bytes(const tgb200_config& c) {
+  const int64_t N = c.n_cells, V = c.n_voxels, K = c.n_genes, T = c.n_types;
+  const int64_t Ke = round_up(K + 2 + T, 64), ld = round_up(V, 64), nv = N * ld, nk = N * Ke, vk = V * Ke;
+  const bool bf16 = c.precision == TGB200_PREC_BF16, x3 = c.precision == TGB200_PREC_BF16X3, tcm = bf16 || x3;
+  int64_t b = 0;
+  auto A = [&](int64_t bytes) { b += alloc_bytes(bytes); };
+  if (x3) A(4 * nv);                                           // dpf
+  if (bf16) {
+    A(2 * nk); for (int i = 0; i < 4; ++i) A(4 * N);          // Sxs, lse0, lse1, inv_zt, zsum
+    if (c.lambda_r != 0.f) A(4 * N);
+    if (c.lambda_l1 != 0.f || c.lambda_l2 != 0.f) { A(4 * N); A(4 * N); }
+    A(16 * N); A(2 * nv); A(2 * nk); A(2 * vk); A(2 * nv); A(4 * N);   // rowc, Pb, Sxb, dYb, dq, rcenter
+  } else if (x3) {
+    A(6 * nv); A(6 * nk); A(6 * vk);
+  } else {
+    A(4 * nv);
+  }
+  A(4 * nk); A(4 * vk); A(4 * V); A(4 * N); A((int64_t)sizeof(RowStat) * N); A(8 * N); A(4 * N);
+  int nc = 1;
+  if (bf16 && !c.constrained) {
+    nc = N >= 32768 ? 4 : (N >= 8192 ? 2 : 1);
+    while (nc > 1 && N / nc < 1024) --nc;
+  }
+  int splits = 1;
+  if (nc == 1 && tcm) {
+    splits = tc_forward_splits(kMaxSms, (int)N, (int)V, (int)Ke);
+    if (x3) splits = std::max(splits, tc_splits_for_chain(N, 2048));
+  } else if (!tcm) {
+    splits = std::clamp((int)ceil_div(2 * kMaxSms, ceil_div(V, 128) * ceil_div(Ke, 128)), 1, (int)ceil_div(N, 512));
+  }
+  if (splits > 1) A(4 * splits * vk);
+  A(4 * (vk + kTail));
+  if (!tcm) A(4 * vk);
+  if (c.constrained) { for (int i = 0; i < 4; ++i) A(4 * N); A(4 * nk); A(16); }
+  const int64_t r_parts = tcm ? tc_dp_row_parts((int)V) : ceil_div(Ke, SG_BN);
+  A(4 * r_parts * N);
+  A(4 * Ke); A(4 * V);
+  int64_t loss_rows = 16;
+  while (ceil_div(V, loss_rows) > 512 && loss_rows < kLossRowsMax) loss_rows += 16;
+  const int64_t nchunk = ceil_div(V, loss_rows), ncolchunk = ceil_div(Ke, kLossCols);
+  A(4 * 7 * Ke); A(4 * nchunk * 3 * Ke); A(4 * Ke); A(4 * Ke); A(4 * Ke); A(4 * V);
+  if (c.lambda_g2 != 0.f) { A(4 * ncolchunk * V * 2); A(4 * V); A(4 * V); }
+  if (c.lambda_neighborhood_g1 > 0.f) { A(4 * vk); A(4 * Ke); A(4 * vk); A(4 * nchunk * 2 * Ke); A(4 * Ke); A(4 * Ke); }
+  if (c.lambda_getis_ord > 0.f) {
+    A(4 * vk); A(4 * Ke); A(4 * Ke); A(4 * vk); A(4 * nchunk * 2 * Ke); A(4 * Ke); A(4 * Ke);
+  }
+  if (c.lambda_ct_islands > 0.f) { A(4 * V * T); A(4 * ceil_div(V * T, 256)); }
+  return b;
+}
+
+// What the handle allocates after tgb200_create and a row split must leave free.  1 GiB holds CUDA's loading of this
+// library's kernels with their local memory, the legacy draw's scratch (tens of MiB at 160k x 24k), the CSR graphs of
+// the spatial terms (12 B per edge), the history (64 B per epoch), tgb200_get_state's one-row scratch and a projection's
+// smallest block; the projection sizes its blocks to the memory then free, and its output (n_voxels x genes floats) is the
+// caller's choice.  Added to it: the validation's scratch and set_comm's copy of the exchange buffer, which scale with the
+// shape.
+static int64_t reserve_bytes(const tgb200_config& c) {
+  const int64_t V = c.n_voxels, Ke = round_up((int64_t)c.n_genes + 2 + c.n_types, 64);
+  return ((int64_t)1 << 30) + alloc_bytes(4 * (2 * Ke + 2 * V)) + alloc_bytes(4 * TGB200_HIST_COLS) +
+         alloc_bytes(4 * ceil_div(Ke, kLossCols) * V * 2) + alloc_bytes(4 * (V * Ke + kTail));
+}
+
+// bytes of one row of M, m / mb and v
+static int64_t state_row_bytes(const tgb200_config& c) {
+  return round_up(c.n_voxels, 64) * (c.precision == TGB200_PREC_BF16 ? 4 + 2 + 4 : 4 + 4 + 4);
+}
+
+// device bytes of rows [0, R) of the state and of a ring of two slots of `rb` rows (three allocations each)
+static int64_t state_device_bytes(const tgb200_config& c, int64_t R, int64_t rb) {
+  const int64_t ld = round_up(c.n_voxels, 64), mb = c.precision == TGB200_PREC_BF16 ? 2 : 4;
+  return 2 * alloc_bytes(4 * R * ld) + alloc_bytes(mb * R * ld) + 2 * (2 * alloc_bytes(4 * rb * ld) + alloc_bytes(mb * rb * ld));
+}
+
+static int64_t env_rows(const char* name) {
+  const char* e = getenv(name);
+  return e && *e ? atoll(e) : -1;
+}
+
+extern "C" int tgb200_plan_state(const tgb200_config* cfg, uint64_t device_free, tgb200_state_plan* out) {
+  if (!cfg || !out) return fail(TGB200_ERR_INVALID, "null argument");
+  const tgb200_config& c = *cfg;
+  if (c.n_cells <= 0 || c.n_voxels <= 0 || c.n_genes <= 0 || c.n_types < 0)
+    return fail(TGB200_ERR_INVALID, "bad shape cells=%d voxels=%d genes=%d types=%d", c.n_cells, c.n_voxels, c.n_genes, c.n_types);
+  if (c.precision != TGB200_PREC_FP32 && c.precision != TGB200_PREC_BF16 && c.precision != TGB200_PREC_BF16X3)
+    return fail(TGB200_ERR_INVALID, "unknown precision %d", c.precision);
+  if (c.state_memory < TGB200_STATE_DEVICE || c.state_memory > TGB200_STATE_AUTO)
+    return fail(TGB200_ERR_INVALID, "unknown state_memory %d", c.state_memory);
+  if (c.state_memory != TGB200_STATE_DEVICE && c.precision == TGB200_PREC_FP32)
+    return fail(TGB200_ERR_UNSUPPORTED, "state_memory = %s needs precision bf16 or bf16x3: fp32 fuses Adam into its FFMA contraction",
+                state_memory_name(c.state_memory));
+  const int64_t N = c.n_cells, sr = state_row_bytes(c), ops = operand_bytes(c), res = reserve_bytes(c);
+  const int64_t free_b = (int64_t)std::min<uint64_t>(device_free, (uint64_t)INT64_MAX);
+  // rows per ring slot: both slots take at most an eighth of what the operands leave free and 128 MiB in all -- a block
+  // of 64 MiB is copied at link speed
+  int64_t rb0 = env_rows("TGB200_STATE_BLOCK_ROWS");
+  if (rb0 < 0) rb0 = std::min<int64_t>(std::max<int64_t>(free_b - ops, 0) / 8, (int64_t)128 << 20) / (2 * sr);
+  rb0 = std::clamp<int64_t>(rb0, 1, N);
+  int64_t R = N, rb = 0;
+  if (c.state_memory == TGB200_STATE_HOST) {
+    R = 0; rb = rb0;
+  } else if (c.state_memory == TGB200_STATE_AUTO) {
+    const int64_t forced = env_rows("TGB200_STATE_RESIDENT_ROWS");
+    if (forced >= 0) {
+      R = std::min<int64_t>(forced, N);
+      rb = R < N ? std::min<int64_t>(rb0, N - R) : 0;
+    } else if (ops + state_device_bytes(c, N, 0) + res > free_b) {
+      // R + 2 rb rows of state fit in what the operands, the reserve and the allocations' rounding leave; the slots
+      // shrink when fewer than 2 rb0 rows fit, and R + rb <= N holds because fewer than N rows fit
+      const int64_t k = std::max<int64_t>(free_b - ops - res - 9 * alloc_bytes(1), 0) / sr;
+      rb = std::clamp<int64_t>(std::min<int64_t>(rb0, k / 2), 1, N);
+      R = std::max<int64_t>(k - 2 * rb, 0);
+    }
+  }
+  out->resident_rows = (int32_t)R;
+  out->block_rows = (int32_t)rb;
+  out->device_bytes = ops + state_device_bytes(c, R, rb);
+  out->reserve_bytes = res;
+  out->host_bytes = (N - R) * sr;
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_resident_rows(tgb200_mapper* h, int32_t* out) {
+  if (!h || !out) return fail(TGB200_ERR_INVALID, "null argument");
+  *out = h->R;
+  return TGB200_OK;
+}
 
 extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (!cfg || !out) return fail(TGB200_ERR_INVALID, "null argument");
@@ -323,10 +462,11 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
       return fail(TGB200_ERR_INVALID, "constrained mode has no spatial / L1 / L2 terms (mapping_optimizer.py:417-432)");
     if (cfg->n_cells_global > 0 && cfg->n_cells_global != cfg->n_cells && cfg->target_count <= 0.f) return fail(TGB200_ERR_INVALID, "target_count must be given");
   }
-  if (cfg->state_memory != TGB200_STATE_DEVICE && cfg->state_memory != TGB200_STATE_HOST)
+  if (cfg->state_memory < TGB200_STATE_DEVICE || cfg->state_memory > TGB200_STATE_AUTO)
     return fail(TGB200_ERR_INVALID, "unknown state_memory %d", cfg->state_memory);
-  if (cfg->state_memory == TGB200_STATE_HOST && cfg->precision == TGB200_PREC_FP32)
-    return fail(TGB200_ERR_UNSUPPORTED, "state_memory = host needs precision bf16 or bf16x3: fp32 fuses Adam into its FFMA contraction");
+  if (cfg->state_memory != TGB200_STATE_DEVICE && cfg->precision == TGB200_PREC_FP32)
+    return fail(TGB200_ERR_UNSUPPORTED, "state_memory = %s needs precision bf16 or bf16x3: fp32 fuses Adam into its FFMA contraction",
+                state_memory_name(cfg->state_memory));
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
@@ -338,6 +478,13 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   if (prop.major != 9 || prop.minor != 0)
     return fail(TGB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major, prop.minor);
   CK(cudaSetDevice(cfg->device));
+  // the row split of TGB200_STATE_AUTO, planned on the memory free before anything of this handle is allocated
+  tgb200_state_plan plan{};
+  if (cfg->state_memory == TGB200_STATE_AUTO) {
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    CKS(tgb200_plan_state(cfg, free_b, &plan));
+  }
 
   tgb200_mapper* h = new tgb200_mapper();
   h->cfg = *cfg;
@@ -357,11 +504,15 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
   const size_t nv = (size_t)h->N * h->ld, vk = (size_t)h->V * h->Ke;
   int st = TGB200_OK;
   auto A = [&](int s) { if (st == TGB200_OK) st = s; };
-  h->host_state = cfg->state_memory == TGB200_STATE_HOST;
-  h->M.host = h->m.host = h->mb.host = h->v.host = h->host_state;
+  h->R = cfg->state_memory == TGB200_STATE_HOST ? 0 : cfg->state_memory == TGB200_STATE_AUTO ? plan.resident_rows : h->N;
+  h->host_state = h->R < h->N;
+  h->Mh.host = h->mh.host = h->mbh.host = h->vh.host = true;
+  const size_t nr = (size_t)h->R * h->ld, nh = nv - nr;
   if (h->x3) A(h->dpf.alloc(nv, false));
-  A(h->M.alloc(nv)); A(h->v.alloc(nv));
-  if (h->bf16) A(h->mb.alloc(nv)); else A(h->m.alloc(nv));
+  A(h->M.alloc(nr)); A(h->v.alloc(nr));
+  if (h->bf16) A(h->mb.alloc(nr)); else A(h->m.alloc(nr));
+  A(h->Mh.alloc(nh)); A(h->vh.alloc(nh));
+  if (h->bf16) A(h->mbh.alloc(nh)); else A(h->mh.alloc(nh));
   if (h->bf16) {
     A(h->Sxs.alloc((size_t)h->N * h->Ke)); A(h->lse0.alloc(h->N)); A(h->lse1.alloc(h->N)); A(h->inv_zt.alloc(h->N));
     A(h->zsum.alloc(h->N));
@@ -457,7 +608,7 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
     A(h->H.alloc((size_t)h->V * h->T)); A(h->ctpart.alloc(h->n_ct_blocks));
   }
   if (st == TGB200_OK && h->tcm) st = tc_init(h->tc, g_err, sizeof(g_err));
-  if (st == TGB200_OK && h->host_state) st = setup_host_state(h);
+  if (st == TGB200_OK && h->host_state) st = setup_host_state(h, plan.block_rows);
   if (st != TGB200_OK) { delete h; return st; }
   CK(cudaDeviceSynchronize());
   *out = h;
@@ -627,34 +778,52 @@ extern "C" int tgb200_set_graph(tgb200_mapper* h, int which, const int32_t* indp
   return TGB200_OK;
 }
 
-// cudaMemsetAsync(0) of M, m / mb or v; in host memory a kernel writes the zeros (rows of ld elements: 16-byte multiples)
+// cudaMemsetAsync(0) of M, m / mb or v: its device rows `d` and its host rows `hp`, into which a kernel writes the zeros
+// (rows of ld elements: 16-byte multiples)
 template <typename T>
-static int zero_state(tgb200_mapper* h, DevBuf<T>& b, cudaStream_t s) {
-  const size_t bytes = b.n * sizeof(T);
-  if (!b.host) {
-    CK(cudaMemsetAsync(b.p, 0, bytes, s));
-    return TGB200_OK;
-  }
-  const long long n16 = (long long)(bytes / 16);
-  k_zero16<<<(unsigned)std::min<long long>(ceil_div(n16, 256), 2048), 256, 0, s>>>(reinterpret_cast<uint4*>(b.p), n16);
+static int zero_state(tgb200_mapper* h, DevBuf<T>& d, DevBuf<T>& hp, cudaStream_t s) {
+  if (d.n) CK(cudaMemsetAsync(d.p, 0, d.n * sizeof(T), s));
+  if (!hp.n) return TGB200_OK;
+  const long long n16 = (long long)(hp.n * sizeof(T) / 16);
+  k_zero16<<<(unsigned)std::min<long long>(ceil_div(n16, 256), 2048), 256, 0, s>>>(reinterpret_cast<uint4*>(hp.p), n16);
   LAUNCH_CHECK("zero16");
   return TGB200_OK;
 }
 
-// Host state: zero M, m / mb and v once (as the device path's cudaMalloc'd state is), then the ring.  Its two slots take at
-// most an eighth of the free device memory and 128 MiB in all -- a block of 64 MiB is copied at link speed, and the
-// device keeps room for the projection's and validation's scratch; TGB200_STATE_BLOCK_ROWS sets the rows per block.
-static int setup_host_state(tgb200_mapper* h) {
-  CKS(zero_state(h, h->M, nullptr));
-  if (h->bf16) CKS(zero_state(h, h->mb, nullptr)); else CKS(zero_state(h, h->m, nullptr));
-  CKS(zero_state(h, h->v, nullptr));
+// row r of M, m / mb or v: rows [0, R) in the device buffer `d`, rows [R, N) in the host buffer `hp`
+template <typename T>
+static T* state_row(const tgb200_mapper* h, const DevBuf<T>& d, const DevBuf<T>& hp, int64_t r) {
+  return r < h->R ? d.p + r * h->ld : hp.p + (r - h->R) * h->ld;
+}
+
+// f(r0, r1) for each non-empty part of the state: rows [0, R) on the device, rows [R, N) in host memory
+template <typename F>
+static int state_parts(const tgb200_mapper* h, F f) {
+  if (h->R > 0) CKS(f(0, h->R));
+  if (h->R < h->N) CKS(f(h->R, h->N));
+  return TGB200_OK;
+}
+
+// Host rows: zero them once (as the device rows' cudaMalloc'd buffers are), then the ring.  `block_rows` (auto state:
+// the plan's) sets the rows per slot; 0 (host state) sizes the two slots from the memory the handle left free: at most an
+// eighth of it and 128 MiB in all -- a block of 64 MiB is copied at link speed, and the device keeps room for the
+// projection's and validation's scratch.  TGB200_STATE_BLOCK_ROWS sets the rows per block.
+static int setup_host_state(tgb200_mapper* h, int block_rows) {
+  DevBuf<float> none;
+  DevBuf<__nv_bfloat16> none_b;
+  CKS(zero_state(h, none, h->Mh, nullptr));
+  if (h->bf16) CKS(zero_state(h, none_b, h->mbh, nullptr)); else CKS(zero_state(h, none, h->mh, nullptr));
+  CKS(zero_state(h, none, h->vh, nullptr));
   const size_t row_bytes = (size_t)h->ld * (h->bf16 ? 4 + 2 + 4 : 4 + 4 + 4);
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  const size_t budget = std::min<size_t>(free_b / 8, (size_t)128 << 20);
-  int64_t rows = (int64_t)(budget / (2 * row_bytes));
-  if (const char* e = getenv("TGB200_STATE_BLOCK_ROWS")) rows = atoll(e);
-  h->ring_rows = (int)std::clamp<int64_t>(rows, 1, h->N);
+  int64_t rows = block_rows;
+  if (rows <= 0) {
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const size_t budget = std::min<size_t>(free_b / 8, (size_t)128 << 20);
+    rows = (int64_t)(budget / (2 * row_bytes));
+    if (const char* e = getenv("TGB200_STATE_BLOCK_ROWS")) rows = atoll(e);
+  }
+  h->ring_rows = (int)std::clamp<int64_t>(rows, 1, h->N - h->R);
   const size_t n = (size_t)h->ring_rows * h->ld;
   for (int k = 0; k < 2; ++k) {
     CKS(h->rM[k].alloc(n, false)); CKS(h->rv[k].alloc(n, false));
@@ -668,8 +837,9 @@ static int setup_host_state(tgb200_mapper* h) {
   return TGB200_OK;
 }
 
-// a row-shifted base: row i of the slot block that starts at row b0 is at base + i * ld for i in [b0, b0 + ring_rows), so
-// the kernels index the slot with the mapping's own row numbers and run exactly their resident arithmetic
+// a row-shifted base: row i of the block that starts at row b0 is at base + i * ld for i in [b0, b0 + ring_rows), so
+// the kernels index the slot (or the host part of the state) with the mapping's own row numbers and run exactly their
+// resident arithmetic
 template <typename T>
 static T* shifted(T* slot, int b0, int ld) {
   return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(slot) - (uintptr_t)b0 * ld * sizeof(T));
@@ -677,46 +847,56 @@ static T* shifted(T* slot, int b0, int ld) {
 
 struct StagedPtrs { float* M; float* m; __nv_bfloat16* mb; float* v; };
 
-// Rows [r0, r1) of the host state through the ring, in blocks of ring_rows, each block's kernel on `s`:
-// `launch(b0, b1, ptrs)` with row-shifted slot bases.  The copy-in of block b+1 (stream cin) and the copy-out of block
-// b-1 (stream cout, `write` passes only: M, m / mb, v) overlap block b's kernel.  The pass starts after the work queued on
-// `s` and after the previous staged pass (whatever stream ran it) has finished with the slots and written the host copy
-// back; `s` continues after the last copy-out.  Without host state, one launch on the resident buffers.
+// Rows [r0, r1) of the state, each launch on `s`: `launch(b0, b1, ptrs)` with bases that row i of [b0, b1) is addressed
+// from by the mapping's row number.  Rows below R are launched on the device buffers.  Rows from R on go through the ring
+// in blocks of ring_rows: the copy-in of block b+1 (stream cin) and the copy-out of block b-1 (stream cout, `write`
+// passes only: M, m / mb, v) overlap block b's kernel.  The resident rows are launched in as many pieces as there are
+// staged blocks, plus one, one piece before each block's kernel and one after the last: the copy engines then work under
+// the resident kernels as well, and the pass approaches the larger of the compute of all its rows and the transfer of its
+// staged rows.  A pass with staged rows starts after the work queued on `s` and after the previous staged pass (whatever
+// stream ran it) has finished with the slots and written the host copy back; `s` continues after the last copy-out.
 template <typename F>
 static int staged_rows(tgb200_mapper* h, cudaStream_t s, int r0, int r1, bool write, F launch) {
-  if (!h->host_state) return launch(r0, r1, StagedPtrs{h->M.p, h->m.p, h->mb.p, h->v.p});
-  if (r1 <= r0) return TGB200_OK;
-  const int ld = h->ld;
+  const StagedPtrs dev{h->M.p, h->m.p, h->mb.p, h->v.p};
+  const int rm = std::min(r1, h->R), s0 = std::max(r0, h->R);     // resident rows [r0, rm), staged rows [s0, r1)
+  if (s0 >= r1) return r0 < r1 ? launch(r0, r1, dev) : TGB200_OK;
+  const int ld = h->ld, n_res = std::max(rm - r0, 0), n_blocks = (int)ceil_div(r1 - s0, h->ring_rows);
+  auto resident_piece = [&](int p) -> int {        // piece p of n_blocks + 1
+    const int a = r0 + (int)((int64_t)n_res * p / (n_blocks + 1)), b = r0 + (int)((int64_t)n_res * (p + 1) / (n_blocks + 1));
+    return a < b ? launch(a, b, dev) : TGB200_OK;
+  };
   CK(cudaEventRecord(h->ev_start, s));
   CK(cudaStreamWaitEvent(h->cin, h->ev_start, 0));
   if (h->ring_used) CK(cudaStreamWaitEvent(h->cin, h->ev_last, 0));
   int k = 0;
-  for (int b0 = r0; b0 < r1; b0 += h->ring_rows, ++k) {
+  for (int b0 = s0; b0 < r1; b0 += h->ring_rows, ++k) {
     const int b1 = std::min(r1, b0 + h->ring_rows), sl = k & 1;
-    const size_t off = (size_t)b0 * ld, n = (size_t)(b1 - b0) * ld;
+    const size_t off = (size_t)(b0 - h->R) * ld, n = (size_t)(b1 - b0) * ld;
     if (k >= 2) CK(cudaStreamWaitEvent(h->cin, h->ev_free[sl], 0));       // block k - 2 is done with this slot
-    CK(cudaMemcpyAsync(h->rM[sl].p, h->M.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
+    CK(cudaMemcpyAsync(h->rM[sl].p, h->Mh.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
     if (write) {
-      if (h->bf16) CK(cudaMemcpyAsync(h->rmb[sl].p, h->mb.p + off, n * sizeof(__nv_bfloat16), cudaMemcpyHostToDevice, h->cin));
-      else CK(cudaMemcpyAsync(h->rm[sl].p, h->m.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
-      CK(cudaMemcpyAsync(h->rv[sl].p, h->v.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
+      if (h->bf16) CK(cudaMemcpyAsync(h->rmb[sl].p, h->mbh.p + off, n * sizeof(__nv_bfloat16), cudaMemcpyHostToDevice, h->cin));
+      else CK(cudaMemcpyAsync(h->rm[sl].p, h->mh.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
+      CK(cudaMemcpyAsync(h->rv[sl].p, h->vh.p + off, n * sizeof(float), cudaMemcpyHostToDevice, h->cin));
     }
     CK(cudaEventRecord(h->ev_in[sl], h->cin));
+    CKS(resident_piece(k));
     CK(cudaStreamWaitEvent(s, h->ev_in[sl], 0));
     CKS(launch(b0, b1, StagedPtrs{shifted(h->rM[sl].p, b0, ld), h->rm[sl].p ? shifted(h->rm[sl].p, b0, ld) : nullptr,
                                   h->rmb[sl].p ? shifted(h->rmb[sl].p, b0, ld) : nullptr, shifted(h->rv[sl].p, b0, ld)}));
     CK(cudaEventRecord(h->ev_comp[sl], s));
     if (write) {
       CK(cudaStreamWaitEvent(h->cout, h->ev_comp[sl], 0));
-      CK(cudaMemcpyAsync(h->M.p + off, h->rM[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
-      if (h->bf16) CK(cudaMemcpyAsync(h->mb.p + off, h->rmb[sl].p, n * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost, h->cout));
-      else CK(cudaMemcpyAsync(h->m.p + off, h->rm[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
-      CK(cudaMemcpyAsync(h->v.p + off, h->rv[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
+      CK(cudaMemcpyAsync(h->Mh.p + off, h->rM[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
+      if (h->bf16) CK(cudaMemcpyAsync(h->mbh.p + off, h->rmb[sl].p, n * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost, h->cout));
+      else CK(cudaMemcpyAsync(h->mh.p + off, h->rm[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
+      CK(cudaMemcpyAsync(h->vh.p + off, h->rv[sl].p, n * sizeof(float), cudaMemcpyDeviceToHost, h->cout));
       CK(cudaEventRecord(h->ev_free[sl], h->cout));
     } else {
       CK(cudaEventRecord(h->ev_free[sl], s));
     }
   }
+  CKS(resident_piece(n_blocks));
   // everything of this pass: the last kernel on s and, for a write pass, the copy-outs (cout is in order)
   if (write) CK(cudaEventRecord(h->ev_last, h->cout));
   else CK(cudaEventRecord(h->ev_last, s));
@@ -726,9 +906,9 @@ static int staged_rows(tgb200_mapper* h, cudaStream_t s, int r0, int r1, bool wr
 }
 
 static int zero_moments(tgb200_mapper* h, cudaStream_t s) {
-  if (h->bf16) CKS(zero_state(h, h->mb, s));
-  else CKS(zero_state(h, h->m, s));
-  CKS(zero_state(h, h->v, s));
+  if (h->bf16) CKS(zero_state(h, h->mb, h->mbh, s));
+  else CKS(zero_state(h, h->m, h->mh, s));
+  CKS(zero_state(h, h->v, h->vh, s));
   return TGB200_OK;
 }
 
@@ -830,9 +1010,12 @@ extern "C" int tgb200_set_mapping(tgb200_mapper* h, const float* M0, void* strea
   if (!h || !M0) return fail(TGB200_ERR_INVALID, "null argument");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
-  CKS(zero_state(h, h->M, s));
-  CK(cudaMemcpy2DAsync(h->M.p, (size_t)h->ld * sizeof(float), M0, (size_t)h->V * sizeof(float),
-                       (size_t)h->V * sizeof(float), h->N, cudaMemcpyDefault, s));
+  CKS(zero_state(h, h->M, h->Mh, s));
+  CKS(state_parts(h, [&](int r0, int r1) -> int {
+    CK(cudaMemcpy2DAsync(state_row(h, h->M, h->Mh, r0), (size_t)h->ld * sizeof(float), M0 + (size_t)r0 * h->V,
+                         (size_t)h->V * sizeof(float), (size_t)h->V * sizeof(float), r1 - r0, cudaMemcpyDefault, s));
+    return TGB200_OK;
+  }));
   CKS(reset_optimizer(h, s));
   h->have_mapping = true;
   CK(cudaStreamSynchronize(s));
@@ -876,9 +1059,13 @@ extern "C" int tgb200_init_mapping_normal_rows(tgb200_mapper* h, uint64_t seed, 
   if (first_row < 0) return fail(TGB200_ERR_INVALID, "first_row < 0");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
-  const long long nq = (long long)h->N * (h->ld / 4);
-  k_init_normal<<<(unsigned)ceil_div(nq, 256), 256, 0, s>>>(h->M.p, h->N, h->V, h->ld, seed, (long long)first_row);
-  LAUNCH_CHECK("init_normal");
+  CKS(state_parts(h, [&](int r0, int r1) -> int {      // the device rows and the host rows: the same draw per global row
+    const long long nq = (long long)(r1 - r0) * (h->ld / 4);
+    k_init_normal<<<(unsigned)ceil_div(nq, 256), 256, 0, s>>>(state_row(h, h->M, h->Mh, r0), r1 - r0, h->V, h->ld, seed,
+                                                                 (long long)first_row + r0);
+    LAUNCH_CHECK("init_normal");
+    return TGB200_OK;
+  }));
   CKS(reset_optimizer(h, s));
   h->have_mapping = true;
   return TGB200_OK;
@@ -978,7 +1165,7 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
   std::fill(stats, stats + 8, 0.f);
   EventSet ev;
   for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
-  CKS(zero_state(h, h->M, s));
+  CKS(zero_state(h, h->M, h->Mh, s));
   EndRecord end_h{-1, {0, 0, 0, 0}};
   int64_t n_fixed = 0, n_changed = 0;
   std::vector<float> patch_vals;
@@ -1003,6 +1190,8 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
     p.V = h->V;
     p.ld = h->ld;
     p.M = h->M.p;
+    p.Mh = h->Mh.p;
+    p.split = (long long)h->R * h->ld;
     p.a_end = a_end;
     for (;;) {
       if (nb > (1LL << 30)) return fail(TGB200_ERR_INVALID, "draw of %lld normals is too large", (long long)end_normal);
@@ -1074,20 +1263,21 @@ extern "C" int tgb200_init_mapping_legacy(tgb200_mapper* h, const tgb200_mt_stat
     std::vector<Flagged> fl(nf);
     std::vector<float> dev_vals(nf);
     if (nf) CK(cudaMemcpy(fl.data(), flags.p, nf * sizeof(Flagged), cudaMemcpyDeviceToHost));
-    for (int i = 0; i < nf; ++i) CK(cudaMemcpyAsync(&dev_vals[i], h->M.p + fl[i].idx, sizeof(float), cudaMemcpyDefault, s));
+    auto elem = [&](long long idx) { return state_row(h, h->M, h->Mh, idx / h->ld) + idx % h->ld; };
+    for (int i = 0; i < nf; ++i) CK(cudaMemcpyAsync(&dev_vals[i], elem(fl[i].idx), sizeof(float), cudaMemcpyDefault, s));
     CK(cudaStreamSynchronize(s));
     patch_vals.resize(nf);
     for (int i = 0; i < nf; ++i) {
       patch_vals[i] = (float)polar_value_host(fl[i].w, fl[i].comp);
       if (std::memcmp(&patch_vals[i], &dev_vals[i], sizeof(float)) != 0) {
-        CK(cudaMemcpyAsync(h->M.p + fl[i].idx, &patch_vals[i], sizeof(float), cudaMemcpyDefault, s));
+        CK(cudaMemcpyAsync(elem(fl[i].idx), &patch_vals[i], sizeof(float), cudaMemcpyDefault, s));
         ++n_changed;
       }
     }
     n_fixed = nf;
   }
   float cached = (float)start->gauss;
-  if (hg && t_lo == 0) CK(cudaMemcpyAsync(h->M.p, &cached, sizeof(float), cudaMemcpyDefault, s));   // normal 0
+  if (hg && t_lo == 0) CK(cudaMemcpyAsync(state_row(h, h->M, h->Mh, 0), &cached, sizeof(float), cudaMemcpyDefault, s));   // normal 0
   if (a_end >= 0) CK(cudaEventRecord(ev.e[4], s));
   CKS(reset_optimizer(h, s));
   h->have_mapping = true;
@@ -1830,22 +2020,32 @@ extern "C" int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, 
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
   const size_t w = (size_t)h->V * sizeof(float), pitch = (size_t)h->ld * sizeof(float);
-  if (M) CK(cudaMemcpy2DAsync(M, w, h->M.p, pitch, w, h->N, cudaMemcpyDefault, s));
-  if (m && !h->bf16) CK(cudaMemcpy2DAsync(m, w, h->m.p, pitch, w, h->N, cudaMemcpyDefault, s));
+  // each part of the state (device rows, host rows) on its own
+  auto get = [&](float* dst, const DevBuf<float>& d, const DevBuf<float>& hp) {
+    return state_parts(h, [&](int a, int b) -> int {
+      CK(cudaMemcpy2DAsync(dst + (size_t)a * h->V, w, state_row(h, d, hp, a), pitch, w, b - a, cudaMemcpyDefault, s));
+      return TGB200_OK;
+    });
+  };
+  if (M) CKS(get(M, h->M, h->Mh));
+  if (m && !h->bf16) CKS(get(m, h->m, h->mh));
   if (m && h->bf16) {         // bf16 first moment -> fp32 for the caller
     float* scratch;
     int blk;
     DevBuf<float> one_row;
     CKS(moment_scratch(h, one_row, &scratch, &blk));
-    for (int r0 = 0; r0 < h->N; r0 += blk) {
-      const int nr = h->N - r0 < blk ? h->N - r0 : blk;
-      const long long n = (long long)nr * h->ld;
-      k_bf16_to_f32<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(h->mb.p + (size_t)r0 * h->ld, scratch, n);
-      LAUNCH_CHECK("bf16_to_f32");
-      CK(cudaMemcpy2DAsync(m + (size_t)r0 * h->V, w, scratch, pitch, w, nr, cudaMemcpyDefault, s));
-    }
+    CKS(state_parts(h, [&](int a, int b) -> int {
+      for (int r0 = a; r0 < b; r0 += blk) {
+        const int nr = b - r0 < blk ? b - r0 : blk;
+        const long long n = (long long)nr * h->ld;
+        k_bf16_to_f32<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(state_row(h, h->mb, h->mbh, r0), scratch, n);
+        LAUNCH_CHECK("bf16_to_f32");
+        CK(cudaMemcpy2DAsync(m + (size_t)r0 * h->V, w, scratch, pitch, w, nr, cudaMemcpyDefault, s));
+      }
+      return TGB200_OK;
+    }));
   }
-  if (v) CK(cudaMemcpy2DAsync(v, w, h->v.p, pitch, w, h->N, cudaMemcpyDefault, s));
+  if (v) CKS(get(v, h->v, h->vh));
   if (step) *step = h->step;
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
@@ -1857,27 +2057,36 @@ extern "C" int tgb200_set_state(tgb200_mapper* h, const float* M, const float* m
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(h->cfg.device));
   const size_t w = (size_t)h->V * sizeof(float), pitch = (size_t)h->ld * sizeof(float);
+  auto set = [&](const float* src, DevBuf<float>& d, DevBuf<float>& hp) {
+    return state_parts(h, [&](int a, int b) -> int {
+      CK(cudaMemcpy2DAsync(state_row(h, d, hp, a), pitch, src + (size_t)a * h->V, w, w, b - a, cudaMemcpyDefault, s));
+      return TGB200_OK;
+    });
+  };
   if (M) {
-    CK(cudaMemcpy2DAsync(h->M.p, pitch, M, w, w, h->N, cudaMemcpyDefault, s)); h->have_mapping = true; h->p_state = PState::stale;
+    CKS(set(M, h->M, h->Mh)); h->have_mapping = true; h->p_state = PState::stale;
     h->fwd_ahead = false;
     if (h->bf16) CK(cudaMemsetAsync(h->rcenter.p, 0, h->rcenter.n * sizeof(float), s));
   }
-  if (m && !h->bf16) CK(cudaMemcpy2DAsync(h->m.p, pitch, m, w, w, h->N, cudaMemcpyDefault, s));
+  if (m && !h->bf16) CKS(set(m, h->m, h->mh));
   if (m && h->bf16) {         // fp32 from the caller -> bf16 (exact for values that came out of tgb200_get_state)
     float* scratch;
     int blk;
     DevBuf<float> one_row;
     CKS(moment_scratch(h, one_row, &scratch, &blk));
-    for (int r0 = 0; r0 < h->N; r0 += blk) {
-      const int nr = h->N - r0 < blk ? h->N - r0 : blk;
-      const long long n = (long long)nr * h->ld;
-      CK(cudaMemsetAsync(scratch, 0, (size_t)n * sizeof(float), s));            // pad columns stay zero
-      CK(cudaMemcpy2DAsync(scratch, pitch, m + (size_t)r0 * h->V, w, w, nr, cudaMemcpyDefault, s));
-      k_f32_to_bf16<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(scratch, h->mb.p + (size_t)r0 * h->ld, n);
-      LAUNCH_CHECK("f32_to_bf16");
-    }
+    CKS(state_parts(h, [&](int a, int b) -> int {
+      for (int r0 = a; r0 < b; r0 += blk) {
+        const int nr = b - r0 < blk ? b - r0 : blk;
+        const long long n = (long long)nr * h->ld;
+        CK(cudaMemsetAsync(scratch, 0, (size_t)n * sizeof(float), s));            // pad columns stay zero
+        CK(cudaMemcpy2DAsync(scratch, pitch, m + (size_t)r0 * h->V, w, w, nr, cudaMemcpyDefault, s));
+        k_f32_to_bf16<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(scratch, state_row(h, h->mb, h->mbh, r0), n);
+        LAUNCH_CHECK("f32_to_bf16");
+      }
+      return TGB200_OK;
+    }));
   }
-  if (v) CK(cudaMemcpy2DAsync(h->v.p, pitch, v, w, w, h->N, cudaMemcpyDefault, s));
+  if (v) CKS(set(v, h->v, h->vh));
   h->step = step;
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
@@ -1988,13 +2197,25 @@ extern "C" int tgb200_debug_buffer(tgb200_mapper* h, const char* name, float* ou
     if (cap < count) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)count);
     return widen_bf16(p, count, planes, out_host);
   };
+  // the state: its device rows, then its host rows
+  auto state = [&](const auto& d, const auto& hp) -> int {
+    *n = nv;
+    if (!out_host) return TGB200_OK;
+    if (cap < nv) return fail(TGB200_ERR_INVALID, "buffer '%s' needs %lld floats", name, (long long)nv);
+    const size_t nr = (size_t)h->R * h->ld;
+    if constexpr (sizeof(*d.p) == 2) {
+      if (nr) CKS(widen_bf16(d.p, (int64_t)nr, 1, out_host));
+      if (hp.n) CKS(widen_bf16(hp.p, (int64_t)hp.n, 1, out_host + nr));
+    } else {
+      if (nr) CK(cudaMemcpy(out_host, d.p, nr * sizeof(float), cudaMemcpyDefault));
+      if (hp.n) CK(cudaMemcpy(out_host + nr, hp.p, hp.n * sizeof(float), cudaMemcpyDefault));
+    }
+    return TGB200_OK;
+  };
   if (nm == "Y") { src = h->Y.p; cnt = vk; }
-  else if (nm == "M") { src = h->M.p; cnt = nv; }
-  else if (nm == "v") { src = h->v.p; cnt = nv; }
-  else if (nm == "m") {
-    if (h->bf16) return widened(h->mb.p, nv, 1);
-    src = h->m.p; cnt = nv;
-  }
+  else if (nm == "M") return state(h->M, h->Mh);
+  else if (nm == "v") return state(h->v, h->vh);
+  else if (nm == "m") return h->bf16 ? state(h->mb, h->mbh) : state(h->m, h->mh);
   else if (nm == "Pb" && h->x3) return widened(h->Pb.p, nv, 3);
   else if (nm == "Pf" && !h->tcm) { src = h->Pf.p; cnt = nv; }
   else if (nm == "dpf" && h->x3) { src = h->dpf.p; cnt = nv; }

@@ -67,8 +67,8 @@ def check_state_memory(state_memory, precision):
     """Validate Engine's `state_memory` argument for `precision`."""
     if state_memory not in _lib.STATE_MEMORY:
         raise ValueError(f"state_memory must be one of {list(_lib.STATE_MEMORY)}, got {state_memory!r}")
-    if state_memory == "host" and precision not in HOST_STATE_BYTES_PER_ELEMENT:
-        raise ValueError(f"state_memory='host' needs precision 'bf16' or 'bf16x3', not {precision!r}: fp32 fuses Adam "
+    if state_memory != "device" and precision not in HOST_STATE_BYTES_PER_ELEMENT:
+        raise ValueError(f"state_memory={state_memory!r} needs precision 'bf16' or 'bf16x3', not {precision!r}: fp32 fuses Adam "
                          "into its FFMA contraction's epilogue, which reads the optimizer state of every row on the device")
 
 
@@ -98,10 +98,46 @@ def check_host_state_fits(n_cells, n_voxels, n_genes, precision, device, host_av
             f"operands); {device_free / 2**30:.1f} GiB are free")
 
 
+def plan_state(cfg, device_free):
+    """tgb200_plan_state: where a handle of `cfg` (_lib.Config) keeps its state with `device_free` bytes free on its
+    device -- the split tgb200_create makes (TGB200_STATE_RESIDENT_ROWS / TGB200_STATE_BLOCK_ROWS included)."""
+    plan = _lib.StatePlan()
+    _lib.check(_lib.load().tgb200_plan_state(ctypes.byref(cfg), int(device_free), ctypes.byref(plan)))
+    return plan
+
+
+def check_auto_state_fits(cfg, host_available=None, device_free=None):
+    """Before a state_memory="auto" handle is allocated: plan its split as tgb200_create will, and raise
+    TangramB200Error when the host rows would not fit in MemAvailable or not even the operands, the ring and the reserve
+    fit on the device.  `host_available` / `device_free` (bytes) default to /proc/meminfo and torch.cuda.mem_get_info.
+    Returns the plan."""
+    if device_free is None:
+        import torch
+        device_free, _ = torch.cuda.mem_get_info(cfg.device)
+    plan = plan_state(cfg, device_free)
+    n, v = cfg.n_cells, cfg.n_voxels
+    if plan.host_bytes:
+        if host_available is None:
+            host_available = host_memory_available()
+        if host_available is not None and plan.host_bytes > host_available:
+            raise _lib.TangramB200Error(
+                f"state_memory='auto' keeps {plan.resident_rows} of {n} rows on cuda:{cfg.device} and needs "
+                f"{plan.host_bytes / 2**30:.1f} GiB of pinned host memory for the other {n - plan.resident_rows} rows of "
+                f"M, m and v ({n} x {v}); MemAvailable is {host_available / 2**30:.1f} GiB")
+    need_dev = plan.device_bytes + plan.reserve_bytes
+    if need_dev > device_free:
+        raise _lib.TangramB200Error(
+            f"state_memory='auto' needs {need_dev / 2**30:.1f} GiB on cuda:{cfg.device} for {n} x {v} with "
+            f"{plan.resident_rows} rows resident ({plan.device_bytes / 2**30:.1f} GiB of operands, resident rows and "
+            f"ring, {plan.reserve_bytes / 2**30:.1f} GiB kept free); {device_free / 2**30:.1f} GiB are free")
+    return plan
+
+
 class Engine:
     """Config fields not given default to 0, except lambda_g1 (1) and lambda_d (1 when there is a density).
     state_memory="host" keeps M and Adam's moments in pinned host memory (TGB200_STATE_HOST), after checking that both
-    the host and the device side fit."""
+    the host and the device side fit.  state_memory="auto" keeps as many rows on the device as fit and only the rest in
+    pinned host memory (TGB200_STATE_AUTO), after checking the library's plan of that split."""
 
     def __init__(self, n_cells, n_voxels, n_genes, *, n_types=0, n_cells_global=None, device=0,
                  precision="fp32", density_mode=_lib.DENSITY_CELLS, constrained=False, state_memory="device",
@@ -127,6 +163,8 @@ class Engine:
         cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps = 0.9, 0.999, 1e-8      # torch.optim.Adam defaults
         cfg.constrained = int(constrained)
         cfg.state_memory = _lib.STATE_MEMORY[state_memory]
+        if state_memory == "auto":
+            check_auto_state_fits(cfg)
         self.cfg = cfg
         self._h = ctypes.c_void_p()
         _lib.check(self._lib.tgb200_create(ctypes.byref(cfg), ctypes.byref(self._h)))
@@ -280,6 +318,12 @@ class Engine:
         out = np.empty(max(n.value, 4), dtype=np.float32)
         _lib.check(self._lib.tgb200_debug_buffer(self._h, name.encode(), _lib.ptr(out), out.size, ctypes.byref(n)))
         return out[:n.value]
+
+    def resident_rows(self):
+        """Rows [0, R) of M and Adam's moments are in device memory, the rest in pinned host memory."""
+        n = ctypes.c_int32()
+        _lib.check(self._lib.tgb200_resident_rows(self._h, ctypes.byref(n)))
+        return n.value
 
     def kernel_launches(self):
         n = ctypes.c_int64()

@@ -21,7 +21,9 @@ Additions (keyword-only, all optional):
               leaves it instead of after the rank's last row, so that draws made one after another from it (cross_val's
               folds) are the same on every rank
   state_memory "device" (default) | "host": keep M and Adam's moments in pinned host memory, so that a mapping about
-              3.5x (bf16) or 2.2x (bf16x3) larger fits one GPU, with bit-identical results; fp32 is refused
+              3.5x (bf16) or 2.2x (bf16x3) larger fits one GPU, with bit-identical results; fp32 is refused.
+              "auto": keep as many rows on the device as fit and only the rest in host memory (the device handle when
+              every row fits); `resident_rows` tells how many stayed
   train(..., resume=True)  continue with the Adam state of the previous train() call (the reference -- and the default
               here -- builds a fresh optimizer in every train() call, mapping_optimizer.py:373)
   train(..., out=tensor)   write softmax(M) into a CUDA tensor instead of returning a host array
@@ -126,6 +128,12 @@ def format_terms(terms):
 class _EngineMapper:
     """What Mapper and MapperConstrained share: an Engine (`_engine`) of n_cells x n_voxels, the cell-sharded setup and
     loop, the epoch-chunk schedule, the history fetch and the result buffer."""
+
+    @property
+    def resident_rows(self):
+        """Rows of this mapper's (shard of the) mapping whose M and Adam's moments are in device memory: all of them
+        with state_memory="device", none with "host", as many as fit with "auto"; the rest are in pinned host memory."""
+        return self._engine.resident_rows()
 
     def _select_rows(self, n_rows_given, n_cells_global, shard, process_group, presharded=False):
         """Cell-sharded operation: the block [r0, r1) of the n_cells_global cells this rank keeps -- all given rows for a

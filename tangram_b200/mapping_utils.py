@@ -254,7 +254,8 @@ def map_cells_to_space(
                     other ranks return None.
     state_memory    "device" (default) | "host": keep the mapping and Adam's moments in pinned host memory (each rank its
                     own shard), so that a mapping too large for the GPU trains there with bit-identical results; bf16 and
-                    bf16x3 only
+                    bf16x3 only.  "auto": keep as many rows on the device as fit and only the rest in host memory (each
+                    rank plans its own shard on its own device)
     keep_on_device  keep the trained mapper (device state ~20 B per mapping element) attached to the result so that
                     project_genes contracts on the GPU; default: release it (`adata_map.X` is all project_genes needs)."""
     _check_shardable(mode, process_group)

@@ -1,11 +1,14 @@
-"""state_memory="host" against the resident handle: seconds per iteration at C3 (100k x 10k x 2k) in bf16 and bf16x3, with
-whether the two handles give the same bits; the bytes the staging ring copies per iteration over the elapsed time (a
+"""state_memory="host" and "auto" against the resident handle: seconds per iteration at C3 (100k x 10k x 2k) in bf16 and
+bf16x3 for "device", "host" and "auto" with 50 %, 75 % and 90 % of the rows forced resident (each auto time next to its
+bound, the larger of the resident time and the staged rows' bytes over the probe's bidirectional bandwidth), with
+whether every placement gives the same history and softmax(M) bits; the bytes the staging ring copies per iteration over the elapsed time (a
 figure derived from the ring's copy sizes, not a measured link counter) next to a plain cudaMemcpyAsync bandwidth
 probe (H2D, D2H, both at once); the seeded legacy draw into host state; and one run at a size that does not fit resident
-(bf16x3 at 160k x 24k by default), only when MemAvailable and the free device memory hold it.  Prints one JSON object;
+(bf16x3 at 160k x 24k by default) with host state and with the unforced auto split (its R, device and pinned bytes),
+only when MemAvailable and the free device memory hold it.  Prints one JSON object;
 with --out also writes it there.
 
-    python tools/state_host_bench.py [--steps 5] [--big-cells 160000] [--big-spots 24000] [--out results.json]
+    python tools/state_host_bench.py [--steps 5] [--big-cells 160000] [--big-spots 24000] [--skip-big-host] [--out results.json]
 """
 import argparse
 import json
@@ -20,7 +23,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from tangram_b200 import _lib  # noqa: E402
-from tangram_b200.engine import HOST_STATE_BYTES_PER_ELEMENT, Engine, host_memory_available  # noqa: E402
+from tangram_b200.engine import HOST_STATE_BYTES_PER_ELEMENT, Engine, host_memory_available, plan_state  # noqa: E402
 
 # bytes per mapping element the ring copies in one steady-state iteration (staged_rows): the update copies M, m / mb and
 # v in and out; bf16x3 also runs the exact row pass every iteration, which copies M in once more.  Derived from the copy
@@ -91,19 +94,44 @@ def time_steps(e, steps, warmup=2):
     return (time.perf_counter() - t0) / steps
 
 
-def c3_pair(precision, steps, N=100_000, V=10_000, K=2_000):
-    """Resident and host state at C3 from the same Philox draw: s/iteration and whether the mappings agree bit for bit."""
+AUTO_FRACTIONS = (0.5, 0.75, 0.9)
+
+
+def c3_placements(precision, steps, bidir_gbs, N=100_000, V=10_000, K=2_000):
+    """Resident, host and auto state (R forced to each of AUTO_FRACTIONS of the rows) at C3 from the same Philox draw:
+    s/iteration, the auto bound, and whether the history and the mapping agree bit for bit with the resident handle's."""
     out = {}
-    maps = {}
-    for where in ("device", "host"):
-        t0 = time.perf_counter()
-        e = make_engine(N, V, K, precision, where)
-        e.init_mapping_normal(7)
-        torch.cuda.synchronize()
+    ref_map = ref_hist = None
+    same = True
+    ld = -(-V // 64) * 64
+    placements = [("device", None), ("host", None)] + [(f"auto_{int(f * 100)}", int(f * N)) for f in AUTO_FRACTIONS]
+    for where, R in placements:
+        if R is not None:
+            os.environ["TGB200_STATE_RESIDENT_ROWS"] = str(R)
+        try:
+            t0 = time.perf_counter()
+            e = make_engine(N, V, K, precision, "auto" if R is not None else where)
+            e.init_mapping_normal(7)
+            torch.cuda.synchronize()
+        finally:
+            os.environ.pop("TGB200_STATE_RESIDENT_ROWS", None)
         setup = time.perf_counter() - t0
         s_it = time_steps(e, steps)
-        maps[where] = e.get_mapping(np.empty((N, V), dtype=np.float32))
+        mapping = e.get_mapping(np.empty((N, V), dtype=np.float32))
+        hist = e.history(0, e.history_len())
+        if ref_map is None:
+            ref_map, ref_hist = mapping, hist
+        else:
+            same = same and bool(np.array_equal(mapping.view(np.uint32), ref_map.view(np.uint32)) and
+                                 np.array_equal(hist.view(np.uint32), ref_hist.view(np.uint32)))
+        del mapping
         out[where] = dict(setup_s=round(setup, 2), s_per_iter=round(s_it, 4))
+        if R is not None:
+            to_dev, to_host = LINK_BYTES[precision]
+            staged_s = (to_dev + to_host) * (N - R) * ld / (bidir_gbs * 1e9)
+            bound = max(out["device"]["s_per_iter"], staged_s)
+            out[where].update(resident_rows=e.resident_rows(), ring_rows=int(e.debug("ring")[0]),
+                              bound_s=round(bound, 4), of_bound=round(bound / s_it, 2))
         if where == "host":
             out[where]["ring_rows"] = int(e.debug("ring")[0])
             to_dev, to_host = LINK_BYTES[precision]
@@ -117,11 +145,11 @@ def c3_pair(precision, steps, N=100_000, V=10_000, K=2_000):
             out[where]["legacy_draw_s"] = round(time.perf_counter() - t0, 2)
         e.close()
     out["slowdown"] = round(out["host"]["s_per_iter"] / out["device"]["s_per_iter"], 2)
-    out["same_bits"] = bool(np.array_equal(maps["device"].view(np.uint32), maps["host"].view(np.uint32)))
+    out["same_bits"] = same
     return out
 
 
-def big_run(N, V, K, steps, precision="bf16x3"):
+def big_run(N, V, K, steps, precision="bf16x3", placements=("host", "auto")):
     dev_b, host_b = HOST_STATE_BYTES_PER_ELEMENT[precision]
     elems = N * (-(-V // 64) * 64)
     avail = host_memory_available() or 0
@@ -132,19 +160,27 @@ def big_run(N, V, K, steps, precision="bf16x3"):
     if host_b * elems + (8 << 30) > avail:
         res["run"] = "not run: MemAvailable is too small for the pinned host state plus 8 GiB of headroom"
         return res
-    try:
-        t0 = time.perf_counter()
-        e = make_engine(N, V, K, precision, "host")
-        e.init_mapping_normal(7)
-        torch.cuda.synchronize()
-        res["setup_s"] = round(time.perf_counter() - t0, 1)
-        res["device_used_gib"] = round((free - torch.cuda.mem_get_info(0)[0]) / 2**30, 1)
-        res["s_per_iter"] = round(time_steps(e, steps, warmup=1), 3)
-        res["final_loss"] = float(e.history(e.history_len() - 1, 1)[0, 0])
-        e.close()
-        res["run"] = "ran"
-    except _lib.TangramB200Error as ex:
-        res["run"] = f"refused: {ex}"
+    for where in placements:
+        r = res[where] = {}
+        try:
+            t0 = time.perf_counter()
+            free = torch.cuda.mem_get_info(0)[0]
+            e = make_engine(N, V, K, precision, where)
+            e.init_mapping_normal(7)
+            torch.cuda.synchronize()
+            r["setup_s"] = round(time.perf_counter() - t0, 1)
+            r["device_used_gib"] = round((free - torch.cuda.mem_get_info(0)[0]) / 2**30, 1)
+            if where == "auto":
+                plan = plan_state(e.cfg, free)
+                r.update(resident_rows=e.resident_rows(), of_rows=N, ring_rows=int(e.debug("ring")[0]),
+                         plan_device_gib=round(plan.device_bytes / 2**30, 1), plan_reserve_gib=round(plan.reserve_bytes / 2**30, 1),
+                         pinned_gib=round(plan.host_bytes / 2**30, 1))
+            r["s_per_iter"] = round(time_steps(e, steps, warmup=1), 3)
+            r["final_loss"] = float(e.history(e.history_len() - 1, 1)[0, 0])
+            e.close()
+            r["run"] = "ran"
+        except _lib.TangramB200Error as ex:
+            r["run"] = f"refused: {ex}"
     return res
 
 
@@ -155,14 +191,16 @@ def main():
     ap.add_argument("--big-spots", type=int, default=24_000)
     ap.add_argument("--big-genes", type=int, default=256)
     ap.add_argument("--skip-big", action="store_true")
+    ap.add_argument("--skip-big-host", action="store_true", help="at the big size, run only the auto split")
     ap.add_argument("--out")
     a = ap.parse_args()
     torch.cuda.init()
     r = dict(card=card(), copy_probe=copy_probe())
     for precision in ("bf16", "bf16x3"):
-        r[f"c3_{precision}"] = c3_pair(precision, a.steps)
+        r[f"c3_{precision}"] = c3_placements(precision, a.steps, r["copy_probe"]["bidirectional_gbs"])
     if not a.skip_big:
-        r["big"] = big_run(a.big_cells, a.big_spots, a.big_genes, 2)
+        r["big"] = big_run(a.big_cells, a.big_spots, a.big_genes, 2,
+                           placements=("auto",) if a.skip_big_host else ("host", "auto"))
     s = json.dumps(r)
     print(s)
     if a.out:
