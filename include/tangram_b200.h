@@ -404,6 +404,27 @@ TGB200_API int tgb200_project_map(const float* map, int64_t rows, int64_t cols, 
                                   const int64_t* indptr, const int32_t* indices, const float* data, int64_t nnz,
                                   int64_t n_genes, float* out, int64_t block_rows, int32_t device, void* stream);
 
+/* Per-label column statistics of an expression matrix (scanpy's rank_genes_groups basic stats), one pass.
+ *   X        dense rows x n_genes, row-major f32, leading dimension x_ld >= n_genes (host or device), or NULL for CSR:
+ *   indptr / indices / data / nnz   canonical CSR as tgb200_project_map takes it (host or device)
+ *   labels_host  rows int32 in [-1, n_labels) (HOST); -1 rows add to nothing
+ *   sum_out, sumsq_out   n_labels x n_genes doubles (host or device): sum of x and of (double)x*(double)x
+ *   nnz_out              n_labels x n_genes int64 (host or device; NULL to skip): entries with x != 0 (NaN counts)
+ *   block_rows           cells staged per block, a multiple of 2048; 0 = sized from free device memory
+ * Order of additions, for label t and gene k: the rows of each aligned range [2048c, 2048c + 2048) labelled t are summed
+ * in fp64 in row order from 0.0 (one chain per range), and the chains are added in order of c from 0.0.  Absent CSR
+ * entries and explicit zeros add +0.0, so dense and CSR input of the same matrix, host and device pointers, any block_rows
+ * and re-runs give identical bits; no atomics.  Dense X in this device's memory is read in place; host X (dense or CSR)
+ * and CSR from anywhere are staged in double-buffered cell blocks.  Device memory: the outputs, two blocks of staging and
+ * the partials of one block's (range, label) runs (20 n_genes bytes each), independent of `rows`.
+ * TGB200_ERR_INVALID for a bad shape, a malformed indptr, a column outside [0, n_genes) or out of order within its row, a
+ * label outside [-1, n_labels), block_rows not a multiple of 2048, or when free device memory cannot hold one block (the
+ * message gives the sizes); TGB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).  Synchronous on `stream`. */
+TGB200_API int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* indptr, const int32_t* indices,
+                                  const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
+                                  const int32_t* labels_host, int32_t n_labels, double* sum_out, double* sumsq_out,
+                                  int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream);
+
 /* Checkpoint / resume (the reference stubs this: `raise NotImplemented`, :151-153).
  * Any pointer may be NULL to skip it.  M, m, v: n_cells x n_voxels f32, host or device. */
 TGB200_API int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream);

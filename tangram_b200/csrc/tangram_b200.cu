@@ -22,6 +22,7 @@
 #include "agreement.cuh"
 #include "annotate.cuh"
 #include "project.cuh"
+#include "group_stats.cuh"
 #include "mt19937_jump.h"
 #include "nccl_dl.h"
 
@@ -2748,4 +2749,237 @@ extern "C" int tgb200_project(tgb200_mapper* h, const float* X, int64_t n_cols, 
   if (!h->have_mapping) return fail(TGB200_ERR_STATE, "no mapping set");
   return project_blocks(h, nullptr, h->N, h->V, h->ld, X, n_cols, nullptr, nullptr, nullptr, 0, n_cols, out, 0, h->cfg.device,
                         (cudaStream_t)stream);
+}
+
+// Per-label column statistics of an expression matrix (scanpy's rank_genes_groups basic statistics), streamed over cell
+// blocks of whole summation ranges (see group_stats.cuh for the order of additions).
+namespace {
+constexpr int64_t kGsBlocks = 8;          // default: about this many blocks, so the copies of one hide under the others
+constexpr int64_t kGsMaxBlock = 32 * kGsRange;   // 32 ranges x the slabs fill the device; larger blocks only add partials
+}  // namespace
+
+extern "C" int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* indptr, const int32_t* indices,
+                                  const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
+                                  const int32_t* labels, int32_t n_labels, double* sum_out, double* sumsq_out,
+                                  int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream) {
+  const bool csr = X == nullptr;
+  if (csr == (indptr == nullptr)) return fail(TGB200_ERR_INVALID, "give exactly one of X (dense) and indptr (CSR)");
+  if (!labels || !sum_out || !sumsq_out) return fail(TGB200_ERR_INVALID, "null argument");
+  if (rows <= 0 || n_genes <= 0 || rows > INT32_MAX || n_genes > INT32_MAX - kGsSlab || (!csr && x_ld < n_genes))
+    return fail(TGB200_ERR_INVALID, "bad shape rows=%lld n_genes=%lld x_ld=%lld", (long long)rows, (long long)n_genes,
+                (long long)x_ld);
+  if (n_labels < 1) return fail(TGB200_ERR_INVALID, "n_labels=%d, must be at least 1", n_labels);
+  if (csr && (nnz < 0 || (nnz > 0 && (!indices || !data))))
+    return fail(TGB200_ERR_INVALID, "CSR with nnz=%lld needs indices and data", (long long)nnz);
+  if (block_rows < 0 || block_rows % kGsRange)
+    return fail(TGB200_ERR_INVALID, "block_rows=%lld is not a multiple of %d", (long long)block_rows, kGsRange);
+  // per range of kGsRange cells: its labelled rows stably sorted by label (offsets in the range), cut into runs of one label
+  const int64_t n_ranges = ceil_div(rows, kGsRange);
+  std::vector<int> perm_g, run_label, run_len, cnt(n_labels, 0), touched;
+  std::vector<int64_t> range_perm(n_ranges + 1, 0), range_run(n_ranges + 1, 0);
+  perm_g.reserve(rows);
+  for (int64_t c = 0; c < n_ranges; ++c) {
+    const int64_t i0 = c * kGsRange, i1 = std::min(rows, i0 + kGsRange);
+    touched.clear();
+    for (int64_t i = i0; i < i1; ++i) {
+      const int32_t l = labels[i];
+      if (l < -1 || l >= n_labels)
+        return fail(TGB200_ERR_INVALID, "label %d of row %lld is outside [-1, %d)", l, (long long)i, n_labels);
+      if (l >= 0 && cnt[l]++ == 0) touched.push_back(l);
+    }
+    std::sort(touched.begin(), touched.end());
+    const size_t base = perm_g.size();
+    int at = 0;
+    for (int l : touched) {                      // cnt[l] becomes the start of label l's run in the range
+      run_label.push_back(l);
+      run_len.push_back(cnt[l]);
+      const int n = cnt[l];
+      cnt[l] = at;
+      at += n;
+    }
+    perm_g.resize(base + at);
+    for (int64_t i = i0; i < i1; ++i)
+      if (labels[i] >= 0) perm_g[base + cnt[labels[i]]++] = (int)(i - i0);
+    for (int l : touched) cnt[l] = 0;
+    range_perm[c + 1] = (int64_t)perm_g.size();
+    range_run[c + 1] = (int64_t)run_label.size();
+  }
+
+  int n_sms = 0;
+  CKS(use_sm90_device(device, &n_sms));
+  cudaStream_t s = (cudaStream_t)stream;
+  // the row pointers are read on the host: every block's entry range is then known to lie inside [0, nnz)
+  std::vector<int64_t> ip;
+  if (csr) {
+    ip.resize(rows + 1);
+    CK(cudaMemcpyAsync(ip.data(), indptr, sizeof(int64_t) * (rows + 1), cudaMemcpyDefault, s));
+    CK(cudaStreamSynchronize(s));
+    if (ip[0] != 0 || ip[rows] != nnz)
+      return fail(TGB200_ERR_INVALID, "CSR indptr runs from %lld to %lld, expected 0 to nnz=%lld", (long long)ip[0],
+                  (long long)ip[rows], (long long)nnz);
+    for (int64_t r = 0; r < rows; ++r)
+      if (ip[r + 1] < ip[r]) return fail(TGB200_ERR_INVALID, "CSR indptr decreases at row %lld", (long long)r);
+  }
+  bool in_place = false;                         // dense X in this device's memory is read where it lives
+  if (!csr) {
+    cudaPointerAttributes at;
+    CK(cudaPointerGetAttributes(&at, X));
+    in_place = (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == device;
+  }
+  const int64_t T = n_labels, G = n_genes, ldx = round_up(n_genes, 4), cap = round_up(rows, kGsRange);
+  // the most of something over the blocks of B cells: of runs, of labelled rows, of stored entries
+  auto block_max = [&](int64_t B, auto&& f) {
+    int64_t m = 0;
+    for (int64_t r0 = 0; r0 < rows; r0 += B) m = std::max<int64_t>(m, f(r0, std::min(rows, r0 + B)));
+    return m;
+  };
+  auto runs_of = [&](int64_t r0, int64_t r1) { return range_run[ceil_div(r1, kGsRange)] - range_run[r0 / kGsRange]; };
+  auto perm_of = [&](int64_t r0, int64_t r1) { return range_perm[ceil_div(r1, kGsRange)] - range_perm[r0 / kGsRange]; };
+  auto nnz_of = [&](int64_t r0, int64_t r1) { return csr ? ip[r1] - ip[r0] : 0; };
+  auto table_ints = [&](int64_t B) {
+    return block_max(B, perm_of) + 2 * block_max(B, runs_of) + B / kGsRange + T + 3;
+  };
+  // outputs, the partials of one block's runs, and per block double-buffered: its tables and its X (dense staging or CSR)
+  auto need = [&](int64_t B) {
+    double b = 24.0 * T * G + 20.0 * block_max(B, runs_of) * G + 2 * 4.0 * table_ints(B);
+    if (csr) b += 2 * (8.0 * block_max(B, nnz_of) + 8.0 * (B + 1));
+    else if (!in_place) b += 2 * 4.0 * B * ldx;
+    return b;
+  };
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const double avail = (double)free_b - 256.0 * (1 << 20);    // headroom for the launches' own allocations
+  int64_t B = block_rows > 0 ? std::min(block_rows, cap)
+                             : std::min({cap, kGsMaxBlock, std::max<int64_t>(kGsRange, round_up(ceil_div(rows, kGsBlocks), kGsRange))});
+  while (block_rows == 0 && B > kGsRange && need(B) > avail) B -= kGsRange;
+  if (need(B) > avail)
+    return fail(TGB200_ERR_INVALID, "group statistics of %lld cells x %lld genes over %d labels need %.2f GiB on device %d in "
+                "blocks of %lld cells (%.2f GiB of it for the result); %.2f GiB are free", (long long)rows, (long long)G,
+                n_labels, need(B) / 1073741824.0, device, (long long)B, 24.0 * T * G / 1073741824.0,
+                free_b / 1073741824.0);
+
+  const int64_t n_blocks = ceil_div(rows, B), max_runs = block_max(B, runs_of);
+  DevBuf<double> sum, sq, psum, psq;
+  DevBuf<long long> cntd;
+  DevBuf<int> pcnt, tab[2], I[2], bad;
+  DevBuf<int64_t> P[2];
+  DevBuf<float> Xf[2], D[2];
+  CKS(sum.alloc((size_t)T * G, false)); CKS(sq.alloc((size_t)T * G, false)); CKS(cntd.alloc((size_t)T * G, false));
+  CKS(psum.alloc((size_t)std::max<int64_t>(max_runs, 1) * G, false));
+  CKS(psq.alloc((size_t)std::max<int64_t>(max_runs, 1) * G, false));
+  CKS(pcnt.alloc((size_t)std::max<int64_t>(max_runs, 1) * G, false));
+  CKS(bad.alloc(1, false));
+  const int64_t block_nnz = block_max(B, nnz_of);
+  for (int k = 0; k < 2; ++k) {
+    CKS(tab[k].alloc(table_ints(B), false));
+    if (csr) {
+      CKS(P[k].alloc(B + 1, false)); CKS(I[k].alloc(std::max<int64_t>(block_nnz, 1), false));
+      CKS(D[k].alloc(std::max<int64_t>(block_nnz, 1), false));
+    } else if (!in_place) {
+      CKS(Xf[k].alloc((size_t)B * ldx, false));
+    }
+  }
+  // zeroed on `stream` before cp.start is recorded, so they come before everything the copy stream orders after it
+  CK(cudaMemsetAsync(sum.p, 0, sizeof(double) * sum.n, s));
+  CK(cudaMemsetAsync(sq.p, 0, sizeof(double) * sq.n, s));
+  CK(cudaMemsetAsync(cntd.p, 0, sizeof(long long) * cntd.n, s));
+  CK(cudaMemsetAsync(bad.p, 0, sizeof(int), s));
+  CopyStream cp;
+  CK(cudaStreamCreateWithFlags(&cp.s, cudaStreamNonBlocking));
+  for (cudaEvent_t* e : {&cp.start, &cp.copied[0], &cp.copied[1], &cp.freed[0], &cp.freed[1]})
+    CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  CK(cudaEventRecord(cp.start, s));                            // inputs written on `stream` before the call
+  CK(cudaStreamWaitEvent(cp.s, cp.start, 0));
+
+  // block b's tables, one int array: perm | run_start | range_runs | lab_ptr | lab_runs (kept until the call returns)
+  struct Tab { std::vector<int> v; int np, nr, nrg; };
+  std::vector<Tab> tabs(n_blocks);
+  auto build_table = [&](int64_t b) {
+    Tab& t = tabs[b];
+    const int64_t c0 = b * B / kGsRange, c1 = std::min(n_ranges, c0 + B / kGsRange);
+    t.nrg = (int)(c1 - c0); t.np = (int)(range_perm[c1] - range_perm[c0]); t.nr = (int)(range_run[c1] - range_run[c0]);
+    t.v.assign((size_t)t.np + 2 * t.nr + t.nrg + T + 3, 0);
+    int* perm = t.v.data();
+    int* run_start = perm + t.np;
+    int* range_runs = run_start + t.nr + 1;
+    int* lab_ptr = range_runs + t.nrg + 1;
+    int* lab_runs = lab_ptr + T + 1;
+    for (int64_t c = c0; c < c1; ++c)
+      for (int64_t p = range_perm[c]; p < range_perm[c + 1]; ++p)
+        perm[p - range_perm[c0]] = perm_g[p] + (int)((c - c0) * kGsRange);
+    for (int k = 0; k < t.nr; ++k) run_start[k + 1] = run_start[k] + run_len[range_run[c0] + k];
+    for (int64_t c = c0; c <= c1; ++c) range_runs[c - c0] = (int)(range_run[c] - range_run[c0]);
+    for (int k = 0; k < t.nr; ++k) ++lab_ptr[run_label[range_run[c0] + k] + 1];
+    for (int64_t l = 0; l < T; ++l) lab_ptr[l + 1] += lab_ptr[l];
+    std::vector<int> next(lab_ptr, lab_ptr + T);
+    for (int k = 0; k < t.nr; ++k) lab_runs[next[run_label[range_run[c0] + k]]++] = k;      // range order within a label
+  };
+  // block b's tables and X into slot b % 2 on the copy stream, once the compute stream has consumed block b - 2 from it
+  auto stage = [&](int64_t b) -> int {
+    const int k = (int)(b & 1);
+    const int64_t r0 = b * B, nb = std::min(B, rows - r0);
+    build_table(b);
+    if (b >= 2) CK(cudaStreamWaitEvent(cp.s, cp.freed[k], 0));
+    CK(cudaMemcpyAsync(tab[k].p, tabs[b].v.data(), sizeof(int) * tabs[b].v.size(), cudaMemcpyHostToDevice, cp.s));
+    if (csr) {
+      const int64_t e0 = ip[r0], ne = ip[r0 + nb] - e0;
+      CK(cudaMemcpyAsync(P[k].p, ip.data() + r0, sizeof(int64_t) * (nb + 1), cudaMemcpyHostToDevice, cp.s));
+      if (ne > 0) {
+        CK(cudaMemcpyAsync(I[k].p, indices + e0, sizeof(int32_t) * ne, cudaMemcpyDefault, cp.s));
+        CK(cudaMemcpyAsync(D[k].p, data + e0, sizeof(float) * ne, cudaMemcpyDefault, cp.s));
+      }
+    } else if (!in_place) {
+      CK(cudaMemcpy2DAsync(Xf[k].p, sizeof(float) * ldx, X + r0 * x_ld, sizeof(float) * x_ld, sizeof(float) * n_genes, nb,
+                           cudaMemcpyDefault, cp.s));
+    }
+    CK(cudaEventRecord(cp.copied[k], cp.s));
+    return TGB200_OK;
+  };
+  CKS(stage(0));
+  const unsigned n_slabs = (unsigned)ceil_div(G, kGsSlab);
+  for (int64_t b = 0; b < n_blocks; ++b) {
+    const int k = (int)(b & 1);
+    const int64_t r0 = b * B, nb = std::min(B, rows - r0);
+    const Tab& t = tabs[b];
+    CK(cudaStreamWaitEvent(s, cp.copied[k], 0));
+    GsArgs a{};
+    a.n_genes = G;
+    a.perm = tab[k].p;
+    a.run_start = a.perm + t.np;
+    a.range_runs = a.run_start + t.nr + 1;
+    const int* lab_ptr = a.range_runs + t.nrg + 1;
+    a.psum = psum.p; a.psq = psq.p; a.pcnt = pcnt.p;
+    if (csr) {
+      a.indptr = P[k].p; a.indices = I[k].p; a.data = D[k].p;
+      k_gs_csr_check<<<(unsigned)ceil_div(nb * kWarp, kGsThreads), kGsThreads, 0, s>>>(P[k].p, I[k].p, (int)nb, G, bad.p);
+      CK(cudaGetLastError());
+    } else {
+      a.x = in_place ? X + r0 * x_ld : Xf[k].p;
+      a.ld = in_place ? x_ld : ldx;
+      a.vec = a.ld % 4 == 0 && reinterpret_cast<uintptr_t>(a.x) % 16 == 0;
+    }
+    if (t.nr > 0) {
+      const dim3 grid(n_slabs, (unsigned)t.nrg);
+      if (csr) k_group_stats<true><<<grid, kGsThreads, 0, s>>>(a);
+      else k_group_stats<false><<<grid, kGsThreads, 0, s>>>(a);
+      CK(cudaGetLastError());
+      const dim3 fgrid((unsigned)ceil_div(G, kGsThreads), (unsigned)std::min<int64_t>(T, 65535));
+      k_group_stats_fold<<<fgrid, kGsThreads, 0, s>>>(psum.p, psq.p, pcnt.p, lab_ptr, lab_ptr + T + 1, n_labels, G, sum.p,
+                                                      sq.p, cntd.p);
+      CK(cudaGetLastError());
+    }
+    CK(cudaEventRecord(cp.freed[k], s));
+    if (b + 1 < n_blocks) CKS(stage(b + 1));                   // after block b's launches: its copies run under them
+  }
+  int bad_host = 0;
+  CK(cudaMemcpyAsync(&bad_host, bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad_host)
+    return fail(TGB200_ERR_INVALID, "a CSR column index is outside [0, %lld) or not strictly increasing within its row",
+                (long long)n_genes);
+  CK(cudaMemcpyAsync(sum_out, sum.p, sizeof(double) * T * G, cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(sumsq_out, sq.p, sizeof(double) * T * G, cudaMemcpyDefault, s));
+  if (nnz_out) CK(cudaMemcpyAsync(nnz_out, cntd.p, sizeof(int64_t) * T * G, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
 }
