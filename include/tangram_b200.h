@@ -425,6 +425,20 @@ TGB200_API int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* i
                                   const int32_t* labels_host, int32_t n_labels, double* sum_out, double* sumsq_out,
                                   int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream);
 
+/* tgb200_group_stats of y = expm1(scale * (double)x) instead of x (scanpy's highly_variable_genes, flavor="seurat":
+ * the statistics of the un-logged expression; scale = ln(base) for log1p data with uns["log1p"]["base"], else 1).
+ *   sum_out, sumsq_out   the fp64 sum of y and of y * y (y * y added with one fused multiply-add, whatever -fmad says)
+ *   nnz_out              entries with x != 0, of the untransformed x (NaN counts), as tgb200_group_stats
+ * y is computed in fp64 for every element, absent CSR entries included (expm1(+-0) = +-0 adds nothing), with the same
+ * order of additions, staging, memory and checks as tgb200_group_stats: dense and CSR, host and device pointers, any
+ * block_rows and re-runs give identical bits.  fp64 expm1 stays finite where scanpy's float32 expm1 overflows (x above
+ * about 88.7).  TGB200_ERR_INVALID also for a scale that is not finite. */
+TGB200_API int tgb200_group_stats_expm1(const float* X, int64_t x_ld, const int64_t* indptr, const int32_t* indices,
+                                        const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
+                                        const int32_t* labels_host, int32_t n_labels, double* sum_out, double* sumsq_out,
+                                        int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream,
+                                        double scale);
+
 /* Checkpoint / resume (the reference stubs this: `raise NotImplemented`, :151-153).
  * Any pointer may be NULL to skip it.  M, m, v: n_cells x n_voxels f32, host or device. */
 TGB200_API int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream);

@@ -8,6 +8,7 @@
     cv_dict = tg.cross_val(ad_sc, ad_sp, cluster_label="cell_type", cv_mode="10fold")   # gene cross-validation
     metrics = tg.train_multiple_Mapper(config, data)     # the tuner's trial: five run-to-run agreement metrics
     tg.rank_genes_groups(ad_sc, groupby="cell_type")     # marker genes per group on the GPU; tg.ctg(ad_sc, "cell_type")
+    tg.highly_variable_genes(ad_sc, n_top_genes=4000)    # highly variable genes on the GPU; tg.hvg(ad_sc)
 
 One process per GPU (process_group=pg, cells and constrained mode): every rank passes the same AnnDatas and gets its
 block of the mapping; project_genes, project_cell_annotations, cell_type_mapping and count_cell_annotations then take that
@@ -28,6 +29,6 @@ from .utils import (  # noqa: F401
 from . import mapping_parameter_tuning  # noqa: F401
 from .mapping_parameter_tuning import train_multiple_Mapper  # noqa: F401
 from .adata import MiniAnnData  # noqa: F401
-from .gene_selection import rank_genes_groups, ctg  # noqa: F401
+from .gene_selection import rank_genes_groups, ctg, highly_variable_genes, hvg  # noqa: F401
 
 __version__ = "0.2.0"

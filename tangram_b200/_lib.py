@@ -118,6 +118,9 @@ SIGNATURES = {
                                           _P, _P, _P, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int64, ctypes.c_int32, _P]),
     "tgb200_group_stats": (ctypes.c_int, [_P, ctypes.c_int64, _P, _P, _P, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                           _P, ctypes.c_int32, _P, _P, _P, ctypes.c_int64, ctypes.c_int32, _P]),
+    "tgb200_group_stats_expm1": (ctypes.c_int, [_P, ctypes.c_int64, _P, _P, _P, ctypes.c_int64, ctypes.c_int64,
+                                                ctypes.c_int64, _P, ctypes.c_int32, _P, _P, _P, ctypes.c_int64,
+                                                ctypes.c_int32, _P, ctypes.c_double]),
     "tgb200_get_state":(ctypes.c_int, [_P, _P, _P, _P, _I64, _P]),
     "tgb200_set_state": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int64, _P]),
     "tgb200_plan_state": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_uint64, ctypes.POINTER(StatePlan)]),

@@ -1,11 +1,15 @@
-// Per-label column statistics of an expression matrix (the basic statistics of scanpy's rank_genes_groups): for every
-// label t and gene k the fp64 sum of x, the fp64 sum of (double)x * (double)x and the count of x != 0 over the rows
-// labelled t, in one streaming pass that reads every dense element or stored CSR entry once.
+// Per-label column statistics of an expression matrix (the basic statistics of scanpy's rank_genes_groups and
+// highly_variable_genes): for every label t and gene k the fp64 sum of y, the fp64 sum of y * y and the count of x != 0
+// over the rows labelled t, in one streaming pass that reads every dense element or stored CSR entry once.  y is the
+// element's value under a compile-time transform: GsValue::kIdentity, y = (double)x (rank_genes_groups), or
+// GsValue::kExpm1, y = expm1(scale * (double)x) in fp64 (highly_variable_genes' seurat flavor, which undoes log1p).
+// The count is always of the untransformed x (NaN counts).
 //
 // Summation order (part of the contract, so the bits do not depend on how the data arrives): each aligned range of
 // kGsRange cells forms one chain per label -- that range's rows of the label, added in row order, starting from 0.0 --
 // and the chains are added in range order, starting from 0.0.  Absent CSR entries and explicit zeros both add +0.0, so
-// dense and CSR input of the same matrix give the same bits; so do host and device pointers and any block size.
+// dense and CSR input of the same matrix give the same bits; so do host and device pointers and any block size.  Under
+// kExpm1 an absent entry becomes expm1(scale * 0.0) = +-0.0, which adds nothing either, so the same holds.
 //
 // Work split: the host stable-sorts the labelled rows of each range by label (perm) and cuts them into runs of one label.
 // k_group_stats: one CTA per (range, slab of kGsSlab genes); each thread owns four genes and walks the range's runs in
@@ -23,6 +27,8 @@ constexpr int kGsSlab = 4 * kGsThreads;        // genes per CTA: four per thread
 constexpr int kGsRange = 2048;                 // cells per summation chain
 constexpr int kGsRows = kGsThreads / kWarp;    // rows per batch: one CSR row per warp
 
+enum class GsValue { kIdentity, kExpm1 };
+
 struct GsArgs {
   const float* x;                              // dense: row i of the block at x + i * ld
   long long ld;
@@ -34,6 +40,7 @@ struct GsArgs {
   const int* perm;                             // labelled rows of the block (offsets in it), each range's stably by label
   const int* run_start;                        // [n_runs + 1]: run k covers perm[run_start[k] .. run_start[k + 1])
   const int* range_runs;                       // [n_ranges + 1]: range r holds runs range_runs[r] .. range_runs[r + 1]
+  double scale;                                // kExpm1: y = expm1(scale * x)
   double* psum;                                // [n_runs][n_genes] per-run partials
   double* psq;
   int* pcnt;
@@ -60,7 +67,7 @@ __device__ __forceinline__ void gs_scatter_row(const GsArgs& a, int row, int s0,
   }
 }
 
-template <bool kCsr>
+template <bool kCsr, GsValue kValue>
 __global__ void __launch_bounds__(kGsThreads) k_group_stats(GsArgs a) {
   __shared__ __align__(16) float tile[kCsr ? kGsRows : 1][kCsr ? kGsSlab : 4];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -110,9 +117,9 @@ __global__ void __launch_bounds__(kGsThreads) k_group_stats(GsArgs a) {
       if (u >= nb) break;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const double d = (double)v[u][e];
-        s[e] += d;
-        q[e] += d * d;                                                    // exact in fp64: fused or not, the same bits
+        const double y = kValue == GsValue::kExpm1 ? expm1(a.scale * (double)v[u][e]) : (double)v[u][e];
+        s[e] += y;
+        q[e] = __fma_rn(y, y, q[e]);    // fused whatever -fmad says; for the identity y * y is exact, so unfused alike
         n[e] += v[u][e] != 0.f;                                           // NaN counts
       }
       if (b0 + u + 1 == next) {                                           // the run ends: flush its partial

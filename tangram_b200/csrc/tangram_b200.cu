@@ -2758,10 +2758,11 @@ constexpr int64_t kGsBlocks = 8;          // default: about this many blocks, so
 constexpr int64_t kGsMaxBlock = 32 * kGsRange;   // 32 ranges x the slabs fill the device; larger blocks only add partials
 }  // namespace
 
-extern "C" int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* indptr, const int32_t* indices,
-                                  const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
-                                  const int32_t* labels, int32_t n_labels, double* sum_out, double* sumsq_out,
-                                  int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream) {
+// The pass behind tgb200_group_stats (value = kIdentity) and tgb200_group_stats_expm1 (kExpm1, y = expm1(scale * x)).
+static int group_stats_pass(GsValue value, double scale, const float* X, int64_t x_ld, const int64_t* indptr,
+                            const int32_t* indices, const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
+                            const int32_t* labels, int32_t n_labels, double* sum_out, double* sumsq_out,
+                            int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream) {
   const bool csr = X == nullptr;
   if (csr == (indptr == nullptr)) return fail(TGB200_ERR_INVALID, "give exactly one of X (dense) and indptr (CSR)");
   if (!labels || !sum_out || !sumsq_out) return fail(TGB200_ERR_INVALID, "null argument");
@@ -2949,6 +2950,7 @@ extern "C" int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* i
     a.range_runs = a.run_start + t.nr + 1;
     const int* lab_ptr = a.range_runs + t.nrg + 1;
     a.psum = psum.p; a.psq = psq.p; a.pcnt = pcnt.p;
+    a.scale = scale;
     if (csr) {
       a.indptr = P[k].p; a.indices = I[k].p; a.data = D[k].p;
       k_gs_csr_check<<<(unsigned)ceil_div(nb * kWarp, kGsThreads), kGsThreads, 0, s>>>(P[k].p, I[k].p, (int)nb, G, bad.p);
@@ -2960,8 +2962,13 @@ extern "C" int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* i
     }
     if (t.nr > 0) {
       const dim3 grid(n_slabs, (unsigned)t.nrg);
-      if (csr) k_group_stats<true><<<grid, kGsThreads, 0, s>>>(a);
-      else k_group_stats<false><<<grid, kGsThreads, 0, s>>>(a);
+      if (value == GsValue::kExpm1) {
+        if (csr) k_group_stats<true, GsValue::kExpm1><<<grid, kGsThreads, 0, s>>>(a);
+        else k_group_stats<false, GsValue::kExpm1><<<grid, kGsThreads, 0, s>>>(a);
+      } else {
+        if (csr) k_group_stats<true, GsValue::kIdentity><<<grid, kGsThreads, 0, s>>>(a);
+        else k_group_stats<false, GsValue::kIdentity><<<grid, kGsThreads, 0, s>>>(a);
+      }
       CK(cudaGetLastError());
       const dim3 fgrid((unsigned)ceil_div(G, kGsThreads), (unsigned)std::min<int64_t>(T, 65535));
       k_group_stats_fold<<<fgrid, kGsThreads, 0, s>>>(psum.p, psq.p, pcnt.p, lab_ptr, lab_ptr + T + 1, n_labels, G, sum.p,
@@ -2982,4 +2989,22 @@ extern "C" int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* i
   if (nnz_out) CK(cudaMemcpyAsync(nnz_out, cntd.p, sizeof(int64_t) * T * G, cudaMemcpyDefault, s));
   CK(cudaStreamSynchronize(s));
   return TGB200_OK;
+}
+
+extern "C" int tgb200_group_stats(const float* X, int64_t x_ld, const int64_t* indptr, const int32_t* indices,
+                                  const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
+                                  const int32_t* labels, int32_t n_labels, double* sum_out, double* sumsq_out,
+                                  int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream) {
+  return group_stats_pass(GsValue::kIdentity, 1.0, X, x_ld, indptr, indices, data, nnz, rows, n_genes, labels, n_labels,
+                          sum_out, sumsq_out, nnz_out, block_rows, device, stream);
+}
+
+extern "C" int tgb200_group_stats_expm1(const float* X, int64_t x_ld, const int64_t* indptr, const int32_t* indices,
+                                        const float* data, int64_t nnz, int64_t rows, int64_t n_genes,
+                                        const int32_t* labels, int32_t n_labels, double* sum_out, double* sumsq_out,
+                                        int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream,
+                                        double scale) {
+  if (!std::isfinite(scale)) return fail(TGB200_ERR_INVALID, "scale=%g is not finite", scale);
+  return group_stats_pass(GsValue::kExpm1, scale, X, x_ld, indptr, indices, data, nnz, rows, n_genes, labels, n_labels,
+                          sum_out, sumsq_out, nnz_out, block_rows, device, stream);
 }
