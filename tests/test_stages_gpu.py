@@ -37,6 +37,9 @@ pytestmark = pytest.mark.gpu
 U = 2.0 ** -24          # fp32 unit roundoff
 UB = 2.0 ** -8          # bf16 unit roundoff
 UM = 2.0 ** -21         # MUFU ex2 / rcp / sqrt .approx.ftz: <= 2^-22.5 .. 2^-22 relative, doubled
+TINY = 2.0 ** -126      # fp32's smallest normal: an .ftz MUFU result whose exact value is below it may be 0
+SUB = 2.0 ** -149       # fp32's smallest subnormal: an IEEE rounding into the subnormal range is off by <= SUB / 2
+UBS = 2.0 ** -134       # half of bf16's smallest subnormal (2^-133): a bf16 rounding of a value below 2^-126 is off by <= it
 B1, B2, EPS, LR = 0.9, 0.999, 1e-8, 0.1
 ALL_TERMS = dict(lambda_g2=0.5, lambda_r=1e-3, lambda_l1=1e-7, lambda_l2=1e-7, lambda_neighborhood_g1=0.96,
                  lambda_ct_islands=0.17, lambda_getis_ord=0.71)
@@ -146,10 +149,13 @@ def _x3_forward_consts(r):
 
 
 # ---------------------------------------------------------------------------------------------------------------- row pass
-def _check_row_pass(r, M, P_dev, stats, mode):
+def _check_row_pass(r, M, P_dev, stats, mode, floor=0.0):
     """P = expf(M - mx) (1 / z) (IEEE expf <= 2 ulp, z summed in fp32 over V elements, one product), mx exact:
          |log z - ref| <= (V + 4) u,   |P - ref| <= (V + 12 + |M - mx|) u P   (+ u P when P is split into three planes)
-    rel-Fro and bias: the row sums' error is a per-row constant, sqrt-class in practice: <= 16 u."""
+    rel-Fro and bias: the row sums' error is a per-row constant, sqrt-class in practice: <= 16 u.
+    floor: P may reach fp32's subnormal range, where expf's 2 ulp and the product's half ulp are absolute (3 SUB, plus
+    2^-134 when P is held in three bf16 planes, whose lowest bits fall below bf16's subnormals): the elementwise bound
+    gets that absolute floor, and the statistics run over P >= 2^-126."""
     torch = _torch()
     V = r.V
     Mv = M[:, :V]
@@ -160,9 +166,13 @@ def _check_row_pass(r, M, P_dev, stats, mode):
     _check(f"{mode} 1 / z", stats[:, 1], torch.exp(mx - lse), torch.exp(mx - lse), (V + 4) * U, 16 * U, 16 * U)
     Pref = torch.softmax(Mv, dim=1)
     c = (V + 13 + (Mv - mx[:, None]).abs()) * U
-    err_ok = (P_dev[:, :V] - Pref).abs() <= c * Pref
+    err_ok = (P_dev[:, :V] - Pref).abs() <= c * Pref + floor
     assert bool(err_ok.all()), f"{mode} P: {int((~err_ok).sum())} elements off"
-    _check(f"{mode} P (stat)", P_dev[:, :V], Pref, Pref, 1.0, 16 * U, 16 * U)
+    if floor:
+        keep = Pref >= TINY
+        _check(f"{mode} P (stat, P >= 2^-126)", P_dev[:, :V][keep], Pref[keep], Pref[keep], 1.0, 16 * U, 16 * U)
+    else:
+        _check(f"{mode} P (stat)", P_dev[:, :V], Pref, Pref, 1.0, 16 * U, 16 * U)
     assert torch.count_nonzero(P_dev[:, V:]) == 0, "pad columns of P"
     if r.lam.get("lambda_r"):
         logP = torch.log_softmax(Mv, dim=1)
@@ -291,9 +301,10 @@ def _check_loss_stage(r, Y_dev, dY_dev, hist, M, mode):
 
 
 # -------------------------------------------------------------------------------------------------------------- the update
-def _adam64(M, m, v, g, dg, t, lr=LR):
+def _adam64(M, m, v, g, dg, t, lr=LR, floor=0.0):
     """torch.optim.Adam's step in float64 from (M, m, v, g) with |g error| <= dg -> (M', m', v') and first-order bounds
-    of the fp32 update on them (one rounding per operation, six operations: 8 u relative slack)."""
+    of the fp32 update on them (one rounding per operation, six operations: 8 u relative slack).  floor: an absolute
+    error of m' and v' on top (their roundings in fp32's subnormal range), carried into M' through m' / denom."""
     torch = _torch()
     bc1, bc2 = 1 - B1 ** t, 1 - B2 ** t
     m1 = m + (g - m) * (1 - B1)
@@ -301,8 +312,8 @@ def _adam64(M, m, v, g, dg, t, lr=LR):
     den = v1.sqrt() / bc2 ** 0.5 + EPS
     step = (lr / bc1) * m1 / den
     M1 = M - step
-    dm = (1 - B1) * dg + 4 * U * (m.abs() + m1.abs() + g.abs())
-    dv = (1 - B2) * (2 * g.abs() * dg + dg * dg) + 4 * U * (v1 + v * B2)
+    dm = (1 - B1) * dg + 4 * U * (m.abs() + m1.abs() + g.abs()) + floor
+    dv = (1 - B2) * (2 * g.abs() * dg + dg * dg) + 4 * U * (v1 + v * B2) + floor
     dden = dv / (2 * torch.clamp(v1.sqrt(), min=1e-30) * bc2 ** 0.5) + 4 * U * den
     dM = (lr / bc1) * (dm / den + m1.abs() * dden / (den * den)) + 8 * U * (step.abs() + M1.abs())
     return M1, m1, v1, dM, dm, dv
@@ -323,15 +334,16 @@ def _grad_terms(r, M, P, base, lse, h):
     return g
 
 
-def _check_update(r, pre, post, g, dg, t, mode, m_bf16=False, late=False):
+def _check_update(r, pre, post, g, dg, t, mode, m_bf16=False, late=False, tiny=False):
     """M, m, v after the step, pad columns included (they stay exactly zero).  late: the step may be a small fraction of
     an ulp of M (late in training), and the rounding of M' itself, up to u |M'| and one-sided where the step is below half
-    an ulp, is added to the step's rel-Fro and bias bounds."""
+    an ulp, is added to the step's rel-Fro and bias bounds.  tiny: g, m and v may be subnormal; each of the four fp32
+    operations that form m' or v' may then be off by SUB / 2 absolute (floor 4 SUB)."""
     torch = _torch()
     V = r.V
     M0, m0, v0 = (x[:, :V] for x in pre)
     M1, m1, v1 = (x for x in post)
-    Mr, mr, vr, dM, dm, dv = _adam64(M0, m0, v0, g, dg, t)
+    Mr, mr, vr, dM, dm, dv = _adam64(M0, m0, v0, g, dg, t, floor=4 * SUB if tiny else 0.0)
     for what, got, ref, bound in (("v", v1[:, :V], vr, dv), ("M", M1[:, :V], Mr, dM)):
         bad = (got - ref).abs() > bound
         assert not bool(bad.any()), f"{mode} update {what}: {int(bad.sum())} elements off, first {torch.nonzero(bad)[0].tolist()}"
@@ -531,19 +543,25 @@ def _fp32_forward_consts(r):
     return (2 * chain + r.splits + r.V + 32) * U, 4 * np.sqrt(chain) * U + (r.splits + 16) * U, 20 * U
 
 
-def _check_backward_fp32(r, pre, t, stats, Pf, dY, mode):
+def _check_backward_fp32(r, pre, t, stats, Pf, dY, mode, late=False, tiny=False):
     """fp32 backward from the device's dY_ext: the row-dot, and the fused update from the pre-step state `pre` at step
-    count t (EpiAdam never stores dP: dP is recomputed in float64 from the device's S_ext and dY)."""
+    count t (EpiAdam never stores dP: dP is recomputed in float64 from the device's S_ext and dY).  late, tiny: as in
+    _check_update; tiny adds SUB / 2 to g (its product P (dP - r) rounded into the subnormal range), and holds the row-dot's
+    bias to its elementwise bound: at a peaked state the terms of every voxel but the peak lie below half an ulp of the
+    running sum and are dropped, all on one side."""
     V = r.V
     dPref = r.S @ dY.t()
     scale = r.S.abs() @ dY.abs().t()
     rdot = r.buf("rdot")
     rref = (Pf[:, :V] * dPref).sum(dim=1)
     rscale = (Pf[:, :V] * scale).sum(dim=1)
-    _check(f"{mode} row-dot", rdot, rref, rscale, (2 * (r.Ke + V) + 8) * U, 4 * np.sqrt(r.Ke + V) * U, 4 * U)
+    ce = (2 * (r.Ke + V) + 8) * U
+    _check(f"{mode} row-dot", rdot, rref, rscale, ce, 4 * np.sqrt(r.Ke + V) * U, ce if tiny else 4 * U)
     g = _grad_terms(r, pre[0][:, :V], Pf[:, :V], dPref - rdot[:, None], stats[:, 0] + stats[:, 2], stats[:, 3])
     dg = Pf[:, :V] * (2 * r.Ke + 8) * U * scale + 8 * U * (g.abs() + Pf[:, :V] * (dPref.abs() + rdot.abs()[:, None] + 1.0))
-    _check_update(r, pre, _state(r), g, dg, t + 1, mode)
+    if tiny:
+        dg = dg + SUB
+    _check_update(r, pre, _state(r), g, dg, t + 1, mode, late=late, tiny=tiny)
 
 
 # ------------------------------------------------------------------------------------------------------------------ bf16
@@ -551,12 +569,15 @@ def _bf16_round(x):
     return x.float().to(_torch().bfloat16).double()
 
 
-def _check_carry(r, M, mode):
+def _check_carry(r, M, mode, tiny=False):
     """After step_begin: lseT = lseA + log z~ against float64 logsumexp(M); P~ inv_zt against float64 softmax(M); h.
     z~ sums the fp32 values of P~ (before their bf16 rounding) over V, ex2.approx.ftz on an fma'd argument:
         |lseT - ref| <= (V + 8) u + UM (1 + |lse|),   |P~ inv_zt - P| <= (u_b + (V + 8) u + UM (2 + |M| + |lse|)) P
     P~ carries one bf16 rounding each: rel-Fro <= u_b, |bias| <= u_b / 16.  h = px / z~ - lseT cancels:
-        |h - ref| <= ((V + 8) u + UM (2 + |lse|)) (sum_j P |M| + |lse|)."""
+        |h - ref| <= ((V + 8) u + UM (2 + |lse|)) (sum_j P |M| + |lse|).
+    tiny: the ex2.approx.ftz that wrote P~ returns 0 where its exact value is below 2^-126, so P~ inv_zt may be off by
+    2^-126 inv_zt absolute, and the statistics run over the P~ that are not in that range.  A peaked row can have lse
+    near 0, so h's scale also takes the absolute error UM of log z~ itself (+ 1, as lseT's bound does)."""
     torch = _torch()
     V = r.V
     Mv = M[:, :V]
@@ -569,14 +590,18 @@ def _check_carry(r, M, mode):
     izt = r.buf("inv_zt")
     P = Pt[:, :V] * izt[:, None]
     c = UB + (V + 8) * U + UM * (2 + Mv.abs() + lse.abs()[:, None])
-    bad = (P - Pref).abs() > c * Pref
+    bad = (P - Pref).abs() > c * Pref + (TINY * izt[:, None] if tiny else 0.0)
     assert not bool(bad.any()), f"{mode} P~ / z~: {int(bad.sum())} elements off"
-    _check(f"{mode} P~ / z~ (stat)", P, Pref, Pref, 1e30, UB, UB / 16)
+    if tiny:
+        keep = Pref >= TINY * izt[:, None]
+        _check(f"{mode} P~ / z~ (stat, P~ >= 2^-126)", P[keep], Pref[keep], Pref[keep], 1e30, UB, UB / 16)
+    else:
+        _check(f"{mode} P~ / z~ (stat)", P, Pref, Pref, 1e30, UB, UB / 16)
     assert torch.count_nonzero(Pt[:, V:]) == 0, "pad columns of P~"
     stats = r.buf("stats", 4)
     if r.lam.get("lambda_r"):
         h = (Pref * torch.log_softmax(Mv, dim=1)).sum(dim=1)
-        scale = (Pref * Mv.abs()).sum(dim=1) + lse.abs()
+        scale = (Pref * Mv.abs()).sum(dim=1) + lse.abs() + (1.0 if tiny else 0.0)
         ce = (V + 8) * U + UM * (2 + lse.abs().max().item())
         _check(f"{mode} h", stats[:, 3], h, scale, ce, ce, ce)
     return Pref, lse, izt
@@ -626,9 +651,11 @@ def test_bf16_stages(N, V, K, lam_r):
         _check_bf16_update_step(r, pre, t, lseT_now, f"bf16[{step}]")
 
 
-def _check_bf16_update_step(r, pre, t, lseT_now, mode, late=False):
+def _check_bf16_update_step(r, pre, t, lseT_now, mode, late=False, tiny=False):
     """The bf16 streaming update from the device's dq, rowc = (lse, r', h) and the pre-step state `pre` at step count t
-    (lseT_now: lseT after step_begin), then the P~ and z~ it left for the next forward."""
+    (lseT_now: lseT after step_begin), then the P~ and z~ it left for the next forward.  tiny: the update's
+    ex2.approx.ftz returns 0 for a P below 2^-126, so g may be off by 2^-126 times what P multiplies, and the P~ it writes
+    by 2^-126; m, v as in _check_update_bf16."""
     torch = _torch()
     V = r.V
     dq = r.nv("dq")[:, :V]
@@ -639,15 +666,20 @@ def _check_bf16_update_step(r, pre, t, lseT_now, mode, late=False):
     g = _grad_terms(r, Mv, P, dq - rowc[:, 1:2], rowc[:, 0], rowc[:, 2])
     dg = (UM * (4 + 2 * Mv.abs() + 2 * rowc[:, 0:1].abs()) + 4 * U) * g.abs() + 4 * U * P * (dq.abs() + rowc[:, 1:2].abs())
     dg = dg + (r.lam.get("lambda_r", 0.0) * P * 8 * U * (Mv.abs() + rowc[:, 0:1].abs() + rowc[:, 2:3].abs()))
+    if tiny:
+        base = (dq - rowc[:, 1:2]).abs()
+        if r.lam.get("lambda_r"):
+            base = base + r.lam["lambda_r"] * ((Mv - rowc[:, 0:1]) - rowc[:, 2:3]).abs()
+        dg = dg + TINY * base + SUB
     post = _state(r)
-    _check_update_bf16(r, pre, post, g, dg, t + 1, mode, late=late)
+    _check_update_bf16(r, pre, post, g, dg, t + 1, mode, late=late, tiny=tiny)
     # what the update left for the next forward: P~ = bf16(exp(Mnew - lse)), z~ = sum of the unrounded values
     Mn = post[0][:, :V]
     lseA = r.buf("lseA")
     assert torch.equal(lseA, lseT_now), "after step_end lseA is the offset the new P~ was written with"
     Pt_ref = torch.exp(Mn - lseA[:, None])
     Pt = r.nv("Pb")
-    bad = (Pt[:, :V] - Pt_ref).abs() > (UB + UM * (2 + Mn.abs() + lseA.abs()[:, None])) * Pt_ref
+    bad = (Pt[:, :V] - Pt_ref).abs() > (UB + UM * (2 + Mn.abs() + lseA.abs()[:, None])) * Pt_ref + (TINY if tiny else 0.0)
     assert not bool(bad.any()), f"{mode} P~ after the update: {int(bad.sum())} elements off"
     assert torch.count_nonzero(Pt[:, V:]) == 0, "pad columns of P~"
     _check(f"{mode} z~", r.buf("zsum"), Pt_ref.sum(dim=1), Pt_ref.sum(dim=1),
@@ -693,25 +725,51 @@ def test_bf16_run_prefetches_the_same_forward(N, V, K, lam_r):
     assert torch.count_nonzero(a.nv("Pb")[:, V:]) == 0, "pad columns of P~"
 
 
-def _check_update_bf16(r, pre, post, g, dg, t, mode, late=False):
-    """bf16 update bound: the MUFU rcp / sqrt add 2 UM relative to the step.  late: as in _check_update."""
+def _check_update_bf16(r, pre, post, g, dg, t, mode, late=False, tiny=False):
+    """bf16 update bound: the MUFU rcp / sqrt add 2 UM relative to the step.  late: as in _check_update.
+    tiny: m and v may be subnormal: m', v' get the floor of _check_update, m's bf16 rounding is off by up to 2^-134
+    absolute there.  And m's rounding is checked against the kernel's own fp32 m' = fmaf(g - m, 1 - b1, m), emulated from
+    the float64 g rounded to fp32: the stored bf16 m' must be the round to nearest of a value within g's error bound
+    (1 - b1) dg of it (exactly its round to nearest where that cannot cross a rounding midpoint), and the signed mean of its rounding error must be that of the emulation's
+    within u_b / 16.  On a trained state the signed mean against float64 itself is not a property of the kernel: where g
+    is small against m, m' ~ b1 m with m on the bf16 grid, and round to nearest of those values has a mean of its own."""
     torch = _torch()
     V = r.V
     M0, m0, v0 = (x[:, :V] for x in pre)
     M1, m1, v1 = post
-    Mr, mr, vr, dM, dm, dv = _adam64(M0, m0, v0, g, dg, t)
+    Mr, mr, vr, dM, dm, dv = _adam64(M0, m0, v0, g, dg, t, floor=4 * SUB if tiny else 0.0)
     dM = dM + 4 * UM * (M0 - Mr).abs()
     dv = dv + 4 * UM * vr
     for what, got, ref, bound in (("v", v1[:, :V], vr, dv), ("M", M1[:, :V], Mr, dM)):
         bad = (got - ref).abs() > bound
         assert not bool(bad.any()), f"{mode} update {what}: {int(bad.sum())} elements off, first {torch.nonzero(bad)[0].tolist()}"
-    bound = UB * mr.abs() + dm * (1 + UB)
+    bound = UB * mr.abs() + dm * (1 + UB) + (UBS if tiny else 0.0)
     bad = (m1[:, :V] - mr).abs() > bound
     assert not bool(bad.any()), f"{mode} update m: {int(bad.sum())} elements off"
     live = mr.abs() > 0
-    bias = float(((m1[:, :V] - mr)[live] / mr[live].abs() * torch.sign(mr[live])).mean())
-    print(f"[stage] {mode} update m (bf16 round to nearest) bias {bias:.3g} (bound {UB / 16:.3g})")
-    assert abs(bias) <= UB / 16, f"{mode} update m: rounding bias {bias:.3g}"
+    if tiny:
+        mb = m1[:, :V]
+        m32 = ((g.float() - m0.float()).double() * float(np.float32(1 - B1)) + m0).float().double()   # fmaf: one rounding
+        me = m32.float().to(torch.bfloat16).double()
+        diff = mb != me
+        # g's error (and m''s own fp32 rounding) may move the value the kernel rounds by tau; its bf16 value is then
+        # within half an ulp of that
+        tau = (1 - B1) * dg + 4 * U * (m32.abs() + m0.abs()) + 4 * SUB
+        far = diff & ((mb - m32).abs() > tau + UB * (m32.abs() + tau) + UBS)
+        fl = (dm - 4 * U * (m0.abs() + mr.abs() + g.abs())) * (1 + UB) + UBS
+        live = live & (UB * mr.abs() > fl)
+        rel = lambda x: float(((x - mr)[live] / mr[live].abs() * torch.sign(mr[live])).mean())  # noqa: E731
+        bias, bias_e = rel(mb), rel(me)
+        print(f"[stage] {mode} update m: {int(diff.sum())} of {diff.numel()} differ from round to nearest of the fp32 m' "
+              f"({int(far.sum())} beyond g's error); bias against float64 {bias:.3g}, of that round to nearest {bias_e:.3g}, "
+              f"difference {bias - bias_e:.3g} (bound {UB / 16:.3g})")
+        assert not bool(far.any()), (f"{mode} update m: {int(far.sum())} elements are not the round to nearest of the "
+                                     f"fp32 m', first {torch.nonzero(far)[0].tolist()}")
+        assert abs(bias - bias_e) <= UB / 16, f"{mode} update m: rounding bias {bias:.3g} against {bias_e:.3g} of round to nearest"
+    else:
+        bias = float(((m1[:, :V] - mr)[live] / mr[live].abs() * torch.sign(mr[live])).mean())
+        print(f"[stage] {mode} update m (bf16 round to nearest) bias {bias:.3g} (bound {UB / 16:.3g})")
+        assert abs(bias) <= UB / 16, f"{mode} update m: rounding bias {bias:.3g}"
     for x, name in ((M1, "M"), (m1, "m"), (v1, "v")):
         assert torch.count_nonzero(x[:, V:]) == 0, f"{mode}: pad columns of {name}"
     stepref = M0 - Mr
