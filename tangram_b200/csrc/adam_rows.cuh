@@ -67,11 +67,7 @@ __device__ __forceinline__ uint4 pack_bf8(const float (&f)[8]) {
 #define TGB_ADAM_MAXNREG 96     // two 8-column groups of M, m, v, dq in flight per lane without spills; 2 CTAs of 256 threads per SM
 #endif
 template <bool PLAIN>
-__global__ void __maxnreg__(TGB_ADAM_MAXNREG)
-k_adam_rows(const AdamRowsArgs p) {
-  const int lane = threadIdx.x & 31;
-  const int row = p.row0 + blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (row >= p.row1) return;
+__device__ __forceinline__ void adam_row(const AdamRowsArgs& p, int row, int lane) {
   const RowConst rc = p.rowc[row];
   const float lse_l2e = rc.lse * 1.4426950408889634f;
   const size_t base = (size_t)row * p.ld;
@@ -172,6 +168,23 @@ k_adam_rows(const AdamRowsArgs p) {
     if (p.l1sum) { p.l1sum[row] = l1s; p.l2sum[row] = l2s; }
   }
 }
+template <bool PLAIN>
+__global__ void __maxnreg__(TGB_ADAM_MAXNREG)
+k_adam_rows(const AdamRowsArgs p) {
+  const int row = p.row0 + blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row < p.row1) adam_row<PLAIN>(p, row, threadIdx.x & 31);
+}
+#ifdef TGB_OVERLAP_PROBE
+// Debug build only (tools/overlap_probe.py): the same rows, warps and arithmetic as a persistent grid of 512-thread CTAs.
+// Two of them (2 x 512 x 96 registers) do not fit one SM, so a grid of U CTAs runs on U distinct SMs.
+template <bool PLAIN>
+__global__ void __maxnreg__(TGB_ADAM_MAXNREG)
+k_adam_rows_probe(const AdamRowsArgs p) {
+  const int warps = blockDim.x >> 5;
+  for (int row = p.row0 + blockIdx.x * warps + (threadIdx.x >> 5); row < p.row1; row += gridDim.x * warps)
+    adam_row<PLAIN>(p, row, threadIdx.x & 31);
+}
+#endif
 
 // ---- parity mode (bf16x3): the same streaming pass in the reference's arithmetic ---------------------------------------------
 // IEEE expf / div / sqrt, torch's single-tensor Adam op order (adam_update), P from the row-pass statistics (softmax_prob) --

@@ -606,11 +606,13 @@ static inline int tc_make_map(TcContext& tc, CUtensorMap* map, const void* base,
 
 // Launches k_gemm_tc as a persistent grid of 2-CTA clusters over `pairs` work items (pairs of row tiles x column tiles x
 // splits): at most as many clusters as can be resident at once, which on H100 may leave some SMs idle (the GPCs do not
-// all hold an even number of SMs that a cluster can use).  cudaFuncSetAttribute and the occupancy query are driver calls:
-// they run once per (handle, kernel), not on every launch.
+// all hold an even number of SMs that a cluster can use).  `keep_sms` SMs (rounded up to whole clusters, at least one
+// cluster stays) are left to other work: the streaming update that runs beside a contraction of the bf16 chunk pipeline.
+// Which CTA computes a tile never changes a tile's arithmetic, so the result is the same bits at every grid size.
+// cudaFuncSetAttribute and the occupancy query are driver calls: they run once per (handle, kernel), not on every launch.
 template <class Kern, class... Args>
-static inline int tc_launch(TcContext& tc, Kern kern, int smem, long long pairs, cudaStream_t s, const char* name, char* err,
-                            size_t n, Args... args) {
+static inline int tc_launch(TcContext& tc, Kern kern, int smem, long long pairs, int keep_sms, cudaStream_t s, const char* name,
+                            char* err, size_t n, Args... args) {
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = 2;
@@ -641,7 +643,8 @@ static inline int tc_launch(TcContext& tc, Kern kern, int smem, long long pairs,
     }
     tc.smem_fn[slot] = key; tc.smem_bytes[slot] = smem; tc.clusters[slot] = c;
   }
-  cfg.gridDim = dim3((unsigned)(2 * (pairs < tc.clusters[slot] ? pairs : tc.clusters[slot])));
+  const int clusters = std::max(1, tc.clusters[slot] - (keep_sms + 1) / 2);
+  cfg.gridDim = dim3((unsigned)(2 * (pairs < clusters ? pairs : clusters)));
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { snprintf(err, n, "launch %s: %s", name, cudaGetErrorString(e)); return -2; }
@@ -721,18 +724,18 @@ static inline int tc_forward_launch(TcContext& tc, const TcPlan& pl, int n_pairs
   auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, 0};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
-  return tc_launch(tc, kern, TC_SMEM, tc_pairs(tm, tn, splits), s, "tc_gemm_fwd", err, n, pl.a, pl.b, n_pairs, N, tc_kps(N, splits),
+  return tc_launch(tc, kern, TC_SMEM, tc_pairs(tm, tn, splits), 0, s, "tc_gemm_fwd", err, n, pl.a, pl.b, n_pairs, N, tc_kps(N, splits),
                    tm, tn, splits, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, 0, epi);
 }
 // cells [row0, row1) only (row0 a multiple of 64): `out` = or += this chunk's partial sum -- the host pipelines cell chunks
 // behind the streaming Adam kernel (and the projection adds its 512-cell chains); the chunks run one after the other
 // on one stream, so the summation order is fixed
 static inline int tc_forward_launch_rows(TcContext& tc, const TcPlan& pl, int n_pairs, float* out, int accumulate, int row0, int row1,
-                                         int V, int Ke, cudaStream_t s, char* err, size_t n) {
+                                         int V, int Ke, int keep_sms, cudaStream_t s, char* err, size_t n) {
   auto kern = k_gemm_tc<false, false, tc_stages<TcEpiStore>(), TcEpiStore>;
   TcEpiStore epi{out, Ke, (size_t)V * Ke, V, accumulate};
   const int tm = (int)ceil_div(V, TC_BM), tn = (int)ceil_div(Ke, TC_BN);
-  return tc_launch(tc, kern, TC_SMEM, tc_pairs(tm, tn, 1), s, "tc_gemm_fwd", err, n, pl.a, pl.b, n_pairs, row1,
+  return tc_launch(tc, kern, TC_SMEM, tc_pairs(tm, tn, 1), keep_sms, s, "tc_gemm_fwd", err, n, pl.a, pl.b, n_pairs, row1,
                    (int)round_up(row1 - row0, TC_BK), tm, tn, 1, 1, kPolicyEvictNormal, kPolicyEvictNormal, 0, row0, epi);
 }
 
@@ -754,12 +757,12 @@ static inline int tc_dpstore_epi_plan(TcContext& tc, TcPlan& pl, const __nv_bflo
 }
 template <class Epi>
 static inline int tc_dpstore_launch(TcContext& tc, const TcPlan& pl, int n_pairs, const Epi& epi, int row0, int row1, int V, int Ke,
-                                    cudaStream_t s, char* err, size_t n) {
+                                    int keep_sms, cudaStream_t s, char* err, size_t n) {
   const int tn = (int)ceil_div(V, TC_BN);
   auto kern = k_gemm_tc<true, true, tc_stages<Epi>(), Epi>;
   constexpr int smem = tc_smem<Epi>();
   const int tm0 = row0 / TC_BM, tm = (int)ceil_div(row1, TC_BM) - tm0;
-  return tc_launch(tc, kern, smem, tc_pairs(tm, tn, 1), s, "tc_gemm_bwd_dp", err, n, pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
+  return tc_launch(tc, kern, smem, tc_pairs(tm, tn, 1), keep_sms, s, "tc_gemm_bwd_dp", err, n, pl.a, pl.b, n_pairs, Ke, Ke, tm, tn, 1, 1,
                    kPolicyEvictNormal, kPolicyEvictLast, tm0, 0, epi);
 }
 

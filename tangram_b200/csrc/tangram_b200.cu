@@ -187,6 +187,10 @@ struct tgb200_mapper {
   // chunks; forward(c) of the next iteration waits only for Adam(c).  Which stream a launch goes to is the Lanes of its
   // API call (below).
   bool pipelined = false;       // several chunks: the handle has the streams hi, lo and sf
+  // SMs a pipelined contraction leaves free when an update chunk runs beside it (G(c) for c >= 1 beside A(c-1), the
+  // prefetched F'(c) beside A(c+1)): without them the contraction's grid holds every SM and the update waits for it to
+  // drain.  DESIGN 6b, "Running the update beside the contractions", measures the share.
+  int update_sms = 0;
   // host state (TGB200_STATE_HOST, TGB200_STATE_AUTO): rows [0, R) of M, m / mb and v stay in the device buffers above,
   // rows [R, N) are in pinned host memory (Mh, mh / mbh, vh; R = 0 with host state), and a ring of two device slots of
   // `ring_rows` rows each through which every per-iteration pass streams the host rows (staged_rows): copy-in of block
@@ -562,6 +566,8 @@ extern "C" int tgb200_create(const tgb200_config* cfg, tgb200_mapper** out) {
            cudaEventCreateWithFlags(&h->ev_f[c], cudaEventDisableTiming) == cudaSuccess;
     if (!ok) A(fail(TGB200_ERR_CUDA, "stream / event creation failed: %s", cudaGetErrorString(cudaGetLastError())));
     h->pipelined = ok;
+    h->update_sms = 16;
+    if (const char* e = getenv("TGB200_UPDATE_SMS")) h->update_sms = std::max(0, atoi(e));
   }
   // forward split over cells (deterministic partial planes)
   h->tc.num_sms = prop.multiProcessorCount;
@@ -1418,7 +1424,8 @@ static int forward_plan(tgb200_mapper* h) {
 
 // bf16 mode, cells of chunk c: exact row statistics from the sums the update left (k_row_norm), the scaled forward operand,
 // and -- when the forward is chunked -- this chunk's contribution to Y_ext.  `lseA` / `lseT` as they are for THAT forward.
-static int forward_chunk(tgb200_mapper* h, cudaStream_t s, int c, int fresh, const float* lseA, float* lseT) {
+// `keep_sms`: SMs the contraction leaves to an update chunk running beside it (tc_launch).
+static int forward_chunk(tgb200_mapper* h, cudaStream_t s, int c, int fresh, const float* lseA, float* lseT, int keep_sms) {
   float* rowaux = needs_rowaux(h->cfg) ? h->rowaux.p : nullptr;
   CKS(forward_plan(h));
   const int r0 = h->chunk_row[c], r1 = h->chunk_row[c + 1];
@@ -1433,7 +1440,7 @@ static int forward_chunk(tgb200_mapper* h, cudaStream_t s, int c, int fresh, con
   LAUNCH_CHECK("scale_rows");
   if (h->nchunks > 1) {
     // chunk 0 overwrites the exchange buffer, the others add to it (same stream, fixed order): no partial planes to sum
-    CKS(tc_forward_launch_rows(h->tc, h->plan_fwd, 1, h->Y.p, c > 0 ? 1 : 0, r0, r1, h->V, h->Ke, s, g_err, sizeof(g_err)));
+    CKS(tc_forward_launch_rows(h->tc, h->plan_fwd, 1, h->Y.p, c > 0 ? 1 : 0, r0, r1, h->V, h->Ke, keep_sms, s, g_err, sizeof(g_err)));
     mark(h, s, "tc_gemm_fwd");
   }
   return TGB200_OK;
@@ -1453,7 +1460,7 @@ static int forward_pass(tgb200_mapper* h, cudaStream_t s, int want_entropy) {
       h->fwd_ahead = false;
       for (int c = 0; c < h->nchunks; ++c) CK(cudaStreamWaitEvent(s, h->ev_f[c], 0));
     } else {
-      for (int c = 0; c < h->nchunks; ++c) CKS(forward_chunk(h, s, c, h->p_state == PState::fresh ? 1 : 0, h->lseA, h->lseT));
+      for (int c = 0; c < h->nchunks; ++c) CKS(forward_chunk(h, s, c, h->p_state == PState::fresh ? 1 : 0, h->lseA, h->lseT, 0));
     }
     if (h->nchunks > 1) return TGB200_OK;
   } else if (h->x3) {
@@ -1673,7 +1680,9 @@ static int backward_bf16(tgb200_mapper* h, const Lanes& L, const AdamScalars& a,
   for (int c = 0; c < h->nchunks; ++c) {
     const int r0 = h->chunk_row[c], r1 = h->chunk_row[c + 1];
     TcEpiDpStore epi{h->plan_dp.pt, h->plan_dp.dq, h->ld, h->rcenter.p, h->rpart.p, h->N};
-    CKS(tc_dpstore_launch(h->tc, h->plan_dp, 1, epi, r0, r1, h->V, h->Ke, s, g_err, sizeof(g_err)));
+    // G(c) runs beside A(c - 1); G(0) follows the loss stage, which waited for every update of the previous iteration
+    CKS(tc_dpstore_launch(h->tc, h->plan_dp, 1, epi, r0, r1, h->V, h->Ke, two_streams && c > 0 ? h->update_sms : 0, s, g_err,
+                          sizeof(g_err)));
     mark(h, s, "tc_gemm_bwd_dp");
     if (two_streams) {
       CK(cudaEventRecord(h->ev_g[c], s));
@@ -1700,7 +1709,8 @@ static int backward_bf16(tgb200_mapper* h, const Lanes& L, const AdamScalars& a,
     // (lseT of this iteration is the offset the new P was written with = lseA of the next; the other buffer is free.)
     if (prefetch) {
       if (c == 0) CK(cudaStreamWaitEvent(L.ahead, h->ev_loss, 0));
-      CKS(forward_chunk(h, L.ahead, c, 0, h->lseT, h->lseA));          // waits for ev_a[c]
+      // F'(c) waits for A(c) and runs beside A(c + 1); the last one has no update left beside it
+      CKS(forward_chunk(h, L.ahead, c, 0, h->lseT, h->lseA, c + 1 < h->nchunks ? h->update_sms : 0));   // waits for ev_a[c]
       CK(cudaEventRecord(h->ev_f[c], L.ahead));
     }
   }
@@ -1720,7 +1730,7 @@ static int backward_bf16x3(tgb200_mapper* h, cudaStream_t s, const AdamScalars& 
   TcEpiDpStoreF32 epi{h->dpf.p, h->ld, h->Pb.p, nvp, h->rpart.p, h->N};
   // all six partial products: with only the three or four largest the one-step tests leave their 1e-5 band (measured
   // 28.6 / 25.8 it/s at C3 instead of 21.2 -- not worth the parity-grade mode's point)
-  CKS(tc_dpstore_launch(h->tc, h->plan_dp, 6, epi, 0, h->N, h->V, h->Ke, s, g_err, sizeof(g_err)));
+  CKS(tc_dpstore_launch(h->tc, h->plan_dp, 6, epi, 0, h->N, h->V, h->Ke, 0, s, g_err, sizeof(g_err)));
   mark(h, s, "tc_gemm_bwd_dp");
   k_rowdot_finalize<<<(unsigned)ceil_div(h->N, 256), 256, 0, s>>>(h->rpart.p, h->r_parts, h->N, h->rdot.p);
   LAUNCH_CHECK("rowdot_finalize");
@@ -2720,7 +2730,7 @@ static int project_blocks(tgb200_mapper* h, const float* map, int64_t rows, int6
     // chains of 512 cells, added into out in cell order by the accumulating epilogue (fp32, round-to-nearest)
     for (int64_t c0 = 0; c0 < nb; c0 += kProjChain)
       CKS(tc_forward_launch_rows(tc, pl, 6, O.p, b > 0 || c0 > 0, (int)c0, (int)std::min(nb, c0 + kProjChain), (int)cols,
-                                 (int)ldx, s, g_err, sizeof(g_err)));
+                                 (int)ldx, 0, s, g_err, sizeof(g_err)));
     if (b + 1 < n_blocks) CKS(stage(b + 1));                   // after block b's launches: its copies run under them
   }
   int bad_host = 0;
@@ -3008,3 +3018,61 @@ extern "C" int tgb200_group_stats_expm1(const float* X, int64_t x_ld, const int6
   return group_stats_pass(GsValue::kExpm1, scale, X, x_ld, indptr, indices, data, nnz, rows, n_genes, labels, n_labels,
                           sum_out, sumsq_out, nnz_out, block_rows, device, stream);
 }
+
+#ifdef TGB_OVERLAP_PROBE
+// Debug build only (tools/overlap_probe.py): can a contraction chunk and an update chunk run side by side on disjoint SMs?
+// `kind` 0 is the backward contraction G over chunk 1's rows, 1 the forward contraction F' over chunk 1's rows; its grid
+// is capped at `cap` clusters (0: as many as fit) on the hi stream.  The update runs over chunk 0's rows on the lo
+// stream, as the product launches it (`update_ctas` 0) or as a persistent grid of `update_ctas` CTAs that each hold a
+// whole SM.  `what`: 1 the contraction alone, 2 the update alone, 3 both at once.  For each of `reps` repetitions `out`
+// gets three ms: start to the end of the contraction, to the end of the update, to the end of both.  The kernels read
+// and write the handle's buffers as a step does; what they leave there is not a training state.
+extern "C" TGB200_API int tgb200_debug_overlap_probe(tgb200_mapper* h, int32_t kind, int32_t cap, int32_t update_ctas,
+                                                     int32_t what, int32_t reps, float* out) {
+  if (!h || !out || reps < 1 || what < 1 || what > 3) return fail(TGB200_ERR_INVALID, "bad argument");
+  if (!h->bf16 || !h->pipelined || h->host_state || !h->plan_dp.ready || !h->plan_fwd.ready)
+    return fail(TGB200_ERR_STATE, "needs a resident, pipelined bf16 handle that has run an iteration");
+  CK(cudaSetDevice(h->cfg.device));
+  const int c0 = h->chunk_row[0], c1 = h->chunk_row[1], c2 = h->chunk_row[2];
+  const AdamScalars a = adam_scalars(h->cfg, h->step > 0 ? h->step : 1, 0.1f);
+  const AdamRowsArgs ar{h->M.p, h->mb.p, h->v.p, h->dq.p, h->Pb.p, reinterpret_cast<const RowConst*>(h->rowc.p),
+                        h->zsum.p, h->pxsum.p, h->l1sum.p, h->l2sum.p, h->ld, h->V, c0, c1,
+                        h->cfg.lambda_r, h->cfg.lambda_l1, h->cfg.lambda_l2, a};
+  const bool plain = ar.lam_r == 0.f && ar.lam_l1 == 0.f && ar.lam_l2 == 0.f;
+  const int keep = cap > 0 ? std::max(0, h->tc.num_sms - 2 * cap) : 0;   // every SM of an H100 holds a cluster CTA
+  cudaEvent_t ev[4];
+  for (auto& e : ev) CK(cudaEventCreate(&e));
+  int st = TGB200_OK;
+  CK(cudaDeviceSynchronize());
+  for (int r = 0; r < reps && st == TGB200_OK; ++r) {
+    CK(cudaEventRecord(ev[0], h->hi));
+    CK(cudaStreamWaitEvent(h->lo, ev[0], 0));
+    if (what & 1) {
+      if (kind == 0) {
+        TcEpiDpStore epi{h->plan_dp.pt, h->plan_dp.dq, h->ld, h->rcenter.p, h->rpart.p, h->N};
+        st = tc_dpstore_launch(h->tc, h->plan_dp, 1, epi, c1, c2, h->V, h->Ke, keep, h->hi, g_err, sizeof(g_err));
+      } else {
+        st = tc_forward_launch_rows(h->tc, h->plan_fwd, 1, h->Y.p, 1, c1, c2, h->V, h->Ke, keep, h->hi, g_err, sizeof(g_err));
+      }
+    }
+    if (what & 2) {
+      if (update_ctas <= 0) {
+        if (adam_rows_launch(ar, h->lo)) st = fail(TGB200_ERR_CUDA, "launch adam_rows");
+      } else if (plain) {
+        k_adam_rows_probe<true><<<update_ctas, 512, 0, h->lo>>>(ar);
+      } else {
+        k_adam_rows_probe<false><<<update_ctas, 512, 0, h->lo>>>(ar);
+      }
+      if (cudaGetLastError() != cudaSuccess) st = fail(TGB200_ERR_CUDA, "launch adam_rows_probe");
+    }
+    CK(cudaEventRecord(ev[1], h->hi));
+    CK(cudaEventRecord(ev[2], h->lo));
+    CK(cudaStreamWaitEvent(h->hi, ev[2], 0));
+    CK(cudaEventRecord(ev[3], h->hi));
+    CK(cudaEventSynchronize(ev[3]));
+    for (int i = 0; i < 3; ++i) CK(cudaEventElapsedTime(&out[3 * r + i], ev[0], ev[i + 1]));
+  }
+  for (auto& e : ev) cudaEventDestroy(e);
+  return st;
+}
+#endif
