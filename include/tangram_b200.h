@@ -439,6 +439,28 @@ TGB200_API int tgb200_group_stats_expm1(const float* X, int64_t x_ld, const int6
                                         int64_t* nnz_out, int64_t block_rows, int32_t device, void* stream,
                                         double scale);
 
+/* Spatial neighbour graph (squidpy's gr.spatial_neighbors), exact, in fp64, over a uniform cell grid on the device.
+ *   coords   n x dim fp64, row-major, dim 2 or 3, finite (host or device); n fits int32
+ * d(i, j) = sqrt((dx*dx + dy*dy) + dz*dz) with dx = x_j - x_i, each operation rounded on its own (no FMA): bit-identical
+ * to numpy's np.sqrt(((C[j] - C[i]) ** 2).sum()).  A point is excluded from its own row by index only, so coincident
+ * points are neighbours at distance 0.  Both calls are synchronous on `stream`; TGB200_ERR_INVALID for bad arguments, a
+ * coordinate that is not finite, or data that cannot fit in free device memory (the message gives the sizes);
+ * TGB200_ERR_NO_DEVICE without an sm_90 device (no CPU fallback).
+ *
+ * tgb200_spatial_knn: the k nearest j != i of every point, ranked by (d, j) (ties go to the smaller index), 1 <= k <= 64
+ * and k < n.  indices_out / dist_out: n x k int32 / fp64 (host or device); row i lists its k neighbours in increasing
+ * column order, so it is row i of a canonical CSR with indptr = k * arange(n + 1).
+ *
+ * tgb200_spatial_radius: every j != i with d <= radius (finite, >= 0).  indptr_out: n + 1 int64 (host or device), always
+ * written.  When 0 < indptr_out[n] <= capacity, indices_out / dist_out (int32 / fp64, host or device) receive the rows,
+ * each in search order (not sorted); otherwise they are untouched.  So a caller passes capacity 0 to learn the size and
+ * calls again with buffers of indptr_out[n]; both calls give the same indptr. */
+TGB200_API int tgb200_spatial_knn(const double* coords, int64_t n, int32_t dim, int32_t k, int32_t* indices_out,
+                                  double* dist_out, int32_t device, void* stream);
+TGB200_API int tgb200_spatial_radius(const double* coords, int64_t n, int32_t dim, double radius, int64_t* indptr_out,
+                                     int32_t* indices_out, double* dist_out, int64_t capacity, int32_t device,
+                                     void* stream);
+
 /* Checkpoint / resume (the reference stubs this: `raise NotImplemented`, :151-153).
  * Any pointer may be NULL to skip it.  M, m, v: n_cells x n_voxels f32, host or device. */
 TGB200_API int tgb200_get_state(tgb200_mapper* h, float* M, float* m, float* v, int64_t* step, void* stream);

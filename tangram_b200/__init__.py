@@ -9,6 +9,7 @@
     metrics = tg.train_multiple_Mapper(config, data)     # the tuner's trial: five run-to-run agreement metrics
     tg.rank_genes_groups(ad_sc, groupby="cell_type")     # marker genes per group on the GPU; tg.ctg(ad_sc, "cell_type")
     tg.highly_variable_genes(ad_sc, n_top_genes=4000)    # highly variable genes on the GPU; tg.hvg(ad_sc)
+    tg.spatial_neighbors(ad_sp, set_diag=False)          # the spatial neighbour graph on the GPU (squidpy's)
 
 One process per GPU (process_group=pg, cells and constrained mode): every rank passes the same AnnDatas and gets its
 block of the mapping; project_genes, project_cell_annotations, cell_type_mapping and count_cell_annotations then take that
@@ -30,5 +31,6 @@ from . import mapping_parameter_tuning  # noqa: F401
 from .mapping_parameter_tuning import train_multiple_Mapper  # noqa: F401
 from .adata import MiniAnnData  # noqa: F401
 from .gene_selection import rank_genes_groups, ctg, highly_variable_genes, hvg  # noqa: F401
+from .spatial_neighbors import spatial_neighbors  # noqa: F401
 
 __version__ = "0.2.0"

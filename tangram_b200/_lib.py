@@ -121,6 +121,10 @@ SIGNATURES = {
     "tgb200_group_stats_expm1": (ctypes.c_int, [_P, ctypes.c_int64, _P, _P, _P, ctypes.c_int64, ctypes.c_int64,
                                                 ctypes.c_int64, _P, ctypes.c_int32, _P, _P, _P, ctypes.c_int64,
                                                 ctypes.c_int32, _P, ctypes.c_double]),
+    "tgb200_spatial_knn": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int32, ctypes.c_int32, _P, _P, ctypes.c_int32,
+                                          _P]),
+    "tgb200_spatial_radius": (ctypes.c_int, [_P, ctypes.c_int64, ctypes.c_int32, ctypes.c_double, _P, _P, _P,
+                                             ctypes.c_int64, ctypes.c_int32, _P]),
     "tgb200_get_state":(ctypes.c_int, [_P, _P, _P, _P, _I64, _P]),
     "tgb200_set_state": (ctypes.c_int, [_P, _P, _P, _P, ctypes.c_int64, _P]),
     "tgb200_plan_state": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_uint64, ctypes.POINTER(StatePlan)]),

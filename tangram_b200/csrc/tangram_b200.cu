@@ -23,6 +23,7 @@
 #include "annotate.cuh"
 #include "project.cuh"
 #include "group_stats.cuh"
+#include "neighbors.cuh"
 #include "mt19937_jump.h"
 #include "nccl_dl.h"
 
@@ -3076,3 +3077,215 @@ extern "C" TGB200_API int tgb200_debug_overlap_probe(tgb200_mapper* h, int32_t k
   return st;
 }
 #endif
+
+// Spatial neighbour graph (squidpy's gr.spatial_neighbors): exact k-nearest and radius search over a uniform cell grid
+// (see neighbors.cuh for the kernels and the stop bound).
+namespace {
+constexpr int64_t kNbMaxCellsPerAxis = int64_t(1) << 24;   // keeps the rounding of scaled coordinates below 1e-8 cells
+constexpr int64_t kNbMaxCells = int64_t(1) << 28;
+
+int64_t nb_cell_cap(int64_t n) { return std::min<int64_t>(2 * n + 64, kNbMaxCells); }
+
+// Cells of width h, about `per_cell` points each over the non-degenerate axes' box, at least min_h wide, grown until
+// the grid has at most `cap` cells and no axis more than kNbMaxCellsPerAxis.
+nb::Grid nb_grid(const double lo[3], const double ext[3], int64_t n, double per_cell, double min_h, int64_t cap) {
+  double log_vol = 0.0, max_ext = 0.0;
+  int d_eff = 0;
+  for (int a = 0; a < 3; ++a) {
+    if (ext[a] > 0) { log_vol += std::log(ext[a]); ++d_eff; }
+    max_ext = std::max(max_ext, ext[a]);
+  }
+  double h = d_eff ? std::exp((log_vol + std::log(per_cell / (double)n)) / d_eff) : 1.0;
+  h = std::max(h, min_h);
+  if (!(h > 0) || !std::isfinite(1.0 / h)) h = max_ext > 0 ? max_ext : 1.0;
+  nb::Grid g{};
+  for (;;) {
+    const double inv = 1.0 / h;
+    double total = 1.0;
+    bool ok = true;
+    for (int a = 0; a < 3; ++a) {
+      const double c = std::floor(ext[a] * inv) + 1.0;
+      ok &= c <= (double)kNbMaxCellsPerAxis;
+      total *= c;
+    }
+    if (ok && total <= (double)cap) {
+      g.inv_h = inv;
+      for (int a = 0; a < 3; ++a) { g.lo[a] = lo[a]; g.nc[a] = (int)(std::floor(ext[a] * inv) + 1.0); }
+      break;
+    }
+    h *= 1.25;
+  }
+  g.h_lo = (1.0 / g.inv_h) * (1.0 - 1e-9);
+  if (!(g.h_lo > 1e-150)) g.h_lo = 0.0;        // distances that small underflow when squared: no early stop
+  return g;
+}
+
+// One search's device state: the staged coordinates, the points in cell order and the cell offsets.
+struct NbSearch {
+  DevBuf<double> C, xs, ys, zs;
+  DevBuf<int> orig, cell, count, bad;
+  DevBuf<long long> start, tiles;
+  DevBuf<unsigned long long> box;
+  nb::Grid g{};
+  int n = 0;
+  nb::Points points() const { return nb::Points{xs.p, ys.p, zs.p, orig.p, start.p}; }
+};
+
+int64_t nb_scan_tiles(int64_t n) { return ceil_div(n, nb::kScanTile); }
+
+// out[0..n] = exclusive prefix of in[0..n) and the total; tiles holds 2 (tiles + 1) values.
+int nb_scan(const int* in, int64_t n, long long* out, long long* tiles, cudaStream_t s) {
+  const int64_t nt = nb_scan_tiles(n);
+  nb::k_nb_scan_tiles<<<(unsigned)nt, 256, 0, s>>>(in, n, out, tiles);
+  CK(cudaGetLastError());
+  lrng::k_scan_counts<<<1, 1024, 0, s>>>(tiles, (int)nt, tiles + nt + 1);
+  CK(cudaGetLastError());
+  nb::k_nb_scan_add<<<(unsigned)ceil_div(n + 1, nb::kThreads), nb::kThreads, 0, s>>>(out, n, tiles + nt + 1, (int)nt);
+  CK(cudaGetLastError());
+  return TGB200_OK;
+}
+
+// Device bytes of a search over n points before its output: staged and sorted points, cell ids, the cell histogram
+// and offsets at the cell cap, the scan's tiles.
+double nb_search_bytes(int64_t n, int dim) {
+  const int64_t cells = nb_cell_cap(n);
+  return 8.0 * n * dim + 32.0 * n + 4.0 * n + 12.0 * (cells + 1) + 16.0 * (nb_scan_tiles(std::max(cells, n) + 1) + 1);
+}
+
+// Stages the coordinates, checks them, sizes the grid and sorts the points into cell order.  `out_bytes`: the caller's
+// output buffers, counted in the memory check.
+int nb_build(const double* coords, int64_t n, int dim, double per_cell, double min_h, double out_bytes, int32_t device,
+             cudaStream_t s, const char* what, NbSearch& S) {
+  int n_sms = 0;
+  CKS(use_sm90_device(device, &n_sms));
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const double need = nb_search_bytes(n, dim) + out_bytes, avail = (double)free_b - 256.0 * (1 << 20);
+  if (need > avail)
+    return fail(TGB200_ERR_INVALID, "%s over %lld points in %d-D needs %.3f GiB on device %d (%.3f GiB of it for the "
+                "output); %.3f GiB are free", what, (long long)n, dim, need / 1073741824.0, device,
+                out_bytes / 1073741824.0, free_b / 1073741824.0);
+  S.n = (int)n;
+  CKS(S.C.alloc((size_t)n * dim, false));
+  CK(cudaMemcpyAsync(S.C.p, coords, sizeof(double) * n * dim, cudaMemcpyDefault, s));
+  unsigned long long box0[6];
+  for (int a = 0; a < 3; ++a) { box0[2 * a] = ~0ull; box0[2 * a + 1] = 0ull; }
+  CKS(S.box.alloc(6, false));
+  CKS(S.bad.alloc(1, false));
+  CK(cudaMemcpyAsync(S.box.p, box0, sizeof(box0), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(S.bad.p, 0, sizeof(int), s));
+  const unsigned bb = (unsigned)std::min<int64_t>(ceil_div(n, nb::kThreads), 8 * (int64_t)n_sms);
+  nb::k_nb_bbox<<<bb, nb::kThreads, 0, s>>>(S.C.p, (int)n, dim, S.box.p, S.bad.p);
+  CK(cudaGetLastError());
+  unsigned long long box[6];
+  int bad = 0;
+  CK(cudaMemcpyAsync(box, S.box.p, sizeof(box), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&bad, S.bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad) return fail(TGB200_ERR_INVALID, "%s: a coordinate is not finite", what);
+  double lo[3] = {0, 0, 0}, ext[3] = {0, 0, 0};
+  for (int a = 0; a < dim; ++a) {
+    lo[a] = nb::from_ordered_bits(box[2 * a]);
+    ext[a] = nb::from_ordered_bits(box[2 * a + 1]) - lo[a];
+    if (!std::isfinite(ext[a]))
+      return fail(TGB200_ERR_INVALID, "%s: the coordinates of axis %d span more than the largest double", what, a);
+  }
+  S.g = nb_grid(lo, ext, n, per_cell, min_h, nb_cell_cap(n));
+  const int64_t cells = (int64_t)S.g.nc[0] * S.g.nc[1] * S.g.nc[2];
+  CKS(S.xs.alloc(n, false)); CKS(S.ys.alloc(n, false)); CKS(S.zs.alloc(n, false));
+  CKS(S.orig.alloc(n, false)); CKS(S.cell.alloc(n, false));
+  CKS(S.count.alloc(cells, false));
+  CKS(S.start.alloc(cells + 1, false));
+  CKS(S.tiles.alloc(2 * (nb_scan_tiles(std::max<int64_t>(cells, n) + 1) + 1), false));
+  CK(cudaMemsetAsync(S.count.p, 0, sizeof(int) * cells, s));
+  const unsigned pb = (unsigned)ceil_div(n, nb::kThreads);
+  nb::k_nb_cells<<<pb, nb::kThreads, 0, s>>>(S.C.p, (int)n, dim, S.g, S.cell.p, S.count.p);
+  CK(cudaGetLastError());
+  CKS(nb_scan(S.count.p, cells, S.start.p, S.tiles.p, s));
+  nb::k_nb_scatter<<<pb, nb::kThreads, 0, s>>>(S.C.p, (int)n, dim, S.cell.p, S.count.p, S.start.p, S.xs.p, S.ys.p, S.zs.p,
+                                               S.orig.p);
+  CK(cudaGetLastError());
+  return TGB200_OK;
+}
+
+int nb_check(const double* coords, int64_t n, int32_t dim, int64_t min_n, const char* what) {
+  if (!coords) return fail(TGB200_ERR_INVALID, "%s: null coordinates", what);
+  if (dim != 2 && dim != 3) return fail(TGB200_ERR_INVALID, "%s: dim=%d, must be 2 or 3", what, dim);
+  if (n < min_n || n > INT32_MAX)
+    return fail(TGB200_ERR_INVALID, "%s: n=%lld points, must lie in [%lld, %d]", what, (long long)n, (long long)min_n,
+                INT32_MAX);
+  return TGB200_OK;
+}
+}  // namespace
+
+extern "C" int tgb200_spatial_knn(const double* coords, int64_t n, int32_t dim, int32_t k, int32_t* indices_out,
+                                  double* dist_out, int32_t device, void* stream) {
+  const char* what = "k-nearest-neighbour search";
+  CKS(nb_check(coords, n, dim, 2, what));
+  if (!indices_out || !dist_out) return fail(TGB200_ERR_INVALID, "%s: null output", what);
+  if (k < 1 || k > nb::kMaxK) return fail(TGB200_ERR_INVALID, "%s: k=%d, must lie in [1, %d]", what, k, nb::kMaxK);
+  if (k >= n) return fail(TGB200_ERR_INVALID, "%s: k=%d needs more than k points, got n=%lld", what, k, (long long)n);
+  cudaStream_t s = (cudaStream_t)stream;
+  NbSearch S;
+  CKS(nb_build(coords, n, dim, std::max(2.0, 0.5 * (k + 1)), 0.0, 12.0 * n * k, device, s, what, S));
+  DevBuf<int> cols;
+  DevBuf<double> dists;
+  CKS(cols.alloc((size_t)n * k, false));
+  CKS(dists.alloc((size_t)n * k, false));
+  const unsigned pb = (unsigned)ceil_div(n, nb::kThreads);
+  const nb::Points P = S.points();
+  if (k <= 8) nb::k_nb_knn<8><<<pb, nb::kThreads, 0, s>>>(S.g, P, (int)n, k, cols.p, dists.p);
+  else if (k <= 16) nb::k_nb_knn<16><<<pb, nb::kThreads, 0, s>>>(S.g, P, (int)n, k, cols.p, dists.p);
+  else if (k <= 32) nb::k_nb_knn<32><<<pb, nb::kThreads, 0, s>>>(S.g, P, (int)n, k, cols.p, dists.p);
+  else nb::k_nb_knn<64><<<pb, nb::kThreads, 0, s>>>(S.g, P, (int)n, k, cols.p, dists.p);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(indices_out, cols.p, sizeof(int) * n * k, cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(dist_out, dists.p, sizeof(double) * n * k, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}
+
+extern "C" int tgb200_spatial_radius(const double* coords, int64_t n, int32_t dim, double radius, int64_t* indptr_out,
+                                     int32_t* indices_out, double* dist_out, int64_t capacity, int32_t device,
+                                     void* stream) {
+  const char* what = "radius search";
+  CKS(nb_check(coords, n, dim, 1, what));
+  if (!indptr_out) return fail(TGB200_ERR_INVALID, "%s: null indptr_out", what);
+  if (!(radius >= 0) || !std::isfinite(radius))
+    return fail(TGB200_ERR_INVALID, "%s: radius=%g, must be finite and non-negative", what, radius);
+  if (capacity < 0 || (capacity > 0 && (!indices_out || !dist_out)))
+    return fail(TGB200_ERR_INVALID, "%s: capacity=%lld needs indices_out and dist_out", what, (long long)capacity);
+  cudaStream_t s = (cudaStream_t)stream;
+  NbSearch S;
+  // cells just wider than the radius: rings 0 and 1 hold every neighbour, and the bound after ring 1 exceeds it
+  CKS(nb_build(coords, n, dim, 2.0, radius * (1.0 + 1e-5), 12.0 * (n + 1), device, s, what, S));
+  DevBuf<int> count;
+  DevBuf<long long> off;
+  CKS(count.alloc(n, false));
+  CKS(off.alloc(n + 1, false));
+  const unsigned pb = (unsigned)ceil_div(n, nb::kThreads);
+  const nb::Points P = S.points();
+  nb::k_nb_radius<false><<<pb, nb::kThreads, 0, s>>>(S.g, P, (int)n, radius, count.p, nullptr, nullptr, nullptr);
+  CK(cudaGetLastError());
+  CKS(nb_scan(count.p, n, off.p, S.tiles.p, s));
+  CK(cudaMemcpyAsync(indptr_out, off.p, sizeof(int64_t) * (n + 1), cudaMemcpyDefault, s));
+  long long nnz = 0;
+  CK(cudaMemcpyAsync(&nnz, off.p + n, sizeof(long long), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (nnz == 0 || nnz > capacity) return TGB200_OK;
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  if (12.0 * nnz > (double)free_b - 256.0 * (1 << 20))
+    return fail(TGB200_ERR_INVALID, "%s: %lld neighbour pairs need %.3f GiB on device %d; %.3f GiB are free", what, nnz,
+                12.0 * nnz / 1073741824.0, device, free_b / 1073741824.0);
+  DevBuf<int> cols;
+  DevBuf<double> dists;
+  CKS(cols.alloc(nnz, false));
+  CKS(dists.alloc(nnz, false));
+  nb::k_nb_radius<true><<<pb, nb::kThreads, 0, s>>>(S.g, P, (int)n, radius, nullptr, off.p, cols.p, dists.p);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(indices_out, cols.p, sizeof(int) * nnz, cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(dist_out, dists.p, sizeof(double) * nnz, cudaMemcpyDefault, s));
+  CK(cudaStreamSynchronize(s));
+  return TGB200_OK;
+}

@@ -3,8 +3,8 @@
 (Tangram's tangram/mapping_utils.py:141-428), hosted over the H100 Mapper.
 AnnData in, AnnData out (duck-typed: `anndata` is optional).  `pp_adatas` and
 `adata_to_cluster_expression` are the small host-side preparations this entry needs
-(:20-139); squidpy's neighbour graph must be supplied by the caller in
-`adata_sp.obsp` (scipy CSR), as squidpy itself would leave it.
+(:20-139).  The spatial terms read the neighbour graph from `adata_sp.obsp`
+(scipy CSR); `tg.spatial_neighbors(adata_sp)` builds it on the GPU, as squidpy would.
 """
 import logging
 
@@ -40,8 +40,9 @@ def one_hot_encoding(labels):
 
 
 def pp_adatas(adata_sc, adata_sp, genes=None, gene_to_lowercase=True):
-    """mapping_utils.py:20-100 (gene intersection + density priors).  The squidpy neighbour
-    graph (:95-100) is not computed here: pass it in adata_sp.obsp."""
+    """mapping_utils.py:20-100 (gene intersection + density priors).  The neighbour graph
+    (:95-100) is not computed here: build it with tg.spatial_neighbors(adata_sp), or pass it
+    in adata_sp.obsp."""
     for ad in (adata_sc, adata_sp):
         # sc.pp.filter_genes(ad, min_cells=1) (:47-48): records var['n_cells'], then drops the all-zero genes IN PLACE --
         # through AnnData._inplace_subset_var, as scanpy does (assigning a differently shaped X / var to a real AnnData raises)
