@@ -11,7 +11,8 @@
 //   warpgroup 0     TMA producer (one thread): keeps the operand ring full across tile boundaries, so the loads of
 //                   tile i+1 run while the consumers drain tile i
 //   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the tile, m64n256k16 wgmma into 128 fp32 registers per
-//                   thread, then the epilogue on those registers
+//                   thread, then the epilogue on those registers (the bf16 backward's: packed at once, the rest of it
+//                   deferred into the next tile's first k-blocks)
 #pragma once
 #include <cuda.h>
 #include <cstdio>
@@ -163,6 +164,40 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t a_des
         "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
 }
+// D = A[smem] * B[smem], the first MMA of a tile: D is an output only, so whatever it held before is dead to the compiler
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256k16_first(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, 0, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+      "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+      "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+      "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+      "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+      "}, %128, %129, p, 1, 1, %130, %131;\n\t}"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]),
+        "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]),
+        "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]),
+        "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]),
+        "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]), "=f"(d[37]), "=f"(d[38]), "=f"(d[39]),
+        "=f"(d[40]), "=f"(d[41]), "=f"(d[42]), "=f"(d[43]), "=f"(d[44]), "=f"(d[45]), "=f"(d[46]), "=f"(d[47]),
+        "=f"(d[48]), "=f"(d[49]), "=f"(d[50]), "=f"(d[51]), "=f"(d[52]), "=f"(d[53]), "=f"(d[54]), "=f"(d[55]),
+        "=f"(d[56]), "=f"(d[57]), "=f"(d[58]), "=f"(d[59]), "=f"(d[60]), "=f"(d[61]), "=f"(d[62]), "=f"(d[63]),
+        "=f"(d[64]), "=f"(d[65]), "=f"(d[66]), "=f"(d[67]), "=f"(d[68]), "=f"(d[69]), "=f"(d[70]), "=f"(d[71]),
+        "=f"(d[72]), "=f"(d[73]), "=f"(d[74]), "=f"(d[75]), "=f"(d[76]), "=f"(d[77]), "=f"(d[78]), "=f"(d[79]),
+        "=f"(d[80]), "=f"(d[81]), "=f"(d[82]), "=f"(d[83]), "=f"(d[84]), "=f"(d[85]), "=f"(d[86]), "=f"(d[87]),
+        "=f"(d[88]), "=f"(d[89]), "=f"(d[90]), "=f"(d[91]), "=f"(d[92]), "=f"(d[93]), "=f"(d[94]), "=f"(d[95]),
+        "=f"(d[96]), "=f"(d[97]), "=f"(d[98]), "=f"(d[99]), "=f"(d[100]), "=f"(d[101]), "=f"(d[102]), "=f"(d[103]),
+        "=f"(d[104]), "=f"(d[105]), "=f"(d[106]), "=f"(d[107]), "=f"(d[108]), "=f"(d[109]), "=f"(d[110]), "=f"(d[111]),
+        "=f"(d[112]), "=f"(d[113]), "=f"(d[114]), "=f"(d[115]), "=f"(d[116]), "=f"(d[117]), "=f"(d[118]), "=f"(d[119]),
+        "=f"(d[120]), "=f"(d[121]), "=f"(d[122]), "=f"(d[123]), "=f"(d[124]), "=f"(d[125]), "=f"(d[126]), "=f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "n"(TA), "n"(TB));
+}
 // ---- descriptors ----------------------------------------------------------------------------
 // Shared-memory matrix descriptor (cute/arch/mma_sm90_desc.hpp GmmaDescriptor): start>>4 [0,14),
 // LBO>>4 [16,30), SBO>>4 [32,46), layout SWIZZLE_128B=1 [62,64).
@@ -210,14 +245,41 @@ struct OperandTile {
   }
 };
 
+// ---- phase probe (debug build only) --------------------------------------------------------------
+#ifdef TGB_BWD_PHASE_PROBE
+// tools/bwd_phase_probe.py: for every (tile, consumer warpgroup) of the bf16 backward, thread 0 of the warpgroup writes
+// clock64() at six points of the tile's life (kBwdProbe*), the SM it ran on and globaltimer at the first one, into
+// g_bwd_probe[(tile * 2 + cw) * 8 + ...], tile = row tile * column tiles + column tile.  Null: nothing is recorded.
+enum { kBwdProbeFull, kBwdProbeRetired, kBwdProbePtFull, kBwdProbeStmatrix, kBwdProbeStore, kBwdProbeRead, kBwdProbeSm, kBwdProbeNs };
+__device__ unsigned long long* g_bwd_probe;
+__device__ __forceinline__ void bwd_probe(long long tile, int cw, int what) {
+  if (g_bwd_probe == nullptr || tile < 0 || (threadIdx.x & 127) != 0) return;
+  unsigned long long* p = g_bwd_probe + (tile * 2 + cw) * 8;
+  p[what] = clock64();
+  if (what == kBwdProbeFull) {
+    unsigned long long ns;
+    uint32_t sm;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    p[kBwdProbeSm] = sm;
+    p[kBwdProbeNs] = ns;
+  }
+}
+#define TGB_BWD_PROBE(tile, cw, what) bwd_probe(tile, cw, what)
+#else
+#define TGB_BWD_PROBE(tile, cw, what) ((void)0)
+#endif
+
 // ---- epilogues ------------------------------------------------------------------------------
 // run() gets one consumer thread's accumulator fragment of the m64n256 wgmma: for every 8-column group j, d[4j], d[4j+1]
 // are columns (8j + 2 (lane % 4), +1) of row `row`, and d[4j+2], d[4j+3] the same columns of row `row + 8`.  A quad of
 // lanes covers 8 consecutive columns of a row (one 32-byte sector of fp32).  prologue() is called by all 256 consumer
 // threads (`ct`) before the tile's main loop.
 // An epilogue may also own kSmemBytes of shared memory after the operand ring (EpiSmem).  load() is then called by the
-// producer thread once per tile, after the tile's first STAGES k-blocks have been handed to the ring, to fill it.
-// Each consumer warpgroup `cw` owns one full / free mbarrier pair for its half; `parity` is the tile's phase of both.
+// producer thread during the tile's main loop (TcEpiDpStore: in two rounds, at fixed k-blocks) to fill it.
+// Each consumer warpgroup `cw` owns one full / free mbarrier pair for its half; `parity` is the current phase of both.
+// A deferred epilogue (kDeferred) has no run(): its tile's accumulators are packed into registers right after the last
+// MMA, and the rest runs as kSteps steps interleaved with the next tile's first k-blocks (see k_gemm_tc).
 struct EpiSmem {
   uint8_t* buf;          // 1024-byte aligned
   uint64_t* full;        // [2] arrive count 1 + transaction bytes: the producer's load of half cw has landed
@@ -250,6 +312,7 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 struct TcEpiStore {
   static constexpr int kSmemBytes = 0;
+  static constexpr bool kDeferred = false;
   float* C; int ldc; size_t split_stride; int M;
   int accumulate;        // 1: C += tile (cell chunks of the pipelined forward run one after the other: fixed summation order)
   __device__ __forceinline__ void prologue(const TileCoord&, int) const {}
@@ -279,14 +342,30 @@ struct TcEpiStore {
 // dP_ij - r_i, so the bf16 rounding is relative to the deviation from the row mean, not to dP itself), and the same
 // epilogue accumulates this iteration's row-dot partials r'_i = sum_j Pt_ij dq_ij from the ROUNDED values (so that
 // sum_j g_ij = 0 holds for what the streaming Adam kernel consumes).
-// The tile's Pt comes in by TMA during the main loop, into a 128 x 256 bf16 shared-memory tile (per 64-row half four
-// 64 x 64 boxes of 8 KB, 128-byte swizzle); the epilogue reads it with ldmatrix, writes dq over it with stmatrix and
-// each consumer warpgroup stores its half with TMA.  Both streams use evict_first: they pass through L2 once, beside the
-// dY_ext operand that every tile re-reads.
+// The tile's Pt comes in by TMA in two rounds of 128 columns, each into a 128 x 128 bf16 shared-memory tile (per 64-row
+// half two 64 x 64 boxes of 8 KB, 128-byte swizzle); the epilogue reads a round with ldmatrix, writes dq over it with
+// stmatrix and each consumer warpgroup stores its half of the round with TMA.  Both streams use evict_first: they pass
+// through L2 once, beside the dY_ext operand that every tile re-reads.  A 32 KB buffer (instead of one for the whole
+// 64 KB tile) leaves room for a fourth operand stage.
+// The epilogue is deferred: pack() turns the accumulators into the 64 bf16x2 values that become dq as soon as the tile's
+// last MMA retires, so the next tile's MMAs can start at once, and step(0..7) then does the shared-memory half, each step
+// right after one of the next tile's k-blocks (step_kb): per round, one 64-column box of ldmatrix / row-dot / stmatrix in
+// each of two steps, the TMA store, and the release of the buffer one k-block later.  The row-dot sums the same rounded
+// values in the same order as an epilogue run in one piece, so dq and rpart do not depend on the deferral.
 struct TcEpiDpStore {
-  static constexpr int kSmemBytes = TC_BM * TC_BN * 2;
+  static constexpr int kSmemBytes = TC_BM * (TC_BN / 2) * 2;
   static constexpr int kHalfBytes = kSmemBytes / 2;
   static constexpr int kBoxBytes = 64 * 128;
+  static constexpr bool kDeferred = true;
+  static constexpr int kSteps = 8;                        // per round: two boxes, the store, the release
+  static constexpr int kRound1Kb = 10;                    // the second round's steps start after this k-block
+  // k-block of the next tile after which step s runs: round 0 after k-blocks 0-3, round 1 after kRound1Kb..+3
+  static __host__ __device__ constexpr int step_kb(int s) { return s < 4 ? s : kRound1Kb + s - 4; }
+  // Producer: the previous tile's second round is loaded after the current tile's kLoadKb1-th k-block, the current
+  // tile's first round after its kLoadKb0-th.  The rounds are released after k-blocks 3 and kRound1Kb + 3, and the
+  // producer runs at most STAGES (4) k-blocks ahead of the consumers, so neither load waits for its release or holds up
+  // the ring; the second round still lands well before its steps.
+  static constexpr int kLoadKb1 = 8, kLoadKb0 = 18;
   CUtensorMap pt_map, dq_map;                             // Pt / dq [M][ld] bf16, box {64 columns, 64 rows}
   int ld;                                                 // a multiple of 64
   const float* center;                                    // c_i (per row)
@@ -295,66 +374,103 @@ struct TcEpiDpStore {
   // boxes of the 64-row half starting at row r0 that hold data; with ld a multiple of 64 a box lies wholly inside
   // [0, ld) or wholly past it, and TMA clips the rows >= M of a partly filled one
   __device__ __forceinline__ int boxes(int r0, int n0) const { return r0 < M ? min(TC_BN / 64, (ld - n0) / 64) : 0; }
-  __device__ __forceinline__ void prologue(const TileCoord&, int) const {}
-  __device__ __forceinline__ void load(int m0, int n0, const EpiSmem& es) const {
+  // the tile's index among all tiles of the contraction (the phase probe's record)
+  __device__ __forceinline__ long long tile_id(int m0, int tile_n) const { return (long long)(m0 / TC_BM) * ((ld + TC_BN - 1) / TC_BN) + tile_n; }
+  // c of this thread's rows `row`, `row + 8`, read before the tile's main loop
+  __device__ __forceinline__ void centres(int row, float (&c)[2]) const {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) c[h] = row + 8 * h < M ? center[row + 8 * h] : 0.f;
+  }
+  // v[2j + h] = bf16(d - c) of columns 8j + 2 (lane % 4), +1 of row `row + 8h`
+  static __device__ __forceinline__ void pack(const float (&d)[TC_ACC], const float (&c)[2], uint32_t (&v)[TC_ACC / 2]) {
+#pragma unroll
+    for (int j = 0; j < TC_BN / 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const __nv_bfloat162 d2 = __floats2bfloat162_rn(d[4 * j + 2 * h] - c[h], d[4 * j + 2 * h + 1] - c[h]);
+        v[2 * j + h] = *reinterpret_cast<const uint32_t*>(&d2);
+      }
+    }
+  }
+  // Step s (a constant once the caller's loop is unrolled) of the epilogue of the tile at (m0, tile_n), whose packed
+  // values are v; racc carries the row-dot from step to step.
+  __device__ __forceinline__ void step(int s, const uint32_t (&v)[TC_ACC / 2], float (&racc)[2], int m0, int tile_n, int row,
+                                       int lane, int cw, EpiSmem& es) const {
+    const int r0 = m0 + 64 * cw, n0 = tile_n * TC_BN;
+    const int nb = boxes(r0, n0);
+    const int round = s / 4, sr = s % 4;
+    if (sr < 2) {
+      const int b = 2 * round + sr;                       // the box: columns 64 b .. +64 of the tile
+      // ldmatrix / stmatrix address of this lane: row (lane % 8) of matrix lane / 8, where matrices 0..3 are
+      // (rows +0, columns 8j), (rows +8, 8j), (rows +0, 8j + 8), (rows +8, 8j + 8) of the warp's 16 rows
+      const int mi = lane >> 3, rr = lane & 7;
+      const int arow = ((row - r0) & ~15) + 8 * (mi & 1) + rr;
+      const uint32_t half = smem_u32(es.buf + cw * kHalfBytes) + arow * 128;
+      if (sr == 0) {
+        mbar_wait(&es.full[cw], es.parity);
+        if (round == 0) {
+          TGB_BWD_PROBE(tile_id(m0, tile_n), cw, kBwdProbePtFull);
+          racc[0] = racc[1] = 0.f;
+        }
+      }
+      if (b < nb) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {                     // columns 64 b + 16 q .. +16: j = 8 b + 2 q, +1
+          const uint32_t addr = half + sr * kBoxBytes + (((2 * q + (mi >> 1)) ^ rr) << 4);
+          uint32_t p[4], o[4];
+          ldmatrix_x4(addr, p);
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = 8 * b + 2 * q + e;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const __nv_bfloat162 d2 = *reinterpret_cast<const __nv_bfloat162*>(&v[2 * j + h]);
+              const __nv_bfloat162 p2 = *reinterpret_cast<const __nv_bfloat162*>(&p[2 * e + h]);
+              racc[h] = fmaf(__low2float(p2), __low2float(d2), racc[h]);
+              racc[h] = fmaf(__high2float(p2), __high2float(d2), racc[h]);
+              o[2 * e + h] = v[2 * j + h];
+            }
+          }
+          stmatrix_x4(addr, o);
+        }
+      }
+      if (b == TC_BN / 64 - 1) TGB_BWD_PROBE(tile_id(m0, tile_n), cw, kBwdProbeStmatrix);
+    } else if (sr == 2) {
+      fence_proxy_async_smem();
+      if (cw == 0) named_bar_sync<1>(128); else named_bar_sync<2>(128);    // this warpgroup's stmatrix writes are done
+      if ((threadIdx.x & 127) == 0) {
+        for (int b = 2 * round; b < min(nb, 2 * round + 2); ++b)
+          tma_store_2d(&dq_map, es.buf + cw * kHalfBytes + (b - 2 * round) * kBoxBytes, n0 + 64 * b, r0, kPolicyEvictFirst);
+        bulk_commit();
+      }
+      if (round == 1) {
+        TGB_BWD_PROBE(tile_id(m0, tile_n), cw, kBwdProbeStore);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float sum = quad_sum(racc[h]);
+          if (row + 8 * h < M && (lane & 3) == 0) rpart[(size_t)tile_n * M + row + 8 * h] = sum;
+        }
+      }
+    } else {
+      if ((threadIdx.x & 127) == 0) {
+        bulk_wait_read_all();                             // the half may be refilled once the stores have read it
+        if (round == 1) TGB_BWD_PROBE(tile_id(m0, tile_n), cw, kBwdProbeRead);
+        mbar_arrive(&es.free[cw]);
+      }
+      es.parity ^= 1;
+    }
+  }
+  // round r (columns 128 r .. +128) of the tile's Pt into the buffer, once the consumers have released it; the caller
+  // flips es.parity after each round
+  __device__ __forceinline__ void load(int m0, int n0, int r, const EpiSmem& es) const {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       mbar_wait(&es.free[h], es.parity ^ 1);
-      const int nb = boxes(m0 + 64 * h, n0);
+      const int nb = min(2, max(0, boxes(m0 + 64 * h, n0) - 2 * r));
       mbar_expect_tx(&es.full[h], nb * kBoxBytes);
       for (int b = 0; b < nb; ++b)
-        tma_load_2d(&pt_map, &es.full[h], es.buf + h * kHalfBytes + b * kBoxBytes, n0 + 64 * b, m0 + 64 * h, kPolicyEvictFirst);
-    }
-  }
-  __device__ __forceinline__ void run(const float (&d)[TC_ACC], const TileCoord& t, int row, int lane, int cw,
-                                      const EpiSmem& es) const {
-    const int r0 = t.m0 + 64 * cw;
-    const int nb = boxes(r0, t.n0);
-    float c[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) c[h] = row + 8 * h < M ? center[row + 8 * h] : 0.f;
-    // ldmatrix / stmatrix address of this lane: row (lane % 8) of matrix lane / 8, where matrices 0..3 are
-    // (rows +0, columns 8j), (rows +8, 8j), (rows +0, 8j + 8), (rows +8, 8j + 8) of the warp's 16 rows
-    const int mi = lane >> 3, rr = lane & 7;
-    const int arow = ((row - r0) & ~15) + 8 * (mi & 1) + rr;
-    const uint32_t half = smem_u32(es.buf + cw * kHalfBytes) + arow * 128;
-    mbar_wait(&es.full[cw], es.parity);
-    float racc[2] = {0.f, 0.f};
-#pragma unroll
-    for (int b = 0; b < TC_BN / 64; ++b) {
-      if (b >= nb) break;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {                       // columns 64 b + 16 q .. +16: j = 8 b + 2 q, +1
-        const uint32_t addr = half + b * kBoxBytes + (((2 * q + (mi >> 1)) ^ rr) << 4);
-        uint32_t p[4], o[4];
-        ldmatrix_x4(addr, p);
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int j = 8 * b + 2 * q + e;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const __nv_bfloat162 d2 = __floats2bfloat162_rn(d[4 * j + 2 * h] - c[h], d[4 * j + 2 * h + 1] - c[h]);
-            const __nv_bfloat162 p2 = *reinterpret_cast<const __nv_bfloat162*>(&p[2 * e + h]);
-            racc[h] = fmaf(__low2float(p2), __low2float(d2), racc[h]);
-            racc[h] = fmaf(__high2float(p2), __high2float(d2), racc[h]);
-            o[2 * e + h] = *reinterpret_cast<const uint32_t*>(&d2);
-          }
-        }
-        stmatrix_x4(addr, o);
-      }
-    }
-    fence_proxy_async_smem();
-    if (cw == 0) named_bar_sync<1>(128); else named_bar_sync<2>(128);    // this warpgroup's stmatrix writes are done
-    if ((threadIdx.x & 127) == 0) {
-      for (int b = 0; b < nb; ++b) tma_store_2d(&dq_map, es.buf + cw * kHalfBytes + b * kBoxBytes, t.n0 + 64 * b, r0, kPolicyEvictFirst);
-      bulk_commit();
-      bulk_wait_read_all();                               // the half may be refilled once the stores have read it
-      mbar_arrive(&es.free[cw]);
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const float s = quad_sum(racc[h]);
-      if (row + 8 * h < M && (lane & 3) == 0) rpart[(size_t)t.tile_n * M + row + 8 * h] = s;
+        tma_load_2d(&pt_map, &es.full[h], es.buf + h * kHalfBytes + b * kBoxBytes, n0 + 128 * r + 64 * b, m0 + 64 * h,
+                    kPolicyEvictFirst);
     }
   }
 };
@@ -363,6 +479,7 @@ struct TcEpiDpStore {
 // row-dot partials use P reconstructed from its three bf16 planes (hi + mid + lo = the fp32 value the row pass computed).
 struct TcEpiDpStoreF32 {
   static constexpr int kSmemBytes = 0;
+  static constexpr bool kDeferred = false;
   float* dp; int ld;                       // [rows][ld] fp32
   const __nv_bfloat16* P3; size_t plane;   // three planes of [rows][ld] bf16
   float* rpart;                            // [tiles_n][M]
@@ -470,6 +587,8 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
     setmaxnreg_producer();
     if (threadIdx.x == 0) {
       uint32_t kbg = 0;                         // k-blocks issued so far (ring position)
+      int prev_m0 = -1, prev_n0 = 0;            // a live tile whose epilogue buffer still needs its second round
+      (void)prev_n0;
       for (int w = cluster_index(); w < total; w += cluster_count()) {
         const int z = w / (tiles_n * tiles_mp);
         int tp_i, tn_i;
@@ -495,13 +614,103 @@ k_gemm_tc(const __grid_constant__ TcMaps maps_a, const __grid_constant__ TcMaps 
             if (live) TileA::load(ma, &full_bar[s], sa, m0, k0, policy_a);
             TileB::load_half_pair(mb, &full_bar[s], sb, n0, k0, cluster_rank(), policy_b);
 #ifndef TGB_SKIP_EPI
-            // not before: waiting for the previous tile's epilogue to free its buffer would hold up the ring's prefill
-            if (Epi::kSmemBytes > 0 && live && pr == 6 - n_pairs && kb + 1 == min(STAGES, num_kb)) epi.load(m0, n0, es);
+            // not before: waiting for the consumers to release the buffer would hold up the ring
+            if constexpr (Epi::kSmemBytes > 0) {
+              if (pr == 6 - n_pairs) {
+                if (prev_m0 >= 0 && kb + 1 == min(Epi::kLoadKb1, num_kb)) {
+                  epi.load(prev_m0, prev_n0, 1, es);
+                  es.parity ^= 1;
+                  prev_m0 = -1;
+                }
+                if (live && kb + 1 == min(Epi::kLoadKb0, num_kb)) {
+                  epi.load(m0, n0, 0, es);
+                  es.parity ^= 1;
+                }
+              }
+            }
 #endif
           }
         }
-        if (live) es.parity ^= 1;
+        if (live) { prev_m0 = m0; prev_n0 = n0; }
       }
+#ifndef TGB_SKIP_EPI
+      if constexpr (Epi::kSmemBytes > 0) {
+        if (prev_m0 >= 0) epi.load(prev_m0, prev_n0, 1, es);   // the CTA's last tile
+      }
+#endif
+    }
+  } else if constexpr (Epi::kDeferred) {
+    // ===== consumers, deferred epilogue: tile i's accumulators are packed right after its last MMA, and the rest of its
+    // epilogue runs as steps between tile i+1's first k-blocks, so the tensor pipe always has a k-block queued =====
+    setmaxnreg_consumer();
+    const int cw = wg - 1;
+    const int row_in_tile = 64 * cw + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+    float acc[TC_ACC];
+#pragma unroll
+    for (int i = 0; i < TC_ACC; ++i) acc[i] = 0.f;
+    uint32_t dq[TC_ACC / 2];                    // the pending tile's packed values
+    float racc[2] = {0.f, 0.f};                 // its row-dot, carried from step to step
+    int pend_m0 = -1, pend_tn = 0;              // the pending tile (-1: none)
+    uint32_t kbg = 0;
+    // one k-block of the current tile: its MMAs are issued and the previous k-block's stage is released
+    auto kblock = [&](int kb, long long probe_tile) {
+      const int s = kbg % STAGES;
+      const uint32_t ph = (kbg / STAGES) & 1;
+      mbar_wait(&full_bar[s], ph);
+      if (kb == 0) TGB_BWD_PROBE(probe_tile, cw, kBwdProbeFull);
+      const uint32_t sa = smem_u32(smem + s * kStageBytes) + cw * 8192;
+      const uint32_t sb = smem_u32(smem + s * kStageBytes) + TileA::kBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / TC_MMA_K; ++k) {
+        if (kb == 0 && k == 0) wgmma_m64n256k16_first<kTA, kTB>(acc, TileA::desc(sa, k), TileB::desc(sb, k));
+        else wgmma_m64n256k16<kTA, kTB>(acc, TileA::desc(sa, k), TileB::desc(sb, k), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (kb > 0 && lane < 2) mbar_arrive_cluster(&empty_bar[(kbg - 1) % STAGES], lane);
+      ++kbg;
+    };
+    for (int w = cluster_index(); w < total; w += cluster_count()) {
+      const int split = w / (tiles_n * tiles_mp);
+      int tp_i, tile_n;
+      tile_mn(w - split * tiles_n * tiles_mp, tiles_mp, tiles_n, group_m, tp_i, tile_n);
+      const int m0 = (tm_off + 2 * tp_i + cluster_rank()) * TC_BM;
+      const bool live = m0 < (tm_off + tiles_m) * TC_BM;
+      const int k_begin = k_off + split * k_per_split;
+      const int k_end = min(k_total, k_begin + k_per_split);
+      const int total_kb = (k_end - k_begin + TC_BK - 1) / TC_BK * n_pairs;
+      const long long probe_tile = live ? epi.tile_id(m0, tile_n) : -1;
+      (void)probe_tile;
+      float c[2] = {0.f, 0.f};
+      if (live) epi.centres(m0 + row_in_tile, c);
+      acc_fence(acc);
+      // a phantom tile runs its MMAs on a stale A: the stages are released on the same schedule in both CTAs.  Its
+      // k-blocks still carry the previous tile's steps; a tile with fewer k-blocks than steps runs the rest after them.
+      // Every tile has a first k-block (k_total >= 1), whose first MMA overwrites the accumulators: they are dead from
+      // the pack to there, which leaves the registers for the packed values.
+      constexpr int kPrefix = Epi::step_kb(Epi::kSteps - 1) + 1;
+#pragma unroll
+      for (int p = 0; p < kPrefix; ++p) {
+        if (p == 0 || p < total_kb) kblock(p, probe_tile);
+#pragma unroll
+        for (int s = 0; s < Epi::kSteps; ++s)
+          if (Epi::step_kb(s) == p && pend_m0 >= 0) epi.step(s, dq, racc, pend_m0, pend_tn, pend_m0 + row_in_tile, lane, cw, es);
+      }
+      for (int kb = kPrefix; kb < total_kb; ++kb) kblock(kb, probe_tile);
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (live) TGB_BWD_PROBE(probe_tile, cw, kBwdProbeRetired);
+      if (total_kb > 0 && lane < 2) mbar_arrive_cluster(&empty_bar[(kbg - 1) % STAGES], lane);
+#ifndef TGB_SKIP_EPI
+      Epi::pack(acc, c, dq);                    // also for a phantom tile: a conditional pack would keep the old values live
+      pend_m0 = live ? m0 : -1;
+      pend_tn = tile_n;
+#endif
+    }
+    if (pend_m0 >= 0) {                         // the CTA's last tile
+#pragma unroll
+      for (int s = 0; s < Epi::kSteps; ++s) epi.step(s, dq, racc, pend_m0, pend_tn, pend_m0 + row_in_tile, lane, cw, es);
     }
   } else {
     // ===== consumers: wgmma main loop, then the fused epilogue on the accumulator registers =====
@@ -653,7 +862,7 @@ static inline int tc_launch(TcContext& tc, Kern kern, int smem, long long pairs,
 
 // Operand ring of up to 4 stages of 48 KB (128 x 64 A + 256 x 64 B, bf16), as many as fit beside the epilogue's buffer
 // in the 227 KB an H100 block may use (1 KB of it kept for the alignment of the dynamic buffer, 1 KB for the static
-// barriers): 4 stages (193 KB) without an epilogue buffer, 3 (209 KB) beside TcEpiDpStore's 64 KB.
+// barriers): 4 stages (193 KB), also beside TcEpiDpStore's 32 KB (225 KB).
 constexpr int TC_STAGE_BYTES = (TC_BM + TC_BN) * TC_BK * 2;
 constexpr int TC_SMEM_LIMIT = 227 * 1024;
 template <class Epi>

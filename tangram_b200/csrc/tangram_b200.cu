@@ -3078,6 +3078,19 @@ extern "C" TGB200_API int tgb200_debug_overlap_probe(tgb200_mapper* h, int32_t k
 }
 #endif
 
+#ifdef TGB_BWD_PHASE_PROBE
+// Debug build only (tools/bwd_phase_probe.py): every later bf16 backward contraction on the handle's device records its
+// tiles' phase stamps into `buf` (device memory, 16 x 8 bytes per tile; see g_bwd_probe in gemm_tc.cuh), until the
+// next call.  Null stops the recording.
+extern "C" TGB200_API int tgb200_debug_bwd_phase_probe(tgb200_mapper* h, void* buf) {
+  if (!h) return fail(TGB200_ERR_INVALID, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpyToSymbol(g_bwd_probe, &buf, sizeof(buf)));
+  return TGB200_OK;
+}
+#endif
+
 // Spatial neighbour graph (squidpy's gr.spatial_neighbors): exact k-nearest and radius search over a uniform cell grid
 // (see neighbors.cuh for the kernels and the stop bound).
 namespace {
