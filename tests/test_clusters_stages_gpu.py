@@ -156,12 +156,14 @@ class _Blocks:
         self.n += int(live.sum())
 
     def done(self):
+        """assert the accumulated statistics; -> (max err / bound, rel-Fro, bias)"""
         fro = (self.e2 / self.s2) ** 0.5 if self.s2 > 0 else 0.0
         bias = self.bsum / self.n if self.n else 0.0
         print(f"[stage] {self.what}: max err/bound {self.ratio:.3g}, rel-Fro {fro:.3g} (bound {self.c_fro:.3g}), "
               f"bias {bias:.3g} (bound {self.c_bias:.3g})")
         assert fro <= self.c_fro, f"{self.what}: rel-Frobenius {fro:.3g} > {self.c_fro:.3g}"
         assert abs(bias) <= self.c_bias, f"{self.what}: bias {bias:.3g} beyond {self.c_bias:.3g}"
+        return self.ratio, fro, bias
 
 
 def _free():
@@ -199,11 +201,16 @@ def _check_row_pass_tight(r, M, P_dev, stats, mode, p_extra=0.0):
     assert torch.count_nonzero(P_dev[:, V:]) == 0, "pad columns of P"
     if r.lam.get("lambda_r"):
         logP = torch.log_softmax(M[:, :V], dim=1)
-        aP = logP.abs()
-        hb = ((P * (cP * aP + U * dist + U * aP)).sum(dim=1) + c_logz
-              + (4 * per + int(np.log2(threads)) + 1) * U * (P * aP).sum(dim=1))
-        _tight(f"{mode} h", stats[:, 3], (P * logP).sum(dim=1), hb)
+        _tight(f"{mode} h", stats[:, 3], (P * logP).sum(dim=1), _row_pass_h_bound(r, P, logP, cP, dist, c_logz))
     return P
+
+
+def _row_pass_h_bound(r, P, logP, cP, dist, c_logz):
+    """the row pass's h = sum_j P_j log P_j: each term's P and log P error, the row's serial run and block tree"""
+    threads, _, per = row_pass_layout(r.ld)
+    aP = logP.abs()
+    return ((P * (cP * aP + U * dist + U * aP)).sum(dim=1) + c_logz
+            + (4 * per + int(np.log2(threads)) + 1) * U * (P * aP).sum(dim=1))
 
 
 # ----------------------------------------------------------------------------------------------------------------- forward
@@ -360,7 +367,8 @@ def _check_loss_stage_tight(r, Y_dev, dY_dev, hist, M, stats, row_depth, mode):
         for col in sorted(terms):
             got = float(hist[col])
             err = abs(got - terms[col])
-            print(f"[stage] {mode} history column {col}: err {err:.3g}, err/bound {err / bound[col]:.3g} (bound {bound[col]:.3g})")
+            rel = err / bound[col] if bound[col] else 0.0        # a zero bound (no island indicator can flip) wants err 0
+            print(f"[stage] {mode} history column {col}: err {err:.3g}, err/bound {rel:.3g} (bound {bound[col]:.3g})")
             assert err <= bound[col], f"{mode} history column {col}: {got} vs {terms[col]} (bound {bound[col]:.3g})"
 
         # dY_ext, gene columns: each part's coefficients off by (2.5 D + 8) u relative, times the part's magnitude

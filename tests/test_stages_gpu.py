@@ -183,21 +183,27 @@ def _check_row_pass(r, M, P_dev, stats, mode, floor=0.0):
 
 
 # ----------------------------------------------------------------------------------------------------------------- forward
-def _check_forward(r, Y_dev, P, c_elem, c_fro, c_bias, mode, S=None):
+def _check_forward(r, Y_dev, P, c_elem, c_fro, c_bias, mode, S=None, ref=None):
     """Y_ext = P^T S_ext: the gene columns, the density pair (its hi + lo sum in clusters mode) and the cell-type columns,
-    zero past them."""
+    zero past them.  ref: (P^T S_ext, P^T |S_ext|) summed elsewhere (over row blocks of P) in place of P and S.
+    -> {label: _check's (max err / bound, rel-Fro, bias)}"""
     torch = _torch()
     K, T = r.K, r.T
-    S = r.S if S is None else S
-    Yref = P.t() @ S
-    scale = P.t() @ S.abs()
-    _check(f"{mode} Y genes", Y_dev[:, :K], Yref[:, :K], scale[:, :K], c_elem, c_fro, c_bias)
+    if ref is None:
+        S = r.S if S is None else S
+        Yref, scale = P.t() @ S, P.t() @ S.abs()
+    else:
+        Yref, scale = ref
+    out = {}
+    out["Y genes"] = _check(f"{mode} Y genes", Y_dev[:, :K], Yref[:, :K], scale[:, :K], c_elem, c_fro, c_bias)
     dsum = Y_dev[:, K] + Y_dev[:, K + 1]
-    _check(f"{mode} Y density", dsum, Yref[:, K] + Yref[:, K + 1], scale[:, K] + scale[:, K + 1], c_elem, c_fro, c_bias)
+    out["Y density"] = _check(f"{mode} Y density", dsum, Yref[:, K] + Yref[:, K + 1], scale[:, K] + scale[:, K + 1], c_elem,
+                              c_fro, c_bias)
     if T:
-        _check(f"{mode} Y ct", Y_dev[:, K + 2:K + 2 + T], Yref[:, K + 2:K + 2 + T], scale[:, K + 2:K + 2 + T], c_elem, c_fro, c_bias)
+        out["Y ct"] = _check(f"{mode} Y ct", Y_dev[:, K + 2:K + 2 + T], Yref[:, K + 2:K + 2 + T], scale[:, K + 2:K + 2 + T],
+                             c_elem, c_fro, c_bias)
     assert torch.count_nonzero(Y_dev[:, K + 2 + T:]) == 0, "Y_ext past the last used column"
-    return Yref
+    return out
 
 
 # -------------------------------------------------------------------------------------------------------------- loss stage
@@ -662,17 +668,14 @@ def _check_bf16_update_step(r, pre, t, lseT_now, mode, late=False, tiny=False):
     rowc = r.buf("rowc", 4)
     assert torch.equal(rowc[:, 0], lseT_now), "rowc carries the row's exact log-sum-exp"
     Mv = pre[0][:, :V]
-    P = torch.exp(Mv - rowc[:, 0:1])
-    g = _grad_terms(r, Mv, P, dq - rowc[:, 1:2], rowc[:, 0], rowc[:, 2])
-    dg = (UM * (4 + 2 * Mv.abs() + 2 * rowc[:, 0:1].abs()) + 4 * U) * g.abs() + 4 * U * P * (dq.abs() + rowc[:, 1:2].abs())
-    dg = dg + (r.lam.get("lambda_r", 0.0) * P * 8 * U * (Mv.abs() + rowc[:, 0:1].abs() + rowc[:, 2:3].abs()))
+    P, g, dg = _bf16_update_grad(r, Mv, dq, rowc)
     if tiny:
         base = (dq - rowc[:, 1:2]).abs()
         if r.lam.get("lambda_r"):
             base = base + r.lam["lambda_r"] * ((Mv - rowc[:, 0:1]) - rowc[:, 2:3]).abs()
         dg = dg + TINY * base + SUB
     post = _state(r)
-    _check_update_bf16(r, pre, post, g, dg, t + 1, mode, late=late, tiny=tiny)
+    step_stats = _check_update_bf16(r, pre, post, g, dg, t + 1, mode, late=late, tiny=tiny)
     # what the update left for the next forward: P~ = bf16(exp(Mnew - lse)), z~ = sum of the unrounded values
     Mn = post[0][:, :V]
     lseA = r.buf("lseA")
@@ -684,6 +687,24 @@ def _check_bf16_update_step(r, pre, t, lseT_now, mode, late=False, tiny=False):
     assert torch.count_nonzero(Pt[:, V:]) == 0, "pad columns of P~"
     _check(f"{mode} z~", r.buf("zsum"), Pt_ref.sum(dim=1), Pt_ref.sum(dim=1),
            (V + 8) * U + UM * (2 + Mn.abs().max().item() + lseA.abs().max().item()), (V + 8) * U + 4 * UM, (V + 8) * U + 4 * UM)
+    return step_stats
+
+
+def _bf16_update_grad(r, Mv, dq, rowc):
+    """The streaming update's g from the device's dq (N x V) and rowc = (lse, r', h) in float64, and the bound dg of the
+    kernel's fp32 g on it (MUFU ex2 of an fma'd argument, the fp32 products and sums) -> (P, g, dg)"""
+    torch = _torch()
+    P = torch.exp(Mv - rowc[:, 0:1])
+    g = _grad_terms(r, Mv, P, dq - rowc[:, 1:2], rowc[:, 0], rowc[:, 2])
+    dg = (UM * (4 + 2 * Mv.abs() + 2 * rowc[:, 0:1].abs()) + 4 * U) * g.abs() + 4 * U * P * (dq.abs() + rowc[:, 1:2].abs())
+    dg = dg + (r.lam.get("lambda_r", 0.0) * P * 8 * U * (Mv.abs() + rowc[:, 0:1].abs() + rowc[:, 2:3].abs()))
+    return P, g, dg
+
+
+def _bf16_adam64(M0, m0, v0, g, dg, t, tiny=False):
+    """_adam64 with the bf16 update's MUFU rcp / sqrt: 2 UM relative to the step each, 4 UM to v"""
+    Mr, mr, vr, dM, dm, dv = _adam64(M0, m0, v0, g, dg, t, floor=4 * SUB if tiny else 0.0)
+    return Mr, mr, vr, dM + 4 * UM * (M0 - Mr).abs(), dm, dv + 4 * UM * vr
 
 
 def _bf16_forward_consts(r):
@@ -737,9 +758,7 @@ def _check_update_bf16(r, pre, post, g, dg, t, mode, late=False, tiny=False):
     V = r.V
     M0, m0, v0 = (x[:, :V] for x in pre)
     M1, m1, v1 = post
-    Mr, mr, vr, dM, dm, dv = _adam64(M0, m0, v0, g, dg, t, floor=4 * SUB if tiny else 0.0)
-    dM = dM + 4 * UM * (M0 - Mr).abs()
-    dv = dv + 4 * UM * vr
+    Mr, mr, vr, dM, dm, dv = _bf16_adam64(M0, m0, v0, g, dg, t, tiny)
     for what, got, ref, bound in (("v", v1[:, :V], vr, dv), ("M", M1[:, :V], Mr, dM)):
         bad = (got - ref).abs() > bound
         assert not bool(bad.any()), f"{mode} update {what}: {int(bad.sum())} elements off, first {torch.nonzero(bad)[0].tolist()}"
@@ -775,7 +794,7 @@ def _check_update_bf16(r, pre, post, g, dg, t, mode, late=False, tiny=False):
     stepref = M0 - Mr
     scale = stepref.abs() + dM
     c_fro, c_bias = _late_step_consts(M1[:, :V], scale, 8 * UM, 2 * UM, late)
-    _check(f"{mode} update step", M0 - M1[:, :V], stepref, scale, 1e30, c_fro, c_bias)
+    return _check(f"{mode} update step", M0 - M1[:, :V], stepref, scale, 1e30, c_fro, c_bias)
 
 
 def test_bf16_carry_horizon():
