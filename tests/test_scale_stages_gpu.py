@@ -440,13 +440,13 @@ def test_row_blocks_match_full_tensors():
 class _Work:
     """An Engine on a workload's inputs plus the float64 copies the stage checks read (S_ext on the device)"""
 
-    def __init__(self, name, N, V, K, T, inp, lam, graphs=None, state_memory="device", init=None):
+    def __init__(self, name, N, V, K, T, inp, lam, graphs=None, state_memory="device", init=None, precision="bf16"):
         import torch
         from tangram_b200 import _lib
         from tangram_b200.engine import Engine
-        self.name, self.precision, self.N, self.V, self.K, self.T, self.lam = name, "bf16", N, V, K, T, dict(lam)
+        self.name, self.precision, self.N, self.V, self.K, self.T, self.lam = name, precision, N, V, K, T, dict(lam)
         self.clusters, self.graphs, self.inp = False, graphs or {}, inp
-        self.e = Engine(N, V, K, n_types=T, precision="bf16", density_mode=_lib.DENSITY_CELLS, state_memory=state_memory, **lam)
+        self.e = Engine(N, V, K, n_types=T, precision=precision, density_mode=_lib.DENSITY_CELLS, state_memory=state_memory, **lam)
         self.e.set_expression(inp["S"], inp["G"])
         self.e.set_density(inp["d"])
         for which, g in self.graphs.items():
@@ -594,7 +594,7 @@ BIG_SEED = 42
 CROSS = (213_700, 213_760)      # element 2^31 of an ld = 10048 operand is in row 213,722, byte 2^32 of a bf16 one too
 
 
-def _big_work(state_memory="device"):
+def _big_work(state_memory="device", precision="bf16"):
     from oracle.tangram_oracle import synthetic_inputs
     N, V, K = BIG
     if "big" not in _INPUTS:
@@ -603,7 +603,7 @@ def _big_work(state_memory="device"):
 
     def init(e):
         e.init_mapping_legacy(np.random.RandomState(BIG_SEED).get_state())
-    return _Work("big", N, V, K, 0, _INPUTS["big"], {}, state_memory=state_memory, init=init)
+    return _Work("big", N, V, K, 0, _INPUTS["big"], {}, state_memory=state_memory, init=init, precision=precision)
 
 
 def _big_windows(r):
